@@ -1,6 +1,6 @@
-"""bench.py -- tokens/s of the packed 2-bit Llama-2-7B eval path on N B200s (driver contract).
+"""bench.py -- tokens/s of the packed 2-bit Llama-2-7B eval path on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     ... bench.py --model llama70b|opt30b|opt1.3b [--parallelism pp]     the other BASELINE.json configs (not the headline)
 
@@ -15,7 +15,7 @@ linears each -> final norm -> lm_head -> CE loss), i.e. one pass of llama_eval's
           path's only collective, one all-reduce of the summed NLL, is inside the timed region.
   e2e     the same metric through the public API quip_b200.llama.llama_eval with HOST token ids: every step
           copies its ids from pinned host memory and reads the scalar result back.
-  roofline  the dominant kernel (tcgen05 packed GEMM): algorithmic flops of its launches / their summed
+  roofline  the dominant kernel (wgmma packed GEMM): algorithmic flops of its launches / their summed
           device time, measured with CUDA events around every launch inside the timed region.
   config.glue  which glue ran between the packed linears (HF torch launches or the fused kernels of csrc/glue.cu), chosen
           in the run by `pick_glue`: every fused op against the HF module it replaces (bit-exact except the norm's summation
@@ -32,6 +32,8 @@ linears each -> final norm -> lm_head -> CE loss), i.e. one pass of llama_eval's
   cpu_baseline / --impl reference: the reference's effective path (HF decoder layer with dense fp16
           weights, the per-layer loop of llama.py:174-253 ported in oracle/evalloop.py) on the host cores,
           on a bounded sample (1 decoder layer x 1 sample), extrapolated to 32 layers.
+  --dump-outputs DIR  after the timed steps, rank 0 writes what the last timed step returned (its NLL, float64) to
+          DIR/last_step_nll.npy.  Inputs are seeded, so two builds run with the same arguments can be compared.
 """
 import argparse
 import ctypes as C
@@ -57,11 +59,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d['hbm_gbs'], tflops_burst=d['bf16_tflops'], tflops_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0,
+                source='H100 SXM data sheet (700 W, dense bf16): not a measured figure')
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe: -lms 200).  The process is
+    """nvidia-smi clocks / throttle reasons during the timed region (sampled every 200 ms).  The process is
     started BEFORE the warm-up steps -- nvidia-smi's own start-up (NVML init under the driver lock) slowed the first
     timed steps by ~25 % whenever it coincided with them -- and only the rows that arrive between mark_start() and
     mark_end() are summarised."""
@@ -680,6 +683,8 @@ def main():
                          "the factor bytes drop from n(p1+p2) to p1^2+p2^2 per side (not the headline configuration)")
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-decode', action='store_true', help='skip the one-token decode legs (quick runs)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step returned to DIR/<name>.npy (float64)')
     a = ap.parse_args()
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -818,7 +823,8 @@ def main():
         e0.record()
         nll = torch.zeros((), device=dev)
         for i in range(a.warmup, total):
-            nll += step_fn(ids_dev[i])
+            last = step_fn(ids_dev[i])
+            nll += last
         if world > 1:
             dist.all_reduce(nll)
         e1.record()
@@ -827,6 +833,7 @@ def main():
         if profiling:
             torch.cuda.profiler.stop()
     with torch.no_grad():
+        last_nll = last.detach().double().cpu().reshape(1)   # before any other pass can reuse the step's buffers
         ms = max_over_ranks(e0.elapsed_time(e1))
         launches = lib.quip_launch_count() - launches0       # eager launches; a replayed graph is counted below
 
@@ -875,29 +882,26 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
+    if a.dump_outputs:
+        import numpy as np
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        np.save(os.path.join(a.dump_outputs, 'last_step_nll.npy'), last_nll.numpy())
 
     pk = peaks()
     value = world * a.steps * SEQ / (ms / 1e3)
     e2e_value = world * a.steps * SEQ / (e2e_ms / 1e3)
     achieved = tfl.value / (tms.value / 1e3) / 1e12 if tms.value > 0 else None
-    traffic, traffic_note = None, None
-    prof = os.path.join(ROOT, 'profiles', 'ncu_qgemm_tc_latest.json')
-    if os.path.exists(prof):
-        pj = json.load(open(prof))
-        traffic = pj.get('dram_bytes_per_launch')
-        traffic_note = ('dram__bytes_read+write of one ncu --set full capture, %s: algorithmic %.1f MB (the activations '
-                        'stay largely L2-resident between the kernels of one linear)' % (pj.get('shape'), pj.get('algorithmic_bytes', 0) / 1e6))
     out = dict(base, value=value, ms_per_step=ms / a.steps, dtype='f16', impl='ours', gpu_launches=int(launches),
                e2e=dict(value=e2e_value, unit='tokens/s', h2d_bytes_per_step=SEQ * 8, d2h_bytes_per_step=4,
                         api='quip_b200.llama.llama_eval' if family == 'llama' else 'quip_b200.opt.opt_eval'),
-               roofline=dict(bound='tensor', kernel='qgemm_tc_kernel<2,256> (tcgen05 packed GEMM)', achieved=achieved,
+               roofline=dict(bound='tensor', kernel='qgemm_tc_kernel<2,128> (wgmma packed GEMM)', achieved=achieved,
                              peak=pk['tflops_sustained'], unit='TFLOP/s', frac=(achieved / pk['tflops_sustained']) if achieved else None,
-                             traffic=traffic, traffic_note=traffic_note, launches_timed=int(tn.value), kernel_ms_per_step=tms.value / a.steps,
+                             launches_timed=int(tn.value), kernel_ms_per_step=tms.value / a.steps,
                              share_of_step=tms.value / ms, share_of_serial_replay=tms.value / serial_ms,
                              measured_in=('serial replay of the same K steps with CUDA events around every launch '
                                           '(sibling-stream overlap off, eager launches: %.2f ms/step, host gaps included); '
                                           'share_of_step = its summed launch time / the timed step (one graph replay, overlap '
-                                          'on); the ncu launch list of the same command: profiles/launches_r02.json' % (serial_ms / a.steps)), peak_source=pk['source'] + ', sustained bf16 (kernel timed inside a long step)'),
+                                          'on)' % (serial_ms / a.steps)), peak_source=pk['source'] + ', sustained bf16 (kernel timed inside a long step)'),
                selfcheck=check, clocks=clk.summary())
     if world == 1 and not a.no_decode and a.model == 'llama7b':
         try:

@@ -1,5 +1,5 @@
 /*
- * quip_b200 -- C ABI of the B200-native packed QuantLinear path.
+ * quip_b200 -- C ABI of the H100-native packed QuantLinear path.
  *
  * This is the boundary the reference's FFI for this path would bind.  The
  * reference (Cornell-RelaxML/QuIP) has exactly one native call site on the
@@ -22,7 +22,7 @@
  * no internal allocation -- scratch comes from the caller-provided workspace.
  * Every function returns 0 on success and a non-zero code on error, with a
  * human-readable message available from quip_last_error() (thread-local).
- * There is no CPU fallback: on a machine without an sm_100 device the launch
+ * There is no CPU fallback: on a machine without an sm_90 device the launch
  * entry points return QUIP_ERR_CUDA.
  */
 #ifndef QUIP_B200_H_
@@ -103,7 +103,7 @@ int quip_qlinear_workspace_bytes(const QuipLinearDesc* d, int64_t M, size_t* out
 /* Building blocks (also exported for tests and micro-benchmarks). */
 /* z (M,N) fp16 = x2 (M,K) fp16 contracted with the packed matrix + affine epilogue (+bias if given).
  * xsum (M) fp32 row sums of x2, required unless QUIP_FLAG_SYMMETRIC.  path: 0 auto, 1 few-token kernels (32-token
- * chunks; needs the workspace), 2 tcgen05 kernel. */
+ * chunks; needs the workspace), 2 wgmma kernel. */
 int quip_qgemm(const QuipLinearDesc* d, const void* x2, const float* xsum, const void* bias,
                void* z, int64_t M, int path, void* workspace, size_t workspace_bytes, void* stream);
 int quip_rowsum(const void* x, float* xsum, int64_t M, int32_t K, void* stream);
@@ -177,7 +177,7 @@ int quip_greedy_block(const float* preT, const float* Hb, float* wrT, float* sT,
 int quip_hessian_accumulate(const void* x, double* H, int64_t tokens, int32_t K, void* stream);
 
 /* Optional per-launch timing of the contraction kernels with CUDA events recorded on the launch stream
- * (bench.py's roofline leg).  path: 1 = mma.sync skinny kernel, 2 = tcgen05 kernel.  quip_timing_read
+ * (bench.py's roofline leg).  path: 1 = mma.sync skinny kernel, 2 = wgmma kernel.  quip_timing_read
  * waits for the recorded events and returns the totals since the last reset: device milliseconds,
  * launches, algorithmic flops (2*M*N*K) and algorithmic bytes (packed codes + fp16 activations in + out). */
 int quip_timing_enable(int on);

@@ -7,7 +7,7 @@ This package restates, in numpy / CPU torch, the algorithm of the reference's
                 (reference quant.py:6-21, 57-163; vector_balance.py:499-532)
   packing.py    reference 3-/4-bit packed layouts (quant.py:185-220,
                 zeroShot/models/quant.py:185-199), the natural 2-bit extension,
-                and the native fragment-major layout the sm_100a kernels read
+                and the native fragment-major layout the sm_90a kernels read
   butterfly.py  structured orthogonal multiply (method.py:16-78)
   forward.py    W_ref reconstruction (method.py:195-214) and the factored
                 forward  y = ((x / s) V^T) Q^T U + b

@@ -3,7 +3,7 @@
 Run:  python -m oracle.gen_golden_big [--method ldlq|nearest] [--n 4096 --k 4096]
 
 The small golden layers (oracle/gen_golden.py) never exceed K = 640, so every GPU parity case built on them keeps the
-tcgen05 kernel on one tile per CTA.  This fixture is a whole q_proj-sized Linear through the reference's own flow
+tensor-core kernel on one tile per CTA.  This fixture is a whole q_proj-sized Linear through the reference's own flow
 (`Balance.preproc` with --pre_gptqH --pre_rescale --pre_proj, method.py:139-193; `fasterquant`, bal.py:21-48;
 `postproc`, method.py:195-214), so that the multi-tile persistent path, the 64 x 64 butterflies and the one-kernel
 sides are checked against the reference's own dense fp16 output `F.linear(x, W_ref)`.

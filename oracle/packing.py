@@ -10,7 +10,7 @@ Reference layouts (what a reference-quantized checkpoint would hold):
   * 2-bit: not defined by the reference; the natural extension (16 codes per
     word, code i at bits 2*(i%16) of row i//16) is provided for completeness.
 
-Native layout (what the sm_100a kernels read; documented in DESIGN.md):
+Native layout (what the sm_90a kernels read; documented in DESIGN.md):
   The (N, K) code matrix is cut into super-blocks of 16 rows x 128 k, stored
   [row_block][k_superblock].  Inside a super-block the data are laid out per
   *lane* l = 4*g + t of a warp, lane l owning rows {g, g+8} and, in each of the
@@ -32,7 +32,7 @@ Native layout (what the sm_100a kernels read; documented in DESIGN.md):
               8*(ch%2)+j at bits jj and 16+jj.
   This is exactly the A-fragment ownership of mma.sync.m16n8k16 (rows g/g+8,
   k-pairs) with k re-labelled so a lane's 8 k's are contiguous, which also makes
-  them one 16-byte chunk of a 128B-swizzled K-major tcgen05 operand row.
+  them one 16-byte chunk of a 128B-swizzled K-major wgmma operand row.
 
 Test infrastructure only (see oracle/__init__.py).
 """

@@ -117,7 +117,7 @@ def affine_qfnb(scale, bits, n_rows):
 
 
 def kernel_affine(scales, zeros, bits):
-    """The two per-row coefficients the sm_100a kernels apply in their epilogue.
+    """The two per-row coefficients the sm_90a kernels apply in their epilogue.
 
     The kernels contract x against d = (code - cbar) / 2^bits with
     cbar = (2^bits - 1)/2 (exactly representable in fp16 for bits in {2,3,4}),

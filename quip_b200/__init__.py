@@ -1,7 +1,7 @@
-"""quip_b200: B200-native packed QuantLinear path for QuIP-quantized OPT / Llama models.
+"""quip_b200: H100-native packed QuantLinear path for QuIP-quantized OPT / Llama models.
 
 Host code is Python/PyTorch mirroring the reference's quant.py / opt.py / llama.py surface; the
-compute runs in hand-written sm_100a kernels behind a C ABI (include/quip_b200.h,
+compute runs in hand-written sm_90a kernels behind a C ABI (include/quip_b200.h,
 quip_b200/libquip_b200.so).  Importing the package does not load the library; the first packed
 forward (or `quip_b200._lib.load()`) does, and fails loudly if it is missing.
 """

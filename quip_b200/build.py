@@ -1,4 +1,4 @@
-"""Build libquip_b200.so (all CUDA kernels + the C ABI) in-tree for sm_100a.
+"""Build libquip_b200.so (all CUDA kernels + the C ABI) in-tree for sm_90a (H100).
 
     python -m quip_b200.build [--force] [--verbose]
 
@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, 'build')
 LIB = os.path.join(HERE, 'libquip_b200.so')
 SOURCES = ['api.cu', 'pack.cu', 'rot.cu', 'rot_small.cu', 'rot_fewtok.cu', 'rot_side.cu', 'rot_side_fewtok.cu', 'glue.cu', 'vecquant.cu', 'ldlq.cu', 'hessian.cu', 'qgemm_skinny.cu', 'qgemv.cu', 'qgemm_tc.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -29,6 +29,11 @@ def _stale(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
+    # objects compiled with other flags (another architecture) are stale whatever their timestamps
+    stamp = os.path.join(OBJ, 'flags.txt')
+    flags = ' '.join([NVCC] + FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
     headers = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'), os.path.join(os.path.dirname(HERE), 'include', 'quip_b200.h')]
     jobs = []
     for src in SOURCES:
@@ -51,11 +56,13 @@ def build(force=False, verbose=False):
                 raise RuntimeError(f'nvcc failed on {src}')
     objs = [os.path.join(OBJ, s.replace('.cu', '.o')) for s in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError('link failed')
+    with open(stamp, 'w') as f:
+        f.write(flags)
     return LIB
 
 

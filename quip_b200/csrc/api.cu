@@ -252,7 +252,7 @@ extern "C" int quip_qgemm(const QuipLinearDesc* d, const void* x2, const float* 
   if (int e = check_desc(d)) return e;
   QUIP_CHECK_ARG(x2 && z && M > 0 && M < (1ll << 31), "bad arguments");
   WsPlan p = plan_ws(d, M);
-  QUIP_CHECK_ARG(path >= 0 && path <= 2, "path must be 0 (auto), 1 (few-token kernels) or 2 (tcgen05)");
+  QUIP_CHECK_ARG(path >= 0 && path <= 2, "path must be 0 (auto), 1 (few-token kernels) or 2 (tensor-core GEMM)");
   // the few-token kernels keep split-K partials + arrival counters in the workspace (path 1 loops 32-token chunks for any M)
   if (path == 1 || (path == 0 && M <= SKINNY_MAX_M)) {
     if (!workspace || workspace_bytes < p.total) {

@@ -1,4 +1,4 @@
-// Shared helpers for the quip_b200 sm_100a kernels.
+// Shared helpers for the quip_b200 sm_90a kernels.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -130,7 +130,7 @@ __device__ __forceinline__ uint32_t dq3(uint32_t whi, uint32_t wlo) {
 //   * IMMA.16832 (qgemv.cu, 1-5 tokens): the four A registers are  w & 0x03030303, w & 0x0C0C0C0C,
 //     (w>>4) & 0x03030303, (w>>4) & 0x0C0C0C0C  -- byte j of the word holds "slot" j (bits 0-1 row g,
 //     2-3 row g+8) and slot 4+j (bits 4-5, 6-7);
-//   * HMMA.16816 / tcgen05 (fp16): a register is a pair of codes of one row at the same offset of the low
+//   * HMMA.16816 / wgmma (fp16): a register is a pair of codes of one row at the same offset of the low
 //     and high half-word -- slots (j, j+2) -- so slot s stands for k offset {0,2,1,3,4,6,5,7}[s] and every
 //     fp16x2 register holds two consecutive k.
 // In half-word terms: pair (u = pos/2, row half r) sits at bit 2*slot2(u,r) of each half.  4-bit: word

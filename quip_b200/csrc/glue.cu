@@ -1,8 +1,7 @@
 // Glue kernels of the per-layer eval step: the elementwise work BETWEEN the packed linears of a Llama decoder layer
 // (RMSNorm, residual add, rotary embedding, SiLU gate), each one HBM pass instead of the 5-8 torch launches the HF
-// modules issue.  ncu launch list of the eval step (profiles/launches_r01.json): those torch launches are 27 % of the
-// step (RMSNorm 8 launches ~105 us, rotary 9 launches ~260 us, silu*up 2 launches ~40 us per decoder layer at 2048
-// tokens); the kernels below move the same bytes once: ~34 MB / 67 MB / 135 MB per call, i.e. 5-20 us at HBM speed.
+// modules issue (RMSNorm 8 launches, rotary 9, silu*up 2 per decoder layer); the kernels below move the same bytes
+// once: ~34 MB / 67 MB / 135 MB per call at 2048 tokens.
 //
 // Rounding points follow the HF modules exactly (transformers modeling_llama: LlamaRMSNorm.forward,
 // apply_rotary_pos_emb / rotate_half, LlamaMLP.forward with SiLU), so a layer built on these kernels differs from the
@@ -188,7 +187,7 @@ int stream_grid(int64_t items, int threads) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   const int64_t want = (items + threads - 1) / threads;
   const int64_t cap = (int64_t)sms * 8;                 // 8 CTAs of 256 threads per SM: one full wave, grid-stride beyond

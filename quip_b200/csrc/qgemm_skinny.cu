@@ -251,8 +251,8 @@ static int launch_skinny(const QuipLinearDesc* d, const __half* x, const __half*
 }
 
 // Heuristic split.  Every K split costs a round trip of fp32 partials (write, fence, counter, the last CTA reads them all), and
-// that -- not the staging of the activations -- is what the kernel waits for at 9..32 tokens: on 4096 x 4096 with 32 tokens
-// 8 splits take 36.6 us, 2 splits 17.0 us; with 16 tokens 15.7 against 10.3-10.8 us (profiles/mb_skinny_r02.json).  So: just
+// that -- not the staging of the activations -- is what the kernel waits for at 9..32 tokens, so many splits are slower
+// than few on 4096 x 4096.  So: just
 // enough splits for about one CTA per SM, K slices of at least 512, and as many more as the staged activations of M tokens
 // need to fit shared memory (K = 28672 with 32 tokens: 16 slices).
 int skinny_pick_ksplit(int N, int K, int rows_per_cta, int M) {

@@ -1,39 +1,46 @@
-// Packed-integer x fp16 GEMM on the 5th-generation tensor cores (tcgen05 + TMEM), for many tokens
+// Packed-integer x fp16 GEMM on the Hopper tensor cores (wgmma + TMA), for many tokens
 // (the reference's eval loop calls every Linear with M = 2048: opt.py:262-264, llama.py:226-227).
 //
-//   D[n][m] (TMEM, fp32) = sum_k A[n][k] * B[m][k]
+//   D[n][m] (registers, fp32) = sum_k A[n][k] * B[m][k]
 //     A = packed weights, 128 output rows per tile, expanded to fp16 d=(c-cbar)/2^bits by the
 //         producer warps and written straight into the 128B-swizzled K-major operand layout
 //         (generic-proxy st.shared + fence.proxy.async), never touching HBM as fp16;
 //     B = activations x2 (M,K) fp16, BN tokens per tile, staged by TMA (cp.async.bulk.tensor, 128B
 //         swizzle, out-of-bounds rows zero-filled so ragged M needs no special case);
-//   epilogue: z[m][n] = P_n * D + R_n * xsum[m] (+ bias_n) -> fp16, straight from tcgen05.ld registers.
+//   epilogue: z[m][n] = P_n * D + R_n * xsum[m] (+ bias_n) -> fp16, transposed through shared memory so
+//   that every store is 16 contiguous bytes of one token row.
 //
-// Warp roles (448 threads, one persistent CTA per SM, static tile schedule):
-//   warp 0      TMA producer            warp 1      TMEM alloc + MMA issuer (one lane)
-//   warps 2-5   epilogue (TMEM lane quarter = warp % 4)
-//   warps 6-13  weight producers (2 groups of 4 alternating k super-blocks): 128-bit loads of packed
+// Warp roles (544 threads, one persistent CTA per SM, static tile schedule):
+//   warps 0-7   two consumer warpgroups: warpgroup w issues wgmma.m64nBNk16 for rows 64w..64w+63 of the
+//               tile, then runs the epilogue of those rows
+//   warps 8-15  weight producers (2 groups of 4 alternating k super-blocks): 128-bit loads of packed
 //               words -> registers -> fp16 -> smem
-// Pipelines: smem ring full[s]/empty[s] (TMA + 4 producer warps -> MMA -> tcgen05.commit), and a
-// double-buffered TMEM accumulator tmem_full[a]/tmem_empty[a] (MMA -> epilogue).
+//   warp 16     TMA producer
+// Pipeline: smem ring full[s]/empty[s] (TMA + 4 producer warps -> 8 consumer warps).  The producers keep
+// filling the ring while the consumers run a tile's epilogue.
 #include "tc_common.cuh"
 
 namespace quip {
+
+constexpr int TC_SMEM_MAX = 227 * 1024;                      // opt-in dynamic shared memory per block
 
 template <int BN>
 struct TcCfg {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;            // 16 KB
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES;    // 256 -> 4, 128 -> 6
-  static constexpr int TMEM_COLS = 2 * BN;                     // double-buffered accumulator
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 8192 /*epilogue*/;
+  // epilogue transpose buffer of one consumer warpgroup: BN token rows x 64 n (packed) or 64 token rows x BN
+  // columns (dense), rows padded by 16 bytes against bank conflicts
+  static constexpr int EPI_HALVES = BN * 72 > 64 * (BN + 8) ? BN * 72 : 64 * (BN + 8);
+  static constexpr int EPI_BYTES = 2 * EPI_HALVES * 2;
+  static constexpr int STAGES = (TC_SMEM_MAX - EPI_BYTES - 1024 - 256) / STAGE_BYTES;   // 128 -> 5, 64 -> 8
+  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + EPI_BYTES;
 };
 
 // DENSE = false: A is the packed matrix (N rows, K columns), expanded by the producer warps.
-// DENSE = true : block-diagonal pass with big blocks -- `nblk` independent GEMMs out_b = in_b . F_b^T, A = fp16
-//                factor F_b (N = K = p) fetched by TMA (3-D map, rows/cols beyond p zero-filled), B = the
-//                block's p contiguous activation columns, output written to the same columns.
+// DENSE = true : block-diagonal pass with big blocks -- `nblk` independent GEMMs out_b = in_b . F_b^T, A = the
+//                block's p contiguous activation columns (128 tokens per tile), B = fp16 factor F_b (N = K = p)
+//                fetched by TMA (3-D map, rows/cols beyond p zero-filled), output written to the same columns.
 template <int BITS, int BN, bool DENSE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_a,
@@ -47,14 +54,11 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_gen + (size_t)C::STAGES * C::STAGE_BYTES);
   uint64_t* full = bars;                       // [STAGES]
   uint64_t* empty = bars + C::STAGES;          // [STAGES]
-  uint64_t* tmem_full = empty + C::STAGES;     // [2]
-  uint64_t* tmem_empty = tmem_full + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  __half* epi_stage = reinterpret_cast<__half*>(smem_gen + (size_t)C::STAGES * C::STAGE_BYTES + 256);   // 4 x 2 KB
+  __half* epi = reinterpret_cast<__half*>(smem_gen + (size_t)C::STAGES * C::STAGE_BYTES + 256);   // 2 x EPI_HALVES
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // packed GEMM: 128 output rows (MMA M) x BN tokens (MMA N).  DENSE pass: 128 TOKENS (MMA M) x BN factor rows
-  // (MMA N), so every epilogue thread owns one token row and stores 64 contiguous bytes per 32 columns.
+  // packed GEMM: 128 output rows (wgmma M) x BN tokens (wgmma N).  DENSE pass: 128 TOKENS (wgmma M) x BN factor
+  // rows (wgmma N).
   const int tiles_n = DENSE ? (N + BN - 1) / BN : (N + TC_BM - 1) / TC_BM;
   const int tiles_m = DENSE ? (M + TC_BM - 1) / TC_BM : (M + BN - 1) / BN;
   const int per_blk = tiles_n * tiles_m;
@@ -62,32 +66,20 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   const int KB = (K + TC_BK - 1) / TC_BK;
   const int KSB = K >> 7;
   const int64_t ldz = (int64_t)N * nblk;       // output row pitch (== N for the packed GEMM)
+  constexpr int TMA_WARP = TC_CONSUMER_WARPS + 4 * TC_PROD_GROUPS;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TMA_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
     if (DENSE) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full[s], DENSE ? 1 : 1 + 4);  // TMA producer (+ 4 weight-producer warps)
-      mbar_init(&empty[s], 1);                 // one tcgen05.commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 4);            // 4 epilogue warps
+      mbar_init(&empty[s], TC_CONSUMER_WARPS); // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)C::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == TMA_WARP) {
     // ================= TMA producer: activation tiles =================
     if (lane == 0) {
       int s = 0;
@@ -109,126 +101,100 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
+  } else if (warp < TC_CONSUMER_WARPS) {
+    // ================= consumers: wgmma over the ring, then the epilogue of 64 rows =================
+    const int wg = warp >> 2, wtid = threadIdx.x & 127;
+    const int frow = (warp & 3) * 16 + (lane >> 2);        // accumulator row of d[j] for (j & 2) == 0; +8 otherwise
+    const int fcol = (lane & 3) * 2;                       // accumulator column of d[j] is 8 * (j >> 2) + fcol + (j & 1)
+    __half* eb = epi + wg * C::EPI_HALVES;
+    float acc[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     int s = 0;
     uint32_t ph = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aph = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(&tmem_empty[as], aph ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int blk = tile / per_blk, rr = tile % per_blk;
+      int prev = 0;
       for (int kb = 0; kb < KB; ++kb) {
         mbar_wait(&full[s], ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_addr = smem_base + (uint32_t)(s * C::STAGE_BYTES);
-          const uint64_t adesc = make_sw128_desc(a_addr);
-          const uint64_t bdesc = make_sw128_desc(a_addr + C::A_BYTES);
+        const uint32_t a_addr = smem_base + (uint32_t)(s * C::STAGE_BYTES);
+        const uint64_t adesc = make_sw128_desc(a_addr + (uint32_t)(wg * 64 * 128));
+        const uint64_t bdesc = make_sw128_desc(a_addr + C::A_BYTES);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)     // +32 bytes along K inside the swizzle atom = +2 encoded
-            umma_f16_ss(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-          umma_commit(&empty[s]);                  // frees the stage once these MMAs have read it
-          if (kb == KB - 1) umma_commit(&tmem_full[as]);
+        for (int k = 0; k < TC_BK / 16; ++k)     // +32 bytes along K inside the swizzle atom = +2 encoded
+          wgmma_f16_ss<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous stage's wgmma have read their operands
+        if (kb > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev]);
         }
-        __syncwarp();
+        prev = s;
         if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
-    }
-  } else if (warp < 6) {
-    // ================= epilogue: TMEM -> registers -> z =================
-    const int quarter = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aph = (uint32_t)(it >> 1) & 1u;
-      const int blk = tile / per_blk, rr = tile % per_blk;
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * BN);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
       if constexpr (DENSE) {
-        const int m = (rr / tiles_n) * TC_BM + quarter * 32 + lane;          // this thread's token
-        const int i0 = (rr % tiles_n) * BN;                                  // first factor row of the tile
-        __half* zrow = z + (int64_t)m * ldz + (int64_t)blk * N;
-        mbar_wait(&tmem_full[as], aph);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(taddr + (uint32_t)c0, r);
-          tmem_ld_wait();
-          const int i = i0 + c0;
-          if (m < M && i < N) {
-            if (i + 32 <= N) {
+        // eb[token row r][column c], pitch BN + 8
+        constexpr int EP = BN + 8;
 #pragma unroll
-              for (int v4 = 0; v4 < 4; ++v4) {
-                uint4 o;
-                uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-                for (int h = 0; h < 4; ++h) {
-                  __half2 hv = __floats2half2_rn(__uint_as_float(r[8 * v4 + 2 * h]), __uint_as_float(r[8 * v4 + 2 * h + 1]));
-                  ow[h] = *reinterpret_cast<uint32_t*>(&hv);
-                }
-                *reinterpret_cast<uint4*>(zrow + i + 8 * v4) = o;
-              }
-            } else {
-#pragma unroll
-              for (int c = 0; c < 32; ++c)
-                if (i + c < N) zrow[i + c] = __float2half_rn(__uint_as_float(r[c]));
-            }
-          }
+        for (int j = 0; j < BN / 2; j += 2) {
+          const int r = frow + ((j & 2) ? 8 : 0), c = 8 * (j >> 2) + fcol;
+          *reinterpret_cast<__half2*>(&eb[r * EP + c]) = __floats2half2_rn(acc[j], acc[j + 1]);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        const int m_base = (rr / tiles_n) * TC_BM + wg * 64, i0 = (rr % tiles_n) * BN;
+        for (int idx = wtid; idx < 64 * (BN / 8); idx += 128) {
+          const int r = idx / (BN / 8), v = idx % (BN / 8);
+          const int m = m_base + r, i = i0 + 8 * v;
+          if (m < M && i < N)
+            *reinterpret_cast<uint4*>(z + (int64_t)m * ldz + (int64_t)blk * N + i) =
+                *reinterpret_cast<const uint4*>(&eb[r * EP + 8 * v]);
         }
       } else {
-        const int n = (rr % tiles_n) * TC_BM + quarter * 32 + lane;
-        const int m0 = (rr / tiles_n) * BN;
-        float Pn = 1.f, Rn = 0.f, bn = 0.f;
-        if (n < N) {
-          float sc = scales[n];
-          Pn = sc * (float)(1 << BITS);
-          if (!symmetric) Rn = sc * (0.5f * (float)((1 << BITS) - 1)) - zeros[n];
-          if (bias) bn = __half2float(bias[n]);
-        }
-        __half* stage = epi_stage + (warp - 2) * EPI_STAGE_HALVES;
-        const int n_warp = (rr % tiles_n) * TC_BM + quarter * 32;
-        mbar_wait(&tmem_full[as], aph);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(taddr + (uint32_t)c0, r);
-          tmem_ld_wait();
-          float v[32];
+        // eb[token c][row r], pitch 72
+        constexpr int EP = 72;
+        const int n_base = (rr % tiles_n) * TC_BM + wg * 64, m0 = (rr / tiles_n) * BN;
+        float Pn[2], Rn[2], bn[2];
 #pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            v[c] = Pn * __uint_as_float(r[c]) + bn;
-            if (!symmetric) {
-              const int m = m0 + c0 + c;
-              v[c] += Rn * (m < M ? __ldg(&xsum[m]) : 0.f);
-            }
+        for (int h = 0; h < 2; ++h) {
+          const int n = n_base + frow + 8 * h;
+          Pn[h] = 1.f; Rn[h] = 0.f; bn[h] = 0.f;
+          if (n < N) {
+            const float sc = scales[n];
+            Pn[h] = sc * (float)(1 << BITS);
+            if (!symmetric) Rn[h] = sc * (0.5f * (float)((1 << BITS) - 1)) - zeros[n];
+            if (bias) bn[h] = __half2float(bias[n]);
           }
-          epilogue_store_chunk(stage, v, z, ldz, m0 + c0, M, n_warp, N, lane);
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) {
+          const int h = (j >> 1) & 1, c = 8 * (j >> 2) + fcol + (j & 1), m = m0 + c;
+          float v = Pn[h] * acc[j] + bn[h];
+          if (!symmetric) v += Rn[h] * (m < M ? __ldg(&xsum[m]) : 0.f);
+          eb[c * EP + frow + 8 * h] = __float2half_rn(v);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        for (int idx = wtid; idx < BN * 8; idx += 128) {
+          const int c = idx >> 3, v = idx & 7;
+          const int m = m0 + c, n = n_base + 8 * v;
+          if (m < M && n < N)
+            *reinterpret_cast<uint4*>(z + (int64_t)m * ldz + n) = *reinterpret_cast<const uint4*>(&eb[c * EP + 8 * v]);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // eb is free for the next tile
     }
   } else if (!DENSE) {
     // ================= weight producers: packed words -> fp16 operand tile =================
-    const int pw = (warp - 6) & 3, grp = (warp - 6) >> 2;
+    const int pw = (warp - TC_CONSUMER_WARPS) & 3, grp = (warp - TC_CONSUMER_WARPS) >> 2;
     weight_producer_loop<BITS, C::STAGES, C::STAGE_BYTES>(
         pw, grp, lane, q, KSB, N, empty, smem_base, (int)blockIdx.x, (int)gridDim.x, num_tiles,
         [&](int tile) { return ((tile % per_blk) % tiles_n) * (TC_BM / 16); },
         [&](int s) { mbar_arrive(&full[s]); });
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS)
-                 : "memory");
   }
 }
 
@@ -256,7 +222,7 @@ int num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      g_num_sms = 148;
+      g_num_sms = 132;
   }
   return g_num_sms;
 }
@@ -329,21 +295,21 @@ static int launch_tc_dense(const QuipPass* ps, const __half* in, __half* out, in
 }
 
 int pass_big_tc(const QuipPass* ps, const __half* in, __half* out, int64_t M, int n, cudaStream_t s) {
-  QUIP_CHECK_ARG(!ps->strided && ps->p % 8 == 0 && n % 8 == 0, "tcgen05 pass needs contiguous blocks, p %% 8 == 0");
-  QUIP_CHECK_ARG((((uintptr_t)in | (uintptr_t)out | (uintptr_t)ps->factors) & 15) == 0, "tcgen05 pass: unaligned pointer");
-  return ps->p > 128 ? launch_tc_dense<256>(ps, in, out, (int)M, n, s) : launch_tc_dense<128>(ps, in, out, (int)M, n, s);
+  QUIP_CHECK_ARG(!ps->strided && ps->p % 8 == 0 && n % 8 == 0, "tensor-core pass needs contiguous blocks, p %% 8 == 0");
+  QUIP_CHECK_ARG((((uintptr_t)in | (uintptr_t)out | (uintptr_t)ps->factors) & 15) == 0, "tensor-core pass: unaligned pointer");
+  return launch_tc_dense<128>(ps, in, out, (int)M, n, s);
 }
 
 int qgemm_tc(const QuipLinearDesc* d, const __half* x, const float* xsum, const __half* bias, __half* z, int M,
              cudaStream_t s) {
-  QUIP_CHECK_ARG(((uintptr_t)x & 15) == 0, "tcgen05 path needs 16-byte aligned activations");
-  const bool wide = M > 128;
+  QUIP_CHECK_ARG(((uintptr_t)x & 15) == 0, "tensor-core path needs 16-byte aligned activations");
+  const bool wide = M > 64;
 #define QUIP_TC(B)                                                            \
   if (d->bits == B)                                                           \
-    return wide ? launch_tc<B, 256>(d, x, xsum, bias, z, M, s) : launch_tc<B, 128>(d, x, xsum, bias, z, M, s);
+    return wide ? launch_tc<B, 128>(d, x, xsum, bias, z, M, s) : launch_tc<B, 64>(d, x, xsum, bias, z, M, s);
   QUIP_TC(2) QUIP_TC(3) QUIP_TC(4)
 #undef QUIP_TC
-  set_error("tcgen05 kernel: unsupported bits=%d", d->bits);
+  set_error("tensor-core kernel: unsupported bits=%d", d->bits);
   return QUIP_ERR_UNSUPPORTED;
 }
 

@@ -1,7 +1,7 @@
 // Packed-integer x fp16 contraction for a handful of tokens (decode, M <= 8): the HBM-bound regime
 // of the path (reference Quant3Linear.forward is M == 1 only, quant.py:222-233, on the absent
-// quant_cuda.vecquant3matmul).  Speed of light is one pass over the packed words at ~6.5 TB/s, i.e. an
-// SM has ~22 cycles per 512-byte super-block: the limits are (1) instructions per weight on the ALU
+// quant_cuda.vecquant3matmul).  Speed of light is one pass over the packed words at HBM bandwidth, i.e.
+// an SM has only a few tens of cycles per 512-byte super-block: the limits are (1) instructions per weight on the ALU
 // pipe (LOP3/SHF retire one warp-instruction per 2 cycles per SM sub-partition) and on the legacy tensor
 // pipe (every mma.sync shape retires one per 8 cycles per sub-partition -- tools/mma_rate.cu), and
 // (2) dependent round trips to memory.  Two datapaths share one skeleton:
@@ -962,11 +962,9 @@ static int launch_gv_i8(const QuipLinearDesc* d, const __half* x, const __half* 
 // every warp owns whole row blocks and streams their k run straight from global memory into a register ring
 // (8 x 512 B in flight per warp, 24 warps per SM), accumulates alone and writes its 16 x M outputs itself.  No
 // shared-memory ring, no producer, no barrier after the token prologue: the same shape as a plain read loop
-// (tools/read_bw.cu: 6.7-7.0 TB/s read-only on this GPU) with ~33 instructions of math per 512 bytes.
-// Measured on a 352256 x 4096 matrix, one token: 5.15 TB/s = 78 % of the HBM copy peak (2-bit), 6.7 TB/s
-// (4-bit); the cooperative bulk-copy kernel above stays at 3.8 TB/s there (its ring alone, math removed, moves
-// 4.4 TB/s) but is the faster one for a single layer, where nothing is steady and latency is everything
-// (4096 x 4096: 4.1 us against 8.7 us).
+// (tools/read_bw.cu measures its ceiling) with ~33 instructions of math per 512 bytes.  It is meant for steady
+// streaming over very many row blocks; the cooperative bulk-copy kernel above is the choice for a single layer,
+// where nothing is steady and latency is everything.
 // ---------------------------------------------------------------------------------------------
 constexpr int GS_WARPS = 8;            // per CTA; 3 CTAs per SM
 constexpr int GS_D = 8;                // super-blocks in flight per warp

@@ -475,7 +475,7 @@ extern "C" int quip_rot_pass(const QuipPass* ps, const void* in_, void* out_, in
     return launch_small<64>(ps, in, out, M, n, s);
   }
   if (impl != 1 && impl != 3 && big_ok && M > 32 && ((((uintptr_t)in | (uintptr_t)out | (uintptr_t)ps->factors) & 15) == 0))
-    return pass_big_tc(ps, in, out, M, n, s);      // tcgen05: the 688x688 blocks of an 11008 side are real GEMMs
+    return pass_big_tc(ps, in, out, M, n, s);      // wgmma: the 688x688 blocks of an 11008 side are real GEMMs
   if (impl != 1 && big_ok) {
     size_t smem = (size_t)BIG_STAGES * (BIG_BM + BIG_BN) * BIG_LD * sizeof(__half);
     QUIP_CUDA(cudaFuncSetAttribute(pass_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

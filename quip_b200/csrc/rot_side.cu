@@ -5,8 +5,8 @@
 //
 // (reference: one call of mul_ortho_butterfly, method.py:46-67, plus the scaleWH division of
 // method.py:202-204 on the K side and the bias on the N side.)  As separate kernels -- gather, strided
-// pass, contiguous pass -- each step is a full HBM round trip of the (M, n) activations: 96 MB and ~50 us per
-// 4096-wide side at M = 2048, a third of the step.  Here a CTA keeps 16 token rows in shared memory for
+// pass, contiguous pass -- each step is a full HBM round trip of the (M, n) activations: 96 MB per
+// 4096-wide side at M = 2048.  Here a CTA keeps 16 token rows in shared memory for
 // the whole side: x is read once and x2 written once; the factors (1 MiB per side) come from L2, stored a second
 // time in tensor-core fragment order (QuipPass.factors_frag) so that a warp fetches 512 contiguous bytes per load
 // -- read row-major, every fragment load touched eight cache lines and the load pipe, not the tensor pipe, set the pace.

@@ -3,8 +3,8 @@
 // One side is two block-diagonal passes (reference mul_ortho_butterfly, method.py:46-67): the outputs of the first pass
 // are regrouped -- every block of the second pass takes exactly one output from each block of the first (the (p1, p2)
 // view is multiplied along its columns, then along its rows).  As separate kernels (rot_fewtok.cu) the regrouping is a
-// kernel boundary: 2.2 us of dependent launch latency per pass, four passes per QuantLinear, more than the time the bytes
-// take.  Here the CTA that owns a block c1 of the SECOND pass computes its own inputs: input j of block c1 is output
+// kernel boundary: a dependent launch latency per pass, four passes per QuantLinear, which at a few tokens costs more
+// than the time the bytes take.  Here the CTA that owns a block c1 of the SECOND pass computes its own inputs: input j of block c1 is output
 // i_j of first-pass block c0_j, i.e. ONE ROW of that block's factor times the block's inputs,
 //
 //     t[j]    = sum_k F0[c0_j][i_j][k] * in[ src(pos0(c0_j, k)) ]              (p1 dot products of length p0)

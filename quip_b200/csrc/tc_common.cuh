@@ -1,4 +1,4 @@
-// Device helpers shared by the tcgen05 kernels: mbarrier / TMA / tcgen05 PTX wrappers, the 128B-swizzle
+// Device helpers shared by the tensor-core kernels: mbarrier / TMA / wgmma PTX wrappers, the 128B-swizzle
 // operand descriptor, and the packed-word -> fp16 operand-tile producer.
 #pragma once
 #include <cuda.h>
@@ -7,10 +7,11 @@
 
 namespace quip {
 
-constexpr int TC_BM = 128;            // output rows per tile (MMA M)
+constexpr int TC_BM = 128;            // output rows per tile: two consumer warpgroups of 64 (wgmma M)
 constexpr int TC_BK = 64;             // k per stage = one 128-byte swizzle atom of fp16
 constexpr int TC_PROD_GROUPS = 2;     // producer groups of 4 warps alternate k super-blocks
-constexpr int TC_THREADS = 192 + 128 * TC_PROD_GROUPS;
+constexpr int TC_CONSUMER_WARPS = 8;  // warps 0-7: two consumer warpgroups (wgmma + epilogue)
+constexpr int TC_THREADS = 32 * TC_CONSUMER_WARPS + 128 * TC_PROD_GROUPS + 32;   // + one TMA warp
 constexpr uint32_t TC_WATCHDOG = 1u << 28;
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -48,47 +49,54 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16, single CTA
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// K-major, SWIZZLE_128B operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart.
+// K-major, SWIZZLE_128B operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart (sm_90 wgmma descriptor).
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);        // start address, bits [0,14)
   d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                              // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
   return d;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+
+// D (registers, fp32, 64 x N per warpgroup) (+)= A[smem desc] (64 x 16) * B[smem desc]^T (N x 16), both K-major
+template <int N>
+__device__ __forceinline__ void wgmma_f16_ss(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, int scale_d);
+template <>
+__device__ __forceinline__ void wgmma_f16_ss<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+template <>
+__device__ __forceinline__ void wgmma_f16_ss<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from moving accumulator reads or writes across a wgmma fence / wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // packed words one producer thread needs for one (row block, lane) over one k super-block (128 k)
 template <int BITS>
@@ -139,29 +147,7 @@ __device__ __forceinline__ void tc_store_chunk(const TcWords<BITS>& r, uint32_t 
 }
 
 
-// Epilogue store of one 32-token chunk of a warp's 32 output rows.  After tcgen05.ld every lane owns ONE
-// output row and 32 consecutive tokens, i.e. addresses N*2 bytes apart: storing them directly is 32
-// two-byte warp stores per chunk (measured ~30 cycles each; ~16 us per 128x256 tile, which left the last
-// tile's epilogue fully exposed).  Transposing the chunk through a 2 KB warp-private shared-memory patch
-// turns it into 4 x 16-byte stores per lane, 64 contiguous bytes per token row.
-constexpr int EPI_STAGE_HALVES = 32 * 32;      // per epilogue warp
-__device__ __forceinline__ void epilogue_store_chunk(__half* stage, const float (&v)[32], __half* __restrict__ z,
-                                                     int64_t ldz, int m_base, int M, int n_base, int N, int lane) {
-#pragma unroll
-  for (int c = 0; c < 32; ++c) stage[c * 32 + lane] = __float2half_rn(v[c]);
-  __syncwarp();
-  const int seg = (lane & 3) * 8;
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const int t = (lane >> 2) + 8 * r;
-    const uint4 val = *reinterpret_cast<const uint4*>(&stage[t * 32 + seg]);
-    const int m = m_base + t, n = n_base + seg;
-    if (m < M && n < N) *reinterpret_cast<uint4*>(z + (int64_t)m * ldz + n) = val;
-  }
-  __syncwarp();
-}
-
-// Weight-producer loop shared by the 1-CTA and 2-CTA kernels.  Group `grp` (4 warps) expands the k
+// Weight-producer loop of the packed GEMM.  Group `grp` (4 warps) expands the k
 // super-blocks grp, grp+G, ... of every tile into stages 2*ksb and 2*ksb+1 of the global stage sequence.
 // Two groups are needed because fence.proxy.async compiles to MEMBAR.ALL.CTA, which also waits for the
 // thread's outstanding prefetch loads: with one group the ~1 us global-load latency would be exposed once

@@ -4,7 +4,7 @@ Keeps the reference's structure (opt.py:193-299, llama.py:174-253): catch the in
 0 with a `Catcher`, run the decoder layers one by one on one 2048-token sample at a time (batch 1),
 then final norm -> lm_head -> CrossEntropy on fp16 logits -> ppl = exp(sum NLL / (nsamples*seqlen)).
 
-B200-first differences:
+Differences from the reference loop:
   * packed layers are small (2-bit Llama-2-7B: 1.6 GB codes + 1.9 GB butterfly factors), so the whole
     model stays resident in HBM instead of being shuttled layer by layer over PCIe (opt.py:260,265);
     `offload=True` restores the reference's layer-by-layer residency for models that do not fit;

@@ -2,7 +2,7 @@
 
 The reference's eval loop calls the HF decoder layer (llama.py:227); around the seven linears that layer issues ~25
 elementwise / reduction launches (LlamaRMSNorm 8, apply_rotary_pos_emb 9 for q and k, residual adds, SiLU and the gate
-product) which cost 27 % of a 2048-token step once the linears are packed (profiles/launches_r01.json).  `llama_stack`
+product), a large share of a 2048-token step once the linears are packed.  `llama_stack`
 runs the same layers -- the layer's own modules for every linear and its own weights for the norms -- with that glue as
 four kernel launches per layer:
 
@@ -92,7 +92,7 @@ def mlp_layout_plan(mlp):
     """The combined index of the three permutations around SiLU(gate) * up of a packed Llama MLP -- the output gathers of
     gate_proj / up_proj (y[j] = layout[u_idx[j]]) and the input gather of down_proj (layout[l] = x[v_idx[l]]) -- so that one
     kernel (quip_silu_mul_gather) replaces three gather launches and silu_mul: for an 11008-wide side the gather is a kernel of
-    its own (29 us at 2048 tokens each, profiles/launches_r01.json).  None when the layers are not packed, have a bias /
+    its own.  None when the layers are not packed, have a bias /
     unfolded 1/s at those gathers, or are too wide for 16-bit positions.  Cached on the module."""
     from .quant import QuantLinear
     gate, up, down = mlp.gate_proj, mlp.up_proj, mlp.down_proj

@@ -1,4 +1,4 @@
-"""Llama entry points of the reference's llama.py, on the packed B200 path.
+"""Llama entry points of the reference's llama.py, on the packed H100 path.
 
 Kept names (reference llama.py): get_llama (:19-33), llama_eval (:174-253), llama_pack (:256-275),
 load_quant (:322-358), llama_multigpu (:361-415), benchmark (:418-471).  The reference's llama.py is

@@ -1,4 +1,4 @@
-"""OPT entry points of the reference's opt.py, on the packed B200 path.
+"""OPT entry points of the reference's opt.py, on the packed H100 path.
 
 Kept names (reference opt.py): get_opt (:14-26), opt_eval (:193-299), opt_pack3 (:303-315) ->
 opt_pack, load_quant3 (:317-348) / load_quant (:350-381), opt_multigpu (:384-428), benchmark

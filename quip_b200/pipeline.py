@@ -6,7 +6,7 @@ groups inside one process (opt.py:413-426, llama.py:370-413; SURVEY section 2 #1
 two ways (SURVEY section 8e):
 
   * data parallel over samples (`dp_eval`): the eval loop's samples are independent (opt.py:262-264),
-    the 2-bit model fits one B200 many times over, so every rank holds the packed weights and
+    the 2-bit model fits one 80 GB H100 several times over, so every rank holds the packed weights and
     evaluates samples rank, rank+G, ...; the only collective is one all-reduce of (sum NLL, tokens).
   * layer pipeline (`pp_eval`), for models that do not fit one GPU: contiguous layer ranges per rank
     exactly as opt.py:424-426 (or --layers-dist, llama.py:400-413), micro-batch = one sample, hidden

@@ -1,4 +1,4 @@
-"""Quantizer / QuantLinear / make_quant -- the reference's quant.py surface, backed by sm_100a kernels.
+"""Quantizer / QuantLinear / make_quant -- the reference's quant.py surface, backed by sm_90a kernels.
 
 Reference surface kept (Cornell-RelaxML/QuIP, quant.py):
   * `Quantizer` (quant.py:23-163): `configure / find_params / quantize / enabled / ready`, buffers

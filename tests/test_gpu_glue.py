@@ -1,8 +1,7 @@
 """Glue kernels of csrc/glue.cu (quip_rmsnorm / quip_rope / quip_silu_mul) against the torch restatement of the HF Llama
 modules (oracle/glue.py, pinned bit-for-bit to transformers' LlamaRMSNorm / apply_rotary_pos_emb / SiLU*up on the CPU in
 tests/test_fused_layer.py), at the Llama-2-7B shapes bench.py runs them at.  These are the cases of
-tests/quick_glue_check.py, which ran on a B200 at the end of round 1 (profiles/glue_check_r01.json); the wider shape sweep
-is in tests/test_gpu_staged.py."""
+tests/quick_glue_check.py; the wider shape sweep is in tests/test_gpu_staged.py."""
 import pytest
 import torch
 

@@ -1,14 +1,15 @@
 """The kernels of the benchmark step at the benchmark's own shapes, against independent references.
 
-bench.py runs `qgemm_tc_kernel<2,256,false>` at (N, K, M) in {(4096, 4096), (11008, 4096), (4096, 11008)} x 2048 tokens:
-256-688 tiles on 148 persistent CTAs, i.e. every CTA walks several tiles and exercises the cross-tile weight prefetch, the
-ring-phase wrap and the double-buffered TMEM accumulator -- none of which the small oracle cases (<= 86 tiles) reach.
+bench.py runs `qgemm_tc_kernel<2,128,false>` at (N, K, M) in {(4096, 4096), (11008, 4096), (4096, 11008)} x 2048 tokens:
+512-1376 tiles on 132 persistent CTAs (one per H100 SM), i.e. every CTA walks several tiles and exercises the cross-tile
+weight prefetch, the ring-phase wrap and the epilogue of one tile overlapping the producers of the next -- none of which the
+small oracle cases (<= 86 tiles) reach.
 Here those launches are compared with a float64 contraction of the unpacked codes (tolerance 3e-4: the fp16 output
 rounding), checked for run-to-run determinism, and whole QuantLinear forwards at the same shapes are compared with
   * the fp32 restatement of the pipeline (quip_b200/selfcheck.restated_forward),
   * the reference's own dense path F.linear(x, W_ref), W_ref = fp16(fp16(U^T Q V)/s) (method.py:195-214), restated in
     quip_b200/selfcheck.reference_dense_weight and pinned to the live reference by tests/golden/layer_big_4096.npz,
-  * the live reference's y_ref of that golden layer, replicated to 2048 tokens so it runs through the tcgen05 route.
+  * the live reference's y_ref of that golden layer, replicated to 2048 tokens so it runs through the wgmma route.
 Tolerance for whole layers: 1e-3 relative (north_star), norm-wise.
 """
 import json
@@ -120,7 +121,7 @@ def test_kronecker_layers_at_bench_shapes(K, N):
 def test_golden_4096_layer_from_the_live_reference():
     """tests/golden/layer_big_4096.npz: a q_proj-sized Linear quantized by the reference's own Balance flow (ldlq, 2 bits,
     --incoh_processing).  Its 16-token y_ref through every token-count route, including 2048 tokens (the 16 rows
-    replicated 128 times, so the multi-tile tcgen05 path is compared with the live reference's own output)."""
+    replicated 128 times, so the multi-tile wgmma path is compared with the live reference's own output)."""
     from quip_b200 import quant as Q
     from quip_b200.incoherence import plan_side
     from quip_b200.selfcheck import reference_dense_weight, rel_err
@@ -157,7 +158,7 @@ def test_golden_4096_layer_from_the_live_reference():
                                  (28672, 7168), (2048, 2048), (2048, 8192), (8192, 2048)])
 def test_other_model_shapes_at_2048_tokens(K, N):
     """Layer shapes of BASELINE configs[1], [3], [4] (OPT-1.3b, OPT-30b, Llama-2-70B: sides 2048 = 64 x 32, 7168 = 224 x 32,
-    8192 = 128 x 64, 28672 = 448 x 64, 1024 = 32 x 32) through the many-token route -- dense tcgen05 passes for the wide
+    8192 = 128 x 64, 28672 = 448 x 64, 1024 = 32 x 32) through the many-token route -- dense wgmma passes for the wide
     blocks, small-block passes, the one-kernel side where both blocks are 32 / 64 wide -- against the fp32 restatement."""
     from quip_b200 import quant as Q
     from quip_b200.selfcheck import rel_err, restated_forward

@@ -1,4 +1,4 @@
-"""CUDA kernels vs the CPU oracle, through the C ABI.  Everything except the tcgen05 GEMM (which has
+"""CUDA kernels vs the CPU oracle, through the C ABI.  Everything except the wgmma GEMM (which has
 its own file so a protocol bug there cannot poison this process's CUDA context)."""
 import os
 

@@ -1,6 +1,5 @@
 """Glue kernels (csrc/glue.cu), the fused Llama stack / decode step, and batched-decode token counts (9..32) through the
-few-token passes.  Written in round 1 after its GPU budget was spent ("staged"); verified on a B200 in round 2 and part of
-the default `-m gpu` run since.
+few-token passes.  Written in round 1 after its GPU budget was spent ("staged"); part of the default `-m gpu` run.
 
 Covered: quip_rmsnorm / quip_rope / quip_silu_mul through quip_b200.fused.CudaGlue against the torch restatement
 oracle/glue.py (itself pinned bit-for-bit against the HF modules on the CPU, tests/test_fused_layer.py); the fused Llama stack

@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM GEMM vs the CPU oracle (kept in its own file: see tests/test_gpu_kernels.py)."""
+"""Tensor-core (wgmma + TMA) GEMM vs the CPU oracle (kept in its own file: see tests/test_gpu_kernels.py)."""
 import numpy as np
 import pytest
 
@@ -39,7 +39,7 @@ def test_tc_and_skinny_agree():
 
 
 def test_big_block_pass_on_tensor_cores():
-    """Block-diagonal pass with 688 x 688 blocks (the 11008 side of Llama-2-7B) through the TMA-fed tcgen05 kernel."""
+    """Block-diagonal pass with 688 x 688 blocks (the 11008 side of Llama-2-7B) through the TMA-fed wgmma kernel."""
     from gpu_util import run_pass
     from oracle import butterfly as obf
     for (p, nblk, M, shared) in [(688, 16, 2048, False), (224, 32, 300, False), (128, 8, 129, True), (96, 4, 64, False)]:

@@ -198,9 +198,10 @@ def test_abi_v2_structs_carry_the_optional_pointers():
 
 
 def test_committed_bench_line_has_the_contract_keys():
-    """profiles/bench_r01_final.json is the JSON line bench.py printed on the B200: every key the driver reads is there."""
+    """tests/golden/bench_line_h100.json is the JSON line bench.py printed on an H100 (80 GB HBM3, 400 W power limit):
+    every key a consumer of the line reads is there."""
     import json
-    path = os.path.join(ROOT, 'profiles', 'bench_r01_final.json')
+    path = os.path.join(ROOT, 'tests', 'golden', 'bench_line_h100.json')
     line = [l for l in open(path).read().splitlines() if l.strip().startswith('{')][-1]
     d = json.loads(line)
     for k in ('metric', 'value', 'unit', 'n_gpus', 'steps', 'warmup', 'ms_per_step', 'higher_is_better', 'scaling',

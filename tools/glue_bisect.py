@@ -1,4 +1,4 @@
-"""Where does the fused Llama stack (quip_b200/fused.py) part from the HF decoder layers?  (B200 only)
+"""Where does the fused Llama stack (quip_b200/fused.py) part from the HF decoder layers?  (needs a CUDA device)
 
     python tools/glue_bisect.py [--layers 2] > gpurun_out/glue_bisect.json
 

@@ -1,6 +1,6 @@
 // Legacy (mma.sync) tensor-pipe issue rates on this GPU: how many HMMA.16816 / IMMA.16832 an SM retires per cycle.
 // The few-token contraction (qgemv.cu) spends one MMA per 256 (fp16) or 512 (int8) weights whatever the token
-// count, so this rate, not HBM, can be the ceiling.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/mma_rate tools/mma_rate.cu
+// count, so this rate, not HBM, can be the ceiling.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/mma_rate tools/mma_rate.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

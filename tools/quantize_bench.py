@@ -1,6 +1,6 @@
 """Quantise real Llama-2-7B-shaped decoder layers ON THE GPU with this package's producer (quip_b200/quantize.py: tensor-core
 Hessian accumulation, incoherence processing, LDLQ-RG with the column loops of csrc/ldlq.cu), pack them, and measure the
-perplexity of the packed model against the dense fake-quantised model the reference would evaluate (B200 only).
+perplexity of the packed model against the dense fake-quantised model the reference would evaluate (needs a CUDA device).
 
     python tools/quantize_bench.py [--layers 2] [--calib 4] [--eval 2] > gpurun_out/quantize_bench.json
 

@@ -1,6 +1,6 @@
 // Read-only streaming bandwidth on this GPU: the denominator a weight-streaming kernel (qgemv.cu) can actually
 // reach, as opposed to the copy figure (read + write) of MEASURED_PEAKS.json.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/read_bw tools/read_bw.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/read_bw tools/read_bw.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
