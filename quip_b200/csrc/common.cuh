@@ -158,4 +158,39 @@ __device__ __forceinline__ void expand_chunk(uint32_t w0, uint32_t w1, uint32_t 
   }
 }
 
+// The A fragment of mma.sync m16n8k16 / wgmma m64nNk16 (per warp: 16 rows) in NATURAL k order, straight from the
+// packed words.  Lane (g, t) needs, for k16 step S (0, 1) of chunk CH, rows g / g+8 (row half r = 0 / 1) at chunk k
+//   a0 / a1: 16S + 2t, +1        a2 / a3: 16S + 8 + 2t, +1.
+// In the native layout chunk k = 8t' + pos belongs to lane 4g + t' (same g), pos = 2u + e, so those are pair u = t of
+// lanes 4g + 2S (a0, a1) and 4g + 2S + 1 (a2, a3): every fragment of a row group comes from the words of its lanes
+// 4g..4g+3, held as RowWords w[row_words(BITS)]:
+//   bits 2: w[4t' + ch]                      = word ch of lane 4g + t'          (super-block words 16g + [0,16))
+//   bits 3: as bits 2 (hi plane), w[16 + 2t' + ch/2] = lo-plane word of lane 4g + t'   (words 128 + 8g + [0,8))
+//   bits 4: w[16(ch/2) + 4t' + 2(ch%2) + pos/4]                                  (words 128(ch/2) + 16g + [0,16))
+// Pair u = t of row half r sits at field slot2(t, r) = slot2(t, 0) + r (bits 4: word pos/4 = t/2, slot4(t%2, r)), so
+// one runtime shift per word, by the lane's own field offset, moves row half 0 to field 0 and row half 1 to field 1;
+// the compile-time dq helpers then finish as in expand_chunk.  The fp16 values are the ones expand_chunk makes.
+__host__ __device__ constexpr int row_words(int bits) { return bits == 2 ? 16 : (bits == 3 ? 24 : 32); }
+
+template <int BITS, int CH, int S>
+__device__ __forceinline__ void frag_natural(const uint32_t (&w)[row_words(BITS)], int t, uint32_t* a) {
+  if constexpr (BITS == 2 || BITS == 3) {
+    const uint32_t sh = 2u * (uint32_t)slot2(t, 0);
+    const uint32_t x0 = w[4 * (2 * S) + CH] >> sh, x1 = w[4 * (2 * S + 1) + CH] >> sh;
+    if constexpr (BITS == 2) {
+      a[0] = dq2<0>(x0); a[1] = dq2<1>(x0); a[2] = dq2<0>(x1); a[3] = dq2<1>(x1);
+    } else {
+      // lo plane: pair 8 (CH % 2) + slot of word CH / 2
+      const uint32_t shl = 8u * (CH & 1) + (uint32_t)slot2(t, 0);
+      const uint32_t y0 = w[16 + 2 * (2 * S) + (CH >> 1)] >> shl, y1 = w[16 + 2 * (2 * S + 1) + (CH >> 1)] >> shl;
+      a[0] = dq3<0, 0>(x0, y0); a[1] = dq3<1, 1>(x0, y0); a[2] = dq3<0, 0>(x1, y1); a[3] = dq3<1, 1>(x1, y1);
+    }
+  } else {
+    const uint32_t sh = 4u * (uint32_t)slot4(t & 1, 0);
+    constexpr int i0 = 16 * (CH >> 1) + 4 * (2 * S) + 2 * (CH & 1), i1 = i0 + 4;
+    const uint32_t x0 = ((t & 2) ? w[i0 + 1] : w[i0]) >> sh, x1 = ((t & 2) ? w[i1 + 1] : w[i1]) >> sh;
+    a[0] = dq4<0>(x0); a[1] = dq4<1>(x0); a[2] = dq4<0>(x1); a[3] = dq4<1>(x1);
+  }
+}
+
 }  // namespace quip

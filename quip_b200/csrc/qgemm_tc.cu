@@ -2,52 +2,57 @@
 // (the reference's eval loop calls every Linear with M = 2048: opt.py:262-264, llama.py:226-227).
 //
 //   D[n][m] (registers, fp32) = sum_k A[n][k] * B[m][k]
-//     A = packed weights, 128 output rows per tile, expanded to fp16 d=(c-cbar)/2^bits by the
-//         producer warps and written straight into the 128B-swizzled K-major operand layout
-//         (generic-proxy st.shared + fence.proxy.async), never touching HBM as fp16;
+//     A = packed weights, 128 output rows per tile.  The packed words of a k super-block are staged in shared
+//         memory by TMA, and each consumer warp expands its own 16 rows to fp16 d=(c-cbar)/2^bits directly
+//         into the wgmma A registers (the packed layout is the m16n8k16 A fragment with k relabelled, see
+//         frag_natural), so A never exists as fp16 in shared memory or HBM;
 //     B = activations x2 (M,K) fp16, BN tokens per tile, staged by TMA (cp.async.bulk.tensor, 128B
 //         swizzle, out-of-bounds rows zero-filled so ragged M needs no special case);
 //   epilogue: z[m][n] = P_n * D + R_n * xsum[m] (+ bias_n) -> fp16, transposed through shared memory so
 //   that every store is 16 contiguous bytes of one token row.
 //
-// Warp roles (544 threads, one persistent CTA per SM, static tile schedule):
-//   warps 0-7   two consumer warpgroups: warpgroup w issues wgmma.m64nBNk16 for rows 64w..64w+63 of the
-//               tile, then runs the epilogue of those rows
-//   warps 8-15  weight producers (2 groups of 4 alternating k super-blocks): 128-bit loads of packed
-//               words -> registers -> fp16 -> smem
-//   warp 16     TMA producer
-// Pipeline: smem ring full[s]/empty[s] (TMA + 4 producer warps -> 8 consumer warps).  The producers keep
-// filling the ring while the consumers run a tile's epilogue.
+// Warp roles (288 threads, one persistent CTA per SM, static tile schedule):
+//   warps 0-7   two consumer warpgroups: warpgroup w issues wgmma.m64nBNk16 (A from registers, B from shared
+//               memory) for rows 64w..64w+63 of the tile, then runs the epilogue of those rows
+//   warp 8      TMA producer: activation tile of every 64-k stage, packed words of every 128-k super-block
+// Pipeline: smem ring full[s]/empty[s] (TMA -> 8 consumer warps).  The TMA warp keeps filling the ring while the
+// consumers run a tile's epilogue.  Per SM clock at full tensor rate the shared-memory traffic is the wgmma B reads
+// (64 B) + the TMA writes of B (32 B) + the packed words (about 4 B), under the 128 B/clk the SM can serve.
 #include "tc_common.cuh"
 
 namespace quip {
 
 constexpr int TC_SMEM_MAX = 227 * 1024;                      // opt-in dynamic shared memory per block
 
-template <int BN>
+template <int BITS, int BN, bool DENSE>
 struct TcCfg {
-  static constexpr int A_BYTES = TC_BM * TC_BK * 2;            // 16 KB
+  // A region of a stage: the fp16 A tile (dense), or the packed words of the tile's 8 row blocks for one k super-block
+  // (packed; written on even stages only, the odd stage of the same super-block reads its words from registers)
+  static constexpr int A_BYTES = DENSE ? TC_BM * TC_BK * 2 : (TC_BM / SB_ROWS) * sb_words(BITS) * 4;   // 16 / 4, 6, 8 KB
   static constexpr int B_BYTES = BN * TC_BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;        // multiple of 1024: B stays aligned for its swizzle
   // epilogue transpose buffer of one consumer warpgroup: BN token rows x 64 n (packed) or 64 token rows x BN
   // columns (dense), rows padded by 16 bytes against bank conflicts
   static constexpr int EPI_HALVES = BN * 72 > 64 * (BN + 8) ? BN * 72 : 64 * (BN + 8);
   static constexpr int EPI_BYTES = 2 * EPI_HALVES * 2;
-  static constexpr int STAGES = (TC_SMEM_MAX - EPI_BYTES - 1024 - 256) / STAGE_BYTES;   // 128 -> 5, 64 -> 8
+  static constexpr int STAGES_FIT = (TC_SMEM_MAX - EPI_BYTES - 1024 - 256) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT < 16 ? STAGES_FIT : 16;       // 2 x 16 barriers fill the 256-byte area
   static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + EPI_BYTES;
+  static_assert(STAGE_BYTES % 1024 == 0 && 2 * STAGES * 8 <= 256, "stage layout");
 };
 
-// DENSE = false: A is the packed matrix (N rows, K columns), expanded by the producer warps.
+// DENSE = false: A is the packed matrix (N rows, K columns); its words are staged by TMA and expanded in registers.
 // DENSE = true : block-diagonal pass with big blocks -- `nblk` independent GEMMs out_b = in_b . F_b^T, A = the
 //                block's p contiguous activation columns (128 tokens per tile), B = fp16 factor F_b (N = K = p)
 //                fetched by TMA (3-D map, rows/cols beyond p zero-filled), output written to the same columns.
+// tmap_a: packed words (DENSE = false; 2-D, one row of KSB * sb_words words per 16-row block) or the factors.
 template <int BITS, int BN, bool DENSE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_a,
-                const uint32_t* __restrict__ q, const float* __restrict__ scales, const float* __restrict__ zeros,
-                const __half* __restrict__ bias, const float* __restrict__ xsum, __half* __restrict__ z, int M, int K,
-                int N, int symmetric, int nblk, int shared_factor) {
-  using C = TcCfg<BN>;
+                const float* __restrict__ scales, const float* __restrict__ zeros, const __half* __restrict__ bias,
+                const float* __restrict__ xsum, __half* __restrict__ z, int M, int K, int N, int symmetric, int nblk,
+                int shared_factor) {
+  using C = TcCfg<BITS, BN, DENSE>;
   extern __shared__ unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   unsigned char* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -64,15 +69,14 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   const int per_blk = tiles_n * tiles_m;
   const int num_tiles = per_blk * nblk;
   const int KB = (K + TC_BK - 1) / TC_BK;
-  const int KSB = K >> 7;
   const int64_t ldz = (int64_t)N * nblk;       // output row pitch (== N for the packed GEMM)
-  constexpr int TMA_WARP = TC_CONSUMER_WARPS + 4 * TC_PROD_GROUPS;
+  constexpr int TMA_WARP = TC_CONSUMER_WARPS;
 
   if (warp == TMA_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
-    if (DENSE) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
     for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(&full[s], DENSE ? 1 : 1 + 4);  // TMA producer (+ 4 weight-producer warps)
+      mbar_init(&full[s], 1);                  // TMA producer
       mbar_init(&empty[s], TC_CONSUMER_WARPS); // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -80,7 +84,7 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   __syncthreads();
 
   if (warp == TMA_WARP) {
-    // ================= TMA producer: activation tiles =================
+    // ================= TMA producer: activation tiles (+ packed words, one super-block per even stage) ==========
     if (lane == 0) {
       int s = 0;
       uint32_t ph = 0;
@@ -89,19 +93,23 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
         const int m0 = (rr / tiles_n) * (DENSE ? TC_BM : BN), n0 = (rr % tiles_n) * (DENSE ? BN : TC_BM);
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&empty[s], ph ^ 1u);
-          mbar_arrive_expect_tx(&full[s], DENSE ? C::STAGE_BYTES : C::B_BYTES);
           unsigned char* stage = smem_gen + (size_t)s * C::STAGE_BYTES;
           if (DENSE) {
+            mbar_arrive_expect_tx(&full[s], C::STAGE_BYTES);
             tma_load_2d(stage, &tmap_x, &full[s], blk * K + kb * TC_BK, m0);                     // A: 128 tokens
             tma_load_3d(stage + C::A_BYTES, &tmap_a, &full[s], kb * TC_BK, n0, shared_factor ? 0 : blk);   // B: BN factor rows
           } else {
+            // row blocks beyond N are zero-filled; their output rows are never stored
+            const bool words = (kb & 1) == 0;
+            mbar_arrive_expect_tx(&full[s], C::B_BYTES + (words ? C::A_BYTES : 0));
+            if (words) tma_load_2d(stage, &tmap_a, &full[s], (kb >> 1) * sb_words(BITS), n0 / SB_ROWS);
             tma_load_2d(stage + C::A_BYTES, &tmap_x, &full[s], kb * TC_BK, m0);
           }
           if (++s == C::STAGES) { s = 0; ph ^= 1u; }
         }
       }
     }
-  } else if (warp < TC_CONSUMER_WARPS) {
+  } else {
     // ================= consumers: wgmma over the ring, then the epilogue of 64 rows =================
     const int wg = warp >> 2, wtid = threadIdx.x & 127;
     const int frow = (warp & 3) * 16 + (lane >> 2);        // accumulator row of d[j] for (j & 2) == 0; +8 otherwise
@@ -112,31 +120,105 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     int s = 0;
     uint32_t ph = 0;
+    auto advance = [&]() { if (++s == C::STAGES) { s = 0; ph ^= 1u; } };
+    auto release = [&](int st) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int blk = tile / per_blk, rr = tile % per_blk;
       int prev = 0;
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(&full[s], ph);
-        const uint32_t a_addr = smem_base + (uint32_t)(s * C::STAGE_BYTES);
-        const uint64_t adesc = make_sw128_desc(a_addr + (uint32_t)(wg * 64 * 128));
-        const uint64_t bdesc = make_sw128_desc(a_addr + C::A_BYTES);
-        wgmma_fence();
+      // packed epilogue operands, fetched before the k loop so that their latency is hidden behind it: P_n, R_n,
+      // bias_n of rows frow / frow + 8 in registers, the tile's BN xsum values into L1
+      const int n_base = (rr % tiles_n) * TC_BM + wg * 64, m0 = (rr / tiles_n) * BN;
+      float Pn[2], Rn[2], bn[2];
+      if constexpr (!DENSE) {
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)     // +32 bytes along K inside the swizzle atom = +2 encoded
-          wgmma_f16_ss<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
-        wgmma_commit();
-        wgmma_wait<1>();                         // the previous stage's wgmma have read their operands
-        if (kb > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[prev]);
+        for (int h = 0; h < 2; ++h) {
+          const int n = n_base + frow + 8 * h;
+          Pn[h] = 1.f; Rn[h] = 0.f; bn[h] = 0.f;
+          if (n < N) {
+            const float sc = scales[n];
+            Pn[h] = sc * (float)(1 << BITS);
+            if (!symmetric) Rn[h] = sc * (0.5f * (float)((1 << BITS) - 1)) - zeros[n];
+            if (bias) bn[h] = __half2float(bias[n]);
+          }
         }
-        prev = s;
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+        if (!symmetric && wtid < BN / 32 && m0 + 32 * wtid < M)
+          asm volatile("prefetch.global.L1 [%0];" ::"l"(xsum + m0 + 32 * wtid));
+      }
+      if constexpr (DENSE) {
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(&full[s], ph);
+          const uint32_t a_addr = smem_base + (uint32_t)(s * C::STAGE_BYTES);
+          const uint64_t adesc = make_sw128_desc(a_addr + (uint32_t)(wg * 64 * 128));
+          const uint64_t bdesc = make_sw128_desc(a_addr + C::A_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < TC_BK / 16; ++k)     // +32 bytes along K inside the swizzle atom = +2 encoded
+            wgmma_f16_ss<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          wgmma_commit();
+          wgmma_wait<1>();                         // the previous stage's wgmma have read their operands
+          if (kb > 0) release(prev);
+          prev = s;
+          advance();
+        }
+      } else {
+        // Warp w owns row block w of the tile (rows 16w..16w+15 = the wgmma A rows of its warpgroup).  Each super-block
+        // (two stages) is read from shared memory once, at its even stage; the A fragments of a stage are built while
+        // the previous stage's wgmma run, into the other of two register sets (wgmma reads them asynchronously).
+        const int g = lane >> 2, t = lane & 3;
+        const uint32_t row_off = (uint32_t)(warp * sb_words(BITS) * 4);
+        uint32_t w[row_words(BITS)];
+        uint32_t fa[2][16];                        // A fragments of the even / odd stage: 4 k16 steps x a0..a3
+        auto issue = [&](const uint32_t (&f)[16], int first) {
+          const uint64_t bdesc = make_sw128_desc(smem_base + (uint32_t)(s * C::STAGE_BYTES) + C::A_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < TC_BK / 16; ++k)
+            wgmma_f16_rs<BN>(acc, &f[4 * k], bdesc + (uint64_t)(2 * k), (first && k == 0) ? 0 : 1);
+          wgmma_commit();
+        };
+        auto load_words = [&]() {
+          mbar_wait(&full[s], ph);
+          tc_load_row_words<BITS>(smem_base + (uint32_t)(s * C::STAGE_BYTES) + row_off, g, w);
+        };
+        load_words();
+        frag_natural<BITS, 0, 0>(w, t, &fa[0][0]);
+        frag_natural<BITS, 0, 1>(w, t, &fa[0][4]);
+        frag_natural<BITS, 1, 0>(w, t, &fa[0][8]);
+        frag_natural<BITS, 1, 1>(w, t, &fa[0][12]);
+        const int KSB = KB >> 1;
+        for (int ksb = 0; ksb < KSB; ++ksb) {
+          // even stage: chunks 0-1 of the super-block
+          const int se = s;
+          issue(fa[0], ksb == 0);
+          wgmma_wait<1>();                         // the odd stage of the previous super-block is done with fa[1]
+          if (ksb > 0) release(prev);
+          advance();
+          // odd stage: chunks 2-3, words already in registers
+          mbar_wait(&full[s], ph);
+          frag_natural<BITS, 2, 0>(w, t, &fa[1][0]);
+          frag_natural<BITS, 2, 1>(w, t, &fa[1][4]);
+          frag_natural<BITS, 3, 0>(w, t, &fa[1][8]);
+          frag_natural<BITS, 3, 1>(w, t, &fa[1][12]);
+          issue(fa[1], 0);
+          wgmma_wait<1>();                         // the even stage is done with fa[0] and its shared memory
+          release(se);
+          prev = s;
+          advance();
+          if (ksb + 1 < KSB) {
+            load_words();
+            frag_natural<BITS, 0, 0>(w, t, &fa[0][0]);
+            frag_natural<BITS, 0, 1>(w, t, &fa[0][4]);
+            frag_natural<BITS, 1, 0>(w, t, &fa[0][8]);
+            frag_natural<BITS, 1, 1>(w, t, &fa[0][12]);
+          }
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[prev]);
+      release(prev);
 
       if constexpr (DENSE) {
         // eb[token row r][column c], pitch BN + 8
@@ -158,19 +240,6 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       } else {
         // eb[token c][row r], pitch 72
         constexpr int EP = 72;
-        const int n_base = (rr % tiles_n) * TC_BM + wg * 64, m0 = (rr / tiles_n) * BN;
-        float Pn[2], Rn[2], bn[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int n = n_base + frow + 8 * h;
-          Pn[h] = 1.f; Rn[h] = 0.f; bn[h] = 0.f;
-          if (n < N) {
-            const float sc = scales[n];
-            Pn[h] = sc * (float)(1 << BITS);
-            if (!symmetric) Rn[h] = sc * (0.5f * (float)((1 << BITS) - 1)) - zeros[n];
-            if (bias) bn[h] = __half2float(bias[n]);
-          }
-        }
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) {
           const int h = (j >> 1) & 1, c = 8 * (j >> 2) + fcol + (j & 1), m = m0 + c;
@@ -188,13 +257,6 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       }
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // eb is free for the next tile
     }
-  } else if (!DENSE) {
-    // ================= weight producers: packed words -> fp16 operand tile =================
-    const int pw = (warp - TC_CONSUMER_WARPS) & 3, grp = (warp - TC_CONSUMER_WARPS) >> 2;
-    weight_producer_loop<BITS, C::STAGES, C::STAGE_BYTES>(
-        pw, grp, lane, q, KSB, N, empty, smem_base, (int)blockIdx.x, (int)gridDim.x, num_tiles,
-        [&](int tile) { return ((tile % per_blk) % tiles_n) * (TC_BM / 16); },
-        [&](int s) { mbar_arrive(&full[s]); });
   }
 }
 
@@ -249,18 +311,43 @@ int make_act_map(CUtensorMap* tmap, const void* x, int64_t rows, int64_t cols, i
   return QUIP_OK;
 }
 
+// packed words -> 2-D map: one row of KSB * sb_words words per 16-row block, box {sb_words, 8} = one k super-block of
+// a tile's 8 row blocks; row blocks beyond N are zero-filled
+static int make_words_map(CUtensorMap* tmap, const QuipLinearDesc* d) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) {
+    set_error("cuTensorMapEncodeTiled is not available from the driver");
+    return QUIP_ERR_CUDA;
+  }
+  const int sbw = sb_words(d->bits);
+  cuuint64_t dims[2] = {(cuuint64_t)(d->K / SB_K) * sbw, (cuuint64_t)(d->N / SB_ROWS)};
+  cuuint64_t strides[1] = {dims[0] * sizeof(uint32_t)};
+  cuuint32_t box[2] = {(cuuint32_t)sbw, (cuuint32_t)(TC_BM / SB_ROWS)};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(tmap, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void*)d->qweight, dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled (packed words) failed with CUresult %d (N=%d K=%d bits=%d)", (int)r, d->N, d->K,
+              d->bits);
+    return QUIP_ERR_CUDA;
+  }
+  return QUIP_OK;
+}
+
 template <int BITS, int BN>
 static int launch_tc(const QuipLinearDesc* d, const __half* x, const float* xsum, const __half* bias, __half* z,
                      int M, cudaStream_t s) {
-  using C = TcCfg<BN>;
-  CUtensorMap tmap;
-  if (int e = make_act_map(&tmap, x, M, d->K, BN)) return e;
+  using C = TcCfg<BITS, BN, false>;
+  CUtensorMap tmx, tmq;
+  if (int e = make_act_map(&tmx, x, M, d->K, BN)) return e;
+  if (int e = make_words_map(&tmq, d)) return e;
   auto kern = qgemm_tc_kernel<BITS, BN, false>;
   QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
   int tiles = ceil_div(d->N, TC_BM) * ceil_div(M, BN);
   int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, TC_THREADS, C::SMEM, s>>>(tmap, tmap, reinterpret_cast<const uint32_t*>(d->qweight), d->scales, d->zeros,
-                                         bias, xsum, z, M, d->K, d->N, (d->flags & QUIP_FLAG_SYMMETRIC) ? 1 : 0, 1, 0);
+  kern<<<grid, TC_THREADS, C::SMEM, s>>>(tmx, tmq, d->scales, d->zeros, bias, xsum, z, M, d->K, d->N,
+                                         (d->flags & QUIP_FLAG_SYMMETRIC) ? 1 : 0, 1, 0);
   QUIP_LAUNCHED("qgemm_tc_kernel");
   return QUIP_OK;
 }
@@ -268,7 +355,7 @@ static int launch_tc(const QuipLinearDesc* d, const __half* x, const float* xsum
 // block-diagonal pass with big contiguous blocks on the tensor cores (see DENSE in the kernel)
 template <int BN>
 static int launch_tc_dense(const QuipPass* ps, const __half* in, __half* out, int M, int n, cudaStream_t s) {
-  using C = TcCfg<BN>;
+  using C = TcCfg<2, BN, true>;
   PFN_encodeTiled enc = get_encode();
   CUtensorMap tmx, tma;
   if (int e = make_act_map(&tmx, in, M, n, TC_BM)) return e;       // 128 tokens per tile (MMA M)
@@ -288,7 +375,7 @@ static int launch_tc_dense(const QuipPass* ps, const __half* in, __half* out, in
   QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
   int tiles = ceil_div(p, BN) * ceil_div(M, TC_BM) * ps->nblk;
   int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, TC_THREADS, C::SMEM, s>>>(tmx, tma, nullptr, nullptr, nullptr, nullptr, nullptr, out, M, p, p, 1,
+  kern<<<grid, TC_THREADS, C::SMEM, s>>>(tmx, tma, nullptr, nullptr, nullptr, nullptr, out, M, p, p, 1,
                                          ps->nblk, ps->shared ? 1 : 0);
   QUIP_LAUNCHED("qgemm_tc_kernel<dense>");
   return QUIP_OK;
@@ -302,7 +389,8 @@ int pass_big_tc(const QuipPass* ps, const __half* in, __half* out, int64_t M, in
 
 int qgemm_tc(const QuipLinearDesc* d, const __half* x, const float* xsum, const __half* bias, __half* z, int M,
              cudaStream_t s) {
-  QUIP_CHECK_ARG(((uintptr_t)x & 15) == 0, "tensor-core path needs 16-byte aligned activations");
+  QUIP_CHECK_ARG((((uintptr_t)x | (uintptr_t)d->qweight) & 15) == 0,
+                 "tensor-core path needs 16-byte aligned activations and packed words");
   const bool wide = M > 64;
 #define QUIP_TC(B)                                                            \
   if (d->bits == B)                                                           \
