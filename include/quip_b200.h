@@ -135,6 +135,21 @@ int quip_silu_mul(const void* gate, const void* up, void* out, int64_t n, void* 
 int quip_silu_mul_gather(const void* gate, const void* up, const uint32_t* idx, void* out, int64_t rows, int32_t n,
                          void* stream);
 
+/* One decode-attention step for B sequences, each at its own position, on one layer of the static KV cache.
+ *   q (B, nh, hd) fp16 with rotary applied; k_new / v_new (B, nkv, hd) fp16: this step's key / value;
+ *   k_cache / v_cache (B, nkv, max_len, hd) fp16; positions (B) int64 on the device; out (B, nh, hd) fp16.
+ * Writes k_new / v_new at slot positions[b] and returns
+ *   out[b][h] = softmax_j(scale * q[b][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b],  G = nh / nkv,
+ * reading no slot past positions[b].  fp32 scores, softmax and P.V; one fp16 rounding of the output.  The launch grid
+ * depends on (B, nkv, max_len) only, so one captured graph serves every position.  hd in {64, 128}, nh % nkv == 0,
+ * nh / nkv <= 8; all pointers 16-byte aligned; fp32 scratch from quip_decode_attention_workspace_bytes.  A position
+ * outside [0, max_len) leaves the cache untouched and gives a NaN output row.  Deterministic: bit-identical results from
+ * run to run and for every other content of the other rows. */
+int quip_decode_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                          const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
+                          int32_t max_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+int quip_decode_attention_workspace_bytes(int32_t B, int32_t nh, int32_t hd, int32_t max_len, size_t* out_bytes);
+
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout
  * (bits 3: int32 (K*3/32, N) as Quant3Linear.pack writes it; bits 4: (K/8, N); bits 2: (K/16, N)):

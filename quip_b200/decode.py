@@ -13,6 +13,9 @@ The decoder layers' own modules are reused (input_layernorm, the seven QuantLine
 post_attention_layernorm, final norm, lm_head): same weights, same kernels as `model(...)`; only the glue
 between them is restated.  Llama (MHA or GQA; torch glue or the kernels of csrc/glue.cu) and OPT (the model benchmark() is
 written for, opt.py:431-482: learned positions, LayerNorm with bias, ReLU MLP; torch glue).
+
+`PromptDecoder` is the same step with one position per row and the attention of csrc/attn_decode.cu, filled from a batch
+of prompts by the model's own many-token forward; `generate` runs it greedily from a CUDA graph.
 """
 import math
 
@@ -103,6 +106,35 @@ class GraphDecoder:
         self.k_cache.zero_()
         self.v_cache.zero_()
 
+    # ---- the two seams of a step: which positions it is at, and appending k / v then attending.  This class keeps every
+    # row at one position; PromptDecoder gives each row its own.
+
+    def _step_positions(self):
+        """Position of the step: (1,) (every row at the same position) or (B,); indexes the rotary rows and OPT's
+        learned position table."""
+        return self.position
+
+    def _attn_mask(self, pos):
+        """Boolean mask over the cache slots for _attend, broadcast over rows and heads."""
+        return (self._arange <= pos)[None, None, None, :]                                  # (1, 1, 1, max_len)
+
+    def _attend(self, li, q, k, v, mask, scale):
+        """Append k, v (B, nkv, 1, hd) at the step's position of layer li's cache, attend q (B, nh, 1, hd) over the cache
+        under mask: (B, 1, nh * hd)."""
+        B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
+        pos = self.position
+        self.k_cache[li].index_copy_(2, pos, k)
+        self.v_cache[li].index_copy_(2, pos, v)
+        kk, vv = self.k_cache[li], self.v_cache[li]
+        if nkv != nh:
+            kk = kk.repeat_interleave(nh // nkv, dim=1)
+            vv = vv.repeat_interleave(nh // nkv, dim=1)
+        o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
+        return o.transpose(1, 2).reshape(B, 1, nh * hd)
+
+    def _advance(self):
+        self.position.add_(1)
+
     # ---- the layers of the stage, three kinds of glue.  Each takes the hidden state entering the stage and returns
     # (h, pend): the residual stream and a branch output still to be added to it (None when already added).
 
@@ -111,11 +143,11 @@ class GraphDecoder:
     def _layers_fused(self, h):
         ops = self.ops
         B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
-        pos = self.position
+        pos = self._step_positions()
         h = h.contiguous()
         cos = self.cos.index_select(0, pos).expand(B, hd).contiguous()                     # one row per sequence
         sin = self.sin.index_select(0, pos).expand(B, hd).contiguous()
-        mask = (self._arange <= pos)[None, None, None, :]
+        mask = self._attn_mask(pos)
         pend = None
         for li, layer in enumerate(self.layers):
             a, mlp = layer.self_attn, layer.mlp
@@ -126,15 +158,8 @@ class GraphDecoder:
                 h, x = ops.rmsnorm(h, n1.weight, n1.variance_epsilon, residual=pend)
             q, k, v = self._parallel(x, [a.q_proj, a.k_proj, a.v_proj])
             ops.rope_(q, k, cos, sin, hd)
-            self.k_cache[li].index_copy_(2, pos, k.view(B, 1, nkv, hd).transpose(1, 2))
-            self.v_cache[li].index_copy_(2, pos, v.view(B, 1, nkv, hd).transpose(1, 2))
-            kk, vv = self.k_cache[li], self.v_cache[li]
-            if nkv != nh:
-                kk = kk.repeat_interleave(nh // nkv, dim=1)
-                vv = vv.repeat_interleave(nh // nkv, dim=1)
-            o = F.scaled_dot_product_attention(q.view(B, 1, nh, hd).transpose(1, 2), kk, vv, attn_mask=mask,
-                                               scale=1.0 / math.sqrt(hd))
-            o = o.transpose(1, 2).reshape(B, 1, nh * hd)
+            o = self._attend(li, q.view(B, 1, nh, hd).transpose(1, 2), k.view(B, 1, nkv, hd).transpose(1, 2),
+                             v.view(B, 1, nkv, hd).transpose(1, 2), mask, 1.0 / math.sqrt(hd))
             h, x = ops.rmsnorm(h, n2.weight, n2.variance_epsilon, residual=a.o_proj(o))
             gate, up = self._parallel(x, [mlp.gate_proj, mlp.up_proj])
             pend = mlp.down_proj(ops.silu_mul(gate, up))
@@ -142,10 +167,10 @@ class GraphDecoder:
 
     def _layers_llama(self, h):
         B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
-        pos = self.position
-        cos = self.cos.index_select(0, pos)[None, None]                                    # (1, 1, 1, hd)
-        sin = self.sin.index_select(0, pos)[None, None]
-        mask = (self._arange <= pos)[None, None, None, :]                                  # (1, 1, 1, max_len)
+        pos = self._step_positions()
+        cos = self.cos.index_select(0, pos)[:, None, None]                                 # (1 or B, 1, 1, hd)
+        sin = self.sin.index_select(0, pos)[:, None, None]
+        mask = self._attn_mask(pos)
         for li, layer in enumerate(self.layers):
             a = layer.self_attn
             x = layer.input_layernorm(h)
@@ -155,14 +180,7 @@ class GraphDecoder:
             v = v.view(B, 1, nkv, hd).transpose(1, 2)
             q = q * cos + _rotate_half(q) * sin
             k = k * cos + _rotate_half(k) * sin
-            self.k_cache[li].index_copy_(2, pos, k)
-            self.v_cache[li].index_copy_(2, pos, v)
-            kk, vv = self.k_cache[li], self.v_cache[li]
-            if nkv != nh:
-                kk = kk.repeat_interleave(nh // nkv, dim=1)
-                vv = vv.repeat_interleave(nh // nkv, dim=1)
-            o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=1.0 / math.sqrt(hd))
-            o = o.transpose(1, 2).reshape(B, 1, nh * hd)
+            o = self._attend(li, q, k, v, mask, 1.0 / math.sqrt(hd))
             h = h + a.o_proj(o)
             x = layer.post_attention_layernorm(h)
             mlp = layer.mlp
@@ -174,17 +192,14 @@ class GraphDecoder:
     # biases live inside the (Quant)Linear modules
     def _layers_opt(self, h):
         B, nh, hd = self.batch, self.nh, self.hd
-        pos = self.position
-        mask = (self._arange <= pos)[None, None, None, :]
+        mask = self._attn_mask(self._step_positions())
         for li, layer in enumerate(self.layers):
             a, before = layer.self_attn, layer.do_layer_norm_before
             x = layer.self_attn_layer_norm(h) if before else h
             q, k, v = self._parallel(x, [a.q_proj, a.k_proj, a.v_proj])
             q = (q * a.scaling).view(B, 1, nh, hd).transpose(1, 2)                         # scaled first, as the HF module does
-            self.k_cache[li].index_copy_(2, pos, k.view(B, 1, nh, hd).transpose(1, 2))
-            self.v_cache[li].index_copy_(2, pos, v.view(B, 1, nh, hd).transpose(1, 2))
-            o = F.scaled_dot_product_attention(q, self.k_cache[li], self.v_cache[li], attn_mask=mask, scale=1.0)
-            h = h + a.out_proj(o.transpose(1, 2).reshape(B, 1, nh * hd))
+            o = self._attend(li, q, k.view(B, 1, nh, hd).transpose(1, 2), v.view(B, 1, nh, hd).transpose(1, 2), mask, 1.0)
+            h = h + a.out_proj(o)
             if not before:
                 h = layer.self_attn_layer_norm(h)
             x = layer.final_layer_norm(h) if before else h
@@ -201,7 +216,7 @@ class GraphDecoder:
         h = d.embed_tokens(self.tokens)[:, None, :]
         if d.project_in is not None:
             h = d.project_in(h)
-        return h + F.embedding(self.position + d.embed_positions.offset, d.embed_positions.weight)[None]
+        return h + F.embedding(self._step_positions() + d.embed_positions.offset, d.embed_positions.weight)[:, None]
 
     def _head(self, h, pend):
         """Final norm (fused with the pending residual add on the glue-kernel path) -> lm_head: logits (B, vocab)."""
@@ -232,7 +247,7 @@ class GraphDecoder:
             self.logits = self._head(h, pend)
         else:
             self.h_out.copy_(h if pend is None else h + pend)   # fp16 add: the rounding the fused residual add performs
-        self.position.add_(1)
+        self._advance()
 
     def capture(self):
         """Record one step.  The cache and position are restored afterwards, so capture is side-effect free."""
@@ -240,21 +255,36 @@ class GraphDecoder:
         for mod in self.model.modules():                   # sibling groups launch on side streams: not while capturing
             if isinstance(mod, QuantLinear) and getattr(mod, '_group', None) is not None:
                 raise RuntimeError('dissolve the sibling groups (quant.SiblingGroup.dissolve) before capturing')
-        pos0, k0, v0 = self.position.clone(), self.k_cache.clone(), self.v_cache.clone()
+        state = self._capture_state()
+        saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.no_grad(), torch.cuda.stream(side):
-            for _ in range(2):                             # lazy set-up (descriptors, workspaces) outside the graph
-                self._step()
-            self.position.copy_(pos0)
+            self._warm_up(state, saved)
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph, stream=side, capture_error_mode='thread_local'):
                 self._step()
         torch.cuda.current_stream(self.dev).wait_stream(side)
-        self.position.copy_(pos0)
-        self.k_cache.copy_(k0)
-        self.v_cache.copy_(v0)
+        for t, t0 in zip(state, saved):
+            t.copy_(t0)
         return self
+
+    def _capture_state(self):
+        """The buffers a step changes, which capture() puts back after its warm-up steps."""
+        return [self.position, self.k_cache, self.v_cache]
+
+    def _warm_up(self, state, saved):
+        """Two eager steps for the lazy set-up (descriptors, workspaces) outside the graph.  Each starts from the saved
+        state with the step counters brought into range (a decoder may be captured with its cache full) and is undone
+        afterwards, so no index a warm-up step uses can leave its table."""
+        for _ in range(2):
+            self._counters_in_range()
+            self._step()
+            for t, t0 in zip(state, saved):
+                t.copy_(t0)
+
+    def _counters_in_range(self):
+        self.position.clamp_(max=self.max_len - 1)
 
     def step(self, tokens):
         """tokens (B,) -> logits (B, vocab) for the next position; advances the cache."""
@@ -308,3 +338,175 @@ def graph_decode_throughput(model, batch, steps=32, max_len=64, seed=0):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
     return batch * 1e3 / ms, ms
+
+
+class PromptDecoder(GraphDecoder):
+    """GraphDecoder with one position per row, so prompts of different lengths share a batch.
+
+      * `positions` (B,) on the device, advanced inside the graph: rotary rows cos[positions], OPT's learned position
+        looked up per row;
+      * attention on CUDA is quip_decode_attention (csrc/attn_decode.cu): k / v appended at positions[b] inside the
+        kernel, slots 0 .. positions[b] read and no others, GQA without copies.  On the CPU the same step in torch:
+        per-row scatter into the cache, SDPA under the mask arange(max_len) <= positions[:, None];
+      * `prefill` fills the cache from a batch of prompts with the model's own many-token forward;
+      * max_new > 0: greedy selection inside the step -- tokens = argmax(logits), stored in generated[:, t] -- so a
+        host loop only replays the graph.
+    The whole model, no layer pipeline."""
+
+    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None):
+        super().__init__(model, max_len=max_len, batch=batch, ops=ops)
+        B = self.batch
+        self.positions = torch.zeros(B, dtype=torch.long, device=self.dev)
+        self.max_new = int(max_new)
+        self.generated = torch.zeros(B, max(self.max_new, 1), dtype=torch.long, device=self.dev)
+        self._t = torch.zeros(1, dtype=torch.long, device=self.dev)
+        self._rows = torch.arange(B, device=self.dev)
+        self._pos_host = [0] * B
+        self._t_host = 0
+        self._kernel = self.dev.type == 'cuda'
+
+    def _step_positions(self):
+        return self.positions
+
+    def _attn_mask(self, pos):
+        return None if self._kernel else (self._arange[None] <= pos[:, None])[:, None, None, :]     # (B, 1, 1, max_len)
+
+    def _attend(self, li, q, k, v, mask, scale):
+        B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
+        if self._kernel:
+            from . import fused
+            o = fused.decode_attention(q.reshape(B, nh, hd).contiguous(), k.reshape(B, nkv, hd).contiguous(),
+                                       v.reshape(B, nkv, hd).contiguous(), self.k_cache[li], self.v_cache[li],
+                                       self.positions, scale)
+            return o.view(B, 1, nh * hd)
+        self.k_cache[li][self._rows, :, self.positions] = k[:, :, 0]
+        self.v_cache[li][self._rows, :, self.positions] = v[:, :, 0]
+        kk, vv = self.k_cache[li], self.v_cache[li]
+        if nkv != nh:
+            kk = kk.repeat_interleave(nh // nkv, dim=1)
+            vv = vv.repeat_interleave(nh // nkv, dim=1)
+        o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
+        return o.transpose(1, 2).reshape(B, 1, nh * hd)
+
+    def _advance(self):
+        self.positions.add_(1)
+        if self.max_new:
+            self.tokens.copy_(self.logits.argmax(-1))
+            self.generated.index_copy_(1, self._t, self.tokens[:, None])
+            self._t.add_(1)
+
+    def _capture_state(self):
+        # Not the cache: a warm-up step writes slot positions[b] (clamped to max_len - 1), and a later step writes that
+        # slot before it reads it.  A row clamped from max_len takes no further step: its cache is full.
+        return [self.positions, self.tokens, self._t, self.generated]
+
+    def _counters_in_range(self):
+        self.positions.clamp_(max=self.max_len - 1)
+        self._t.clamp_(max=self.generated.shape[1] - 1)
+
+    def reset(self):
+        """Back to an empty cache: every row at position 0, nothing generated."""
+        super().reset()
+        self.positions.zero_()
+        self._t.zero_()
+        self.generated.zero_()
+        self._pos_host = [0] * self.batch
+        self._t_host = 0
+
+    def prefill(self, prompts):
+        """Fill the cache from `prompts` (B 1-D id tensors): right-padded to the longest, run through the model's own
+        forward (`model.model(ids, attention_mask=..., use_cache=True)`, the packed linears at M = B * P), its keys and
+        values copied to the cache slots 0 .. P-1.  Slots past a row's length hold padding; the step overwrites them in
+        turn and never reads past positions[b].  Returns the logits after each prompt's last token (B, vocab); with
+        max_new > 0 their argmax is the first generated token and the next step's input."""
+        B = self.batch
+        if len(prompts) != B:
+            raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
+        lens = [int(p.numel()) for p in prompts]
+        if min(lens) < 1:
+            raise ValueError('empty prompt')
+        P = max(lens)
+        if P > self.max_len:
+            raise ValueError(f'a prompt of {P} tokens does not fit a cache of {self.max_len} positions')
+        ids = torch.zeros(B, P, dtype=torch.long, device=self.dev)
+        for b, p in enumerate(prompts):
+            ids[b, :lens[b]] = p.reshape(-1).to(self.dev)
+        lens_t = torch.tensor(lens, dtype=torch.long, device=self.dev)
+        attn = (torch.arange(P, device=self.dev)[None] < lens_t[:, None]).long()
+        with torch.no_grad():
+            out = self.model.model(input_ids=ids, attention_mask=attn, use_cache=True)
+            cache = out.past_key_values
+            for li in range(len(self.layers)):
+                self.k_cache[li, :, :, :P].copy_(cache.layers[li].keys)
+                self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
+            logits = self.model.lm_head(out.last_hidden_state[self._rows, lens_t - 1])     # last real token per row
+            self.positions.copy_(lens_t)
+            self._pos_host = list(lens)
+            if self.max_new:
+                self.tokens.copy_(logits.argmax(-1))
+                self.generated[:, 0].copy_(self.tokens)
+                self._t.fill_(1)
+                self._t_host = 1
+        return logits
+
+    def step(self, tokens=None):
+        """One step at every row's own position: tokens (B,) -- or, when generating, the tokens the previous step
+        selected -- to logits (B, vocab); advances every row."""
+        if max(self._pos_host) >= self.max_len:
+            raise ValueError(f'KV cache of {self.max_len} positions is full')
+        if self.max_new and self._t_host >= self.max_new:
+            raise ValueError(f'{self.max_new} tokens generated already')
+        self._pos_host = [p + 1 for p in self._pos_host]
+        self._t_host += 1 if self.max_new else 0
+        if tokens is not None:
+            self.tokens.copy_(tokens.reshape(-1))
+        if self.graph is None:
+            with torch.no_grad():
+                self._step()
+        else:
+            self.graph.replay()
+        return self.logits
+
+
+EOS_CHECK_EVERY = 16
+
+
+def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None):
+    """Greedy continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of
+    new token ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled
+    in one many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
+    max_len (default: longest prompt + max_new_tokens) is the KV cache length.  Stops early once every row has produced
+    an EOS, checked every EOS_CHECK_EVERY steps."""
+    prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
+    max_new_tokens = int(max_new_tokens)
+    if not prompts:
+        raise ValueError('no prompts')
+    if max_new_tokens < 1:
+        raise ValueError(f'max_new_tokens must be at least 1, got {max_new_tokens}')
+    lens = [p.numel() for p in prompts]
+    if min(lens) == 0:
+        raise ValueError('empty prompt')
+    max_len = max(lens) + max_new_tokens if max_len is None else int(max_len)
+    if max(lens) + max_new_tokens > max_len:
+        raise ValueError(f'a prompt of {max(lens)} tokens plus {max_new_tokens} new ones exceeds max_len {max_len}')
+    cfg = model.config
+    if cfg.model_type == 'opt' and max_len > cfg.max_position_embeddings:
+        raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the model')
+    eos = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
+                                           [int(e) for e in eos_token_id])
+    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens)
+    if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
+        dec.capture()
+    dec.prefill(prompts)
+    eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
+    n = 1
+    while n < max_new_tokens:
+        if eos and n % EOS_CHECK_EVERY == 0 and bool(torch.isin(dec.generated[:, :n], eos_t).any(1).all()):
+            break
+        dec.step()
+        n += 1
+    out = []
+    for row in dec.generated[:, :n].cpu():
+        hit = torch.isin(row, eos_t.cpu()).nonzero()
+        out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+    return out

@@ -88,6 +88,43 @@ class CudaGlue:
         return out
 
 
+def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale):
+    """quip_decode_attention on torch tensors: append k_new / v_new (B, nkv, hd) at slot positions[b] of one layer's
+    k_cache / v_cache (B, nkv, max_len, hd) and attend q (B, nh, hd) over slots 0 .. positions[b].  fp16, CUDA,
+    contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream."""
+    ts = (q, k_new, v_new, k_cache, v_cache)
+    for t in ts + (positions,):
+        if not t.is_cuda:
+            raise RuntimeError('decode_attention runs on a CUDA device only (there is no CPU fallback)')
+        if t.device != q.device:
+            raise ValueError('decode_attention: all tensors must be on one device')
+        if not t.is_contiguous():
+            raise ValueError('decode_attention takes contiguous tensors')
+    if any(t.dtype != torch.float16 for t in ts) or positions.dtype != torch.int64:
+        raise ValueError('decode_attention takes fp16 q / k / v / caches and int64 positions')
+    if q.dim() != 3 or k_cache.dim() != 4:
+        raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
+                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
+    B, nh, hd = q.shape
+    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
+    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+            tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,)):
+        raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
+                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
+                         f'{tuple(positions.shape)} do not agree')
+    lib = _lib.load()
+    need = C.c_size_t(0)
+    _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
+    ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
+    out = torch.empty_like(q)
+    with torch.cuda.device(q.device):
+        _lib.check(lib.quip_decode_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                             v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh, nkv, hd,
+                                             max_len, C.c_float(scale), ws.data_ptr(), ws.numel(),
+                                             torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
 def mlp_layout_plan(mlp):
     """The combined index of the three permutations around SiLU(gate) * up of a packed Llama MLP -- the output gathers of
     gate_proj / up_proj (y[j] = layout[u_idx[j]]) and the input gather of down_proj (layout[l] = x[v_idx[l]]) -- so that one
