@@ -150,6 +150,24 @@ int quip_decode_attention(const void* q, const void* k_new, const void* v_new, v
                           int32_t max_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
 int quip_decode_attention_workspace_bytes(int32_t B, int32_t nh, int32_t hd, int32_t max_len, size_t* out_bytes);
 
+/* The same step on an e4m3 KV cache: k_cache / v_cache (B, nkv, max_len, hd) e4m3fn bytes, k_scale / v_scale
+ * (B, nkv, max_len) fp32, one scale per cached head vector x (hd values):
+ *   amax = max_i |x_i|;  s = amax / 448 (IEEE fp32 division; s = 1 when amax == 0);  q_i = e4m3fn(x_i / s), round to
+ *   nearest even, subnormals kept;  the vector's value is float(q_i) * s.
+ * k_new / v_new (fp16) are quantized so, written with their scales at slot positions[b], and attended over as quantized
+ * values like every other slot 0 .. positions[b].  No slot or scale past positions[b] is read.  Same grid, workspace
+ * (quip_decode_attention_workspace_bytes) and determinism as quip_decode_attention; the scale pointers 4-byte aligned.
+ * Non-finite inputs may give a NaN output row. */
+int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                              float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
+                              int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
+                              size_t workspace_bytes, void* stream);
+/* Prefill of an e4m3 cache: src (B, nkv, P, hd) fp16 quantized as above into slots 0 .. P-1 of cache
+ * (B, nkv, max_len, hd) e4m3fn and scales (B, nkv, max_len) fp32; slots >= P are not touched.  hd in {64, 128},
+ * P <= max_len; src and cache 16-byte aligned, scales 4-byte aligned. */
+int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,
+                         int32_t max_len, int32_t hd, void* stream);
+
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout
  * (bits 3: int32 (K*3/32, N) as Quant3Linear.pack writes it; bits 4: (K/8, N); bits 2: (K/16, N)):

@@ -1,5 +1,5 @@
 // Decode attention: one new token per sequence, each sequence at its own position, over the static KV cache of
-// quip_b200/decode.py (one layer: k_cache / v_cache (B, nkv, max_len, hd) fp16).
+// quip_b200/decode.py (one layer: k_cache / v_cache (B, nkv, max_len, hd), fp16 or e4m3 with per-slot fp32 scales).
 //
 //   o[b][h] = softmax_j(scale * q[b][h] . K[b][h/G][j]) V[b][h/G][j],   j = 0 .. positions[b],   G = nh / nkv
 //
@@ -23,7 +23,23 @@
 // and row b's result does not depend on the other rows.
 //
 // A position outside [0, max_len) is not looked at by the main kernel (no slot is written) and gives a NaN output row.
+//
+// e4m3 cache (quip_decode_attention_fp8, the same kernel instantiated for FP8).  Each cached head vector x (the hd
+// values of one layer, row, kv head and slot; fp32 from fp16) is stored as hd e4m3fn bytes q plus one fp32 scale s:
+//
+//   amax = max_i |x_i|;   s = amax / 448 (IEEE fp32 division), s = 1 when amax == 0;   q_i = e4m3fn_rn(x_i / s)
+//
+// round to nearest even, subnormals kept, IEEE division (the build has no fast-math).  |x_i / s| < 464, so the saturating
+// cvt.rn.satfinite.e4m3x2.f32 and a non-saturating conversion (torch's .to(torch.float8_e4m3fn)) give the same bytes.  The
+// value of a slot is float(q_i) * s.  The appending CTA quantizes k_new / v_new (one warp each) and attends over the
+// quantized values of its own slot too, so a step's result equals what every later step reads back.  Scores are
+// s_k[j] * scale * sum_i q_i k8_i, P.V weights are p_j * s_v[j]: one multiply per slot, not per element.  The lanes of a
+// slot are the fp16 kernel's (8 elements each), with 8-byte loads and AD_U8 = 8 loads in flight per lane, so a lane has
+// the same 64 bytes in flight and the same q registers.  A cached slot costs hd + 4 bytes instead of 2 * hd.
+#include <cuda_fp8.h>
 #include <math.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -35,8 +51,10 @@ constexpr int AD_CHUNK = 128;        // KV slots per CTA (at most)
 constexpr int AD_SMALL_CHUNK = 64;   // when B * nkv * ceil(max_len / AD_CHUNK) < AD_SMALL_GRID
 constexpr int AD_SMALL_GRID = 2 * 132;
 constexpr int AD_U = 4;              // slots per slot group whose loads are in flight together
+constexpr int AD_U8 = 8;             // the same for the e4m3 cache (8-byte loads)
 constexpr int AD_THREADS = 128;
 constexpr int AD_MAXG = 8;           // query heads per kv head
+constexpr float E4M3_MAX = 448.f;
 
 union AH8 {
   uint4 v;
@@ -54,18 +72,81 @@ __device__ __forceinline__ void h8_to_f(const uint4& u, float (&f)[8]) {
   }
 }
 
+// 8 e4m3 bytes (element i in byte i) -> fp32, through cvt.rn.f16x2.e4m3x2 (exact: every e4m3 value is an fp16 value)
+__device__ __forceinline__ void e4m3x8_to_f(const uint2& u, float (&f)[8]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t w = i < 2 ? u.x : u.y;
+    const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)((w >> (16 * (i & 1))) & 0xFFFFu), __NV_E4M3);
+    const float2 p = __half22float2(__half2(r));
+    f[2 * i] = p.x;
+    f[2 * i + 1] = p.y;
+  }
+}
+
+// One warp quantizes the head vector x (HD fp16 values): lane l takes elements l*HD/32 .. (l+1)*HD/32 - 1 and returns
+// their e4m3 bytes (element l*HD/32 + i in byte i); every lane gets the scale.
+template <int HD>
+__device__ __forceinline__ uint32_t e4m3_quantize_warp(const __half* __restrict__ x, int lane, float& s) {
+  constexpr int E = HD / 32;   // 2 or 4
+  float f[E];
+  const __half2* x2 = reinterpret_cast<const __half2*>(x) + lane * (E / 2);
+#pragma unroll
+  for (int i = 0; i < E / 2; ++i) {
+    const float2 p = __half22float2(x2[i]);
+    f[2 * i] = p.x;
+    f[2 * i + 1] = p.y;
+  }
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < E; ++i) amax = fmaxf(amax, fabsf(f[i]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  s = amax == 0.f ? 1.f : amax / E4M3_MAX;
+  uint32_t w = 0;
+#pragma unroll
+  for (int i = 0; i < E / 2; ++i) {
+    const __nv_fp8x2_storage_t p =
+        __nv_cvt_float2_to_fp8x2(make_float2(f[2 * i] / s, f[2 * i + 1] / s), __NV_SATFINITE, __NV_E4M3);
+    w |= (uint32_t)p << (16 * i);
+  }
+  return w;
+}
+
+// the bytes of e4m3_quantize_warp to the HD-byte slot dst
+template <int HD>
+__device__ __forceinline__ void e4m3_store_warp(uint8_t* dst, int lane, uint32_t w) {
+  if constexpr (HD == 128) reinterpret_cast<uint32_t*>(dst)[lane] = w;
+  else reinterpret_cast<uint16_t*>(dst)[lane] = (uint16_t)w;
+}
+
+// Shared memory of the e4m3 instantiation: the chunk's slot scales and the appended slot (bytes and scale, k then v).
+template <bool FP8, int HD>
+struct AttnFp8Smem {
+  float ks[AD_CHUNK], vs[AD_CHUNK];
+  alignas(16) uint8_t q[2][HD];
+  float qs[2];
+};
+template <int HD>
+struct AttnFp8Smem<false, HD> {};
+
 // Partials: o  [B][nh][nsplit][HD] fp32, then ml [B][nh][nsplit][2] fp32 (running max, sum of exp).
-template <int HD, int G>
+// FP8: kc / vc hold e4m3 bytes with one fp32 scale per slot in ksc / vsc (same (row, slot) index); fp16: ksc / vsc unused.
+template <bool FP8, int HD, int G>
 __global__ void __launch_bounds__(AD_THREADS)
 attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict__ k_new, const __half* __restrict__ v_new,
-                         __half* __restrict__ kc, __half* __restrict__ vc, const int64_t* __restrict__ positions,
-                         float* __restrict__ part_o, float* __restrict__ part_ml, int nh, int nkv, int max_len,
-                         int nsplit, int chunk, float scale) {
-  constexpr int LPS = HD / 8;                 // lanes per slot: 8 fp16 (16 bytes) per lane
+                         void* __restrict__ kc, void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
+                         const int64_t* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml,
+                         int nh, int nkv, int max_len, int nsplit, int chunk, float scale) {
+  using CT = std::conditional_t<FP8, uint8_t, __half>;   // cache element
+  using LT = std::conditional_t<FP8, uint2, uint4>;      // a lane's 8 elements of a slot
+  constexpr int U = FP8 ? AD_U8 : AD_U;
+  constexpr int LPS = HD / 8;                 // lanes per slot: 8 elements (16 bytes fp16, 8 bytes e4m3) per lane
   constexpr int SG = AD_THREADS / LPS;        // slot groups of the CTA
   constexpr int NW = AD_THREADS / 32;
-  __shared__ float sc[G][AD_CHUNK];           // scores, then exp(score - m)
+  __shared__ float sc[G][AD_CHUNK];           // scores, then exp(score - m) (times s_v for FP8)
   __shared__ float red[NW][G][HD];            // per-warp P.V partials
+  __shared__ AttnFp8Smem<FP8, HD> f8;
 
   const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int64_t pos = positions[b];
@@ -79,9 +160,28 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   const int64_t row = (int64_t)b * nkv + kvh;
   const __half* kn = k_new + row * HD;
   const __half* vn = v_new + row * HD;
-  __half* kr = kc + row * (int64_t)max_len * HD;
-  __half* vr = vc + row * (int64_t)max_len * HD;
-  if (rel < chunk && tid < 2 * LPS) {      // append: this CTA owns slot pos
+  CT* kr = reinterpret_cast<CT*>(kc) + row * (int64_t)max_len * HD;
+  CT* vr = reinterpret_cast<CT*>(vc) + row * (int64_t)max_len * HD;
+  float ks = 0.f, vs = 0.f;                   // FP8: the scales of slot start + tid, in flight during the scores
+  if constexpr (FP8) {
+    if (tid < n && tid != rel) {
+      ks = ksc[row * max_len + start + tid];
+      vs = vsc[row * max_len + start + tid];
+    }
+    if (rel < chunk) {                        // append: this CTA owns slot pos; warp 0 quantizes k_new, warp 1 v_new
+      if (warp < 2) {
+        float s;
+        const uint32_t w = e4m3_quantize_warp<HD>(warp ? vn : kn, lane, s);
+        e4m3_store_warp<HD>((warp ? vr : kr) + pos * HD, lane, w);
+        e4m3_store_warp<HD>(f8.q[warp], lane, w);
+        if (lane == 0) {
+          (warp ? vsc : ksc)[row * max_len + pos] = s;
+          f8.qs[warp] = s;
+        }
+      }
+      __syncthreads();
+    }
+  } else if (rel < chunk && tid < 2 * LPS) {  // append: this CTA owns slot pos
     const int c = tid % LPS;
     if (tid < LPS) reinterpret_cast<uint4*>(kr + pos * HD)[c] = reinterpret_cast<const uint4*>(kn)[c];
     else reinterpret_cast<uint4*>(vr + pos * HD)[c] = reinterpret_cast<const uint4*>(vn)[c];
@@ -94,20 +194,32 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   for (int g = 0; g < G; ++g) h8_to_f(__ldg(reinterpret_cast<const uint4*>(qh + g * HD) + sl), qf[g]);
 
   // scores: slot group sg takes slots sg, sg + SG, ...; all lanes run the same trip count (the shuffles are warp-wide).
-  // AD_U loads are issued before any of them is used; a slot index past n loads slot n - 1 again (valid, discarded).
-  for (int jb = 0; jb < n; jb += AD_U * SG) {
-    uint4 raw[AD_U];
+  // U loads are issued before any of them is used; a slot index past n loads slot n - 1 again (valid, discarded).
+  // FP8: the appended slot is read from shared memory (its load goes to k_new, a valid address, and is discarded).
+  for (int jb = 0; jb < n; jb += U * SG) {
+    LT raw[U];
 #pragma unroll
-    for (int u = 0; u < AD_U; ++u) {
+    for (int u = 0; u < U; ++u) {
       const int j = min(jb + u * SG + sg, n - 1);
-      const __half* src = j == rel ? kn : kr + (int64_t)(start + j) * HD;
-      raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
+      if constexpr (FP8) {
+        const void* src = j == rel ? (const void*)kn : (const void*)(kr + (int64_t)(start + j) * HD);
+        raw[u] = ldg_nc_v2(reinterpret_cast<const uint2*>(src) + sl);
+      } else {
+        const __half* src = j == rel ? kn : kr + (int64_t)(start + j) * HD;
+        raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
+      }
     }
 #pragma unroll
-    for (int u = 0; u < AD_U; ++u) {
+    for (int u = 0; u < U; ++u) {
       const int j = jb + u * SG + sg;
       float kf[8];
-      h8_to_f(raw[u], kf);
+      if constexpr (FP8) {
+        uint2 w = raw[u];
+        if (min(j, n - 1) == rel) w = reinterpret_cast<const uint2*>(f8.q[0])[sl];
+        e4m3x8_to_f(w, kf);
+      } else {
+        h8_to_f(raw[u], kf);
+      }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         float d = 0.f;
@@ -119,18 +231,32 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
       }
     }
   }
+  if constexpr (FP8) {
+    if (tid < n) {
+      f8.ks[tid] = tid == rel ? f8.qs[0] : ks;
+      f8.vs[tid] = tid == rel ? f8.qs[1] : vs;
+    }
+  }
   __syncthreads();
 
   // chunk softmax per head: max, exp, sum (one warp per head, fixed order)
   for (int g = warp; g < G; g += NW) {
     float m = -INFINITY;
-    for (int j = lane; j < n; j += 32) m = fmaxf(m, sc[g][j]);
+    for (int j = lane; j < n; j += 32) {
+      float s = sc[g][j];
+      if constexpr (FP8) {
+        s *= f8.ks[j];
+        sc[g][j] = s;
+      }
+      m = fmaxf(m, s);
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     float l = 0.f;
     for (int j = lane; j < n; j += 32) {
       const float p = expf(sc[g][j] - m);
-      sc[g][j] = p;
+      if constexpr (FP8) sc[g][j] = p * f8.vs[j];
+      else sc[g][j] = p;
       l += p;
     }
 #pragma unroll
@@ -149,20 +275,31 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   for (int g = 0; g < G; ++g)
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[g][e] = 0.f;
-  for (int jb = 0; jb < n; jb += AD_U * SG) {
-    uint4 raw[AD_U];
+  for (int jb = 0; jb < n; jb += U * SG) {
+    LT raw[U];
 #pragma unroll
-    for (int u = 0; u < AD_U; ++u) {
+    for (int u = 0; u < U; ++u) {
       const int j = min(jb + u * SG + sg, n - 1);
-      const __half* src = j == rel ? vn : vr + (int64_t)(start + j) * HD;
-      raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
+      if constexpr (FP8) {
+        const void* src = j == rel ? (const void*)vn : (const void*)(vr + (int64_t)(start + j) * HD);
+        raw[u] = ldg_nc_v2(reinterpret_cast<const uint2*>(src) + sl);
+      } else {
+        const __half* src = j == rel ? vn : vr + (int64_t)(start + j) * HD;
+        raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
+      }
     }
 #pragma unroll
-    for (int u = 0; u < AD_U; ++u) {
+    for (int u = 0; u < U; ++u) {
       const int j = jb + u * SG + sg;
       if (j < n) {
         float vf[8];
-        h8_to_f(raw[u], vf);
+        if constexpr (FP8) {
+          uint2 w = raw[u];
+          if (j == rel) w = reinterpret_cast<const uint2*>(f8.q[1])[sl];
+          e4m3x8_to_f(w, vf);
+        } else {
+          h8_to_f(raw[u], vf);
+        }
 #pragma unroll
         for (int g = 0; g < G; ++g) {
           const float p = sc[g][j];
@@ -221,34 +358,94 @@ attn_decode_combine_kernel(const float* __restrict__ part_o, const float* __rest
   out[(int64_t)bh * hd + d] = __float2half_rn(O / L);
 }
 
-template <int HD, int G>
-void launch_split(dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
-                  const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len, int nsplit, int chunk, float scale) {
-  attn_decode_split_kernel<HD, G><<<grid, AD_THREADS, 0, st>>>((const __half*)q, (const __half*)kn, (const __half*)vn,
-                                                               (__half*)kc, (__half*)vc, pos, po, pml, nh, nkv, max_len,
-                                                               nsplit, chunk, scale);
-}
+// Prefill: one warp per head vector v = (row, p) of src (rows, P, HD) fp16 -> e4m3 slot p of cache (rows, max_len, HD)
+// and its scale; slots >= P are not touched.
+constexpr int KQ_WARPS = 8;
 
 template <int HD>
+__global__ void __launch_bounds__(KQ_WARPS * 32)
+kv_quantize_fp8_kernel(const __half* __restrict__ src, uint8_t* __restrict__ cache, float* __restrict__ scales,
+                       int64_t nvec, int P, int max_len) {
+  const int64_t v = (int64_t)blockIdx.x * KQ_WARPS + threadIdx.x / 32;
+  if (v >= nvec) return;                      // warp-uniform
+  const int lane = threadIdx.x & 31;
+  const int64_t slot = v / P * max_len + v % P;
+  float s;
+  const uint32_t w = e4m3_quantize_warp<HD>(src + v * HD, lane, s);
+  e4m3_store_warp<HD>(cache + slot * HD, lane, w);
+  if (lane == 0) scales[slot] = s;
+}
+
+template <bool FP8, int HD, int G>
+void launch_split(dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
+                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
+                  int nsplit, int chunk, float scale) {
+  attn_decode_split_kernel<FP8, HD, G><<<grid, AD_THREADS, 0, st>>>((const __half*)q, (const __half*)kn,
+                                                                    (const __half*)vn, kc, vc, ksc, vsc, pos, po, pml,
+                                                                    nh, nkv, max_len, nsplit, chunk, scale);
+}
+
+template <bool FP8, int HD>
 void launch_split_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
-                    const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len, int nsplit, int chunk, float scale) {
+                    float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
+                    int nsplit, int chunk, float scale) {
+#define AD_LAUNCH(g) \
+  launch_split<FP8, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale)
   switch (G) {
-    case 1: launch_split<HD, 1>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 2: launch_split<HD, 2>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 3: launch_split<HD, 3>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 4: launch_split<HD, 4>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 5: launch_split<HD, 5>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 6: launch_split<HD, 6>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    case 7: launch_split<HD, 7>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
-    default: launch_split<HD, 8>(grid, st, q, kn, vn, kc, vc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale); break;
+    case 1: AD_LAUNCH(1); break;
+    case 2: AD_LAUNCH(2); break;
+    case 3: AD_LAUNCH(3); break;
+    case 4: AD_LAUNCH(4); break;
+    case 5: AD_LAUNCH(5); break;
+    case 6: AD_LAUNCH(6); break;
+    case 7: AD_LAUNCH(7); break;
+    default: AD_LAUNCH(8); break;
   }
+#undef AD_LAUNCH
 }
 
 bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
 size_t ws_bytes(int64_t B, int64_t nh, int64_t hd, int64_t nsplit) {
   const size_t o = (size_t)(B * nh * nsplit * hd) * sizeof(float);
   return ((o + 255) & ~(size_t)255) + (size_t)(B * nh * nsplit * 2) * sizeof(float);
+}
+
+// Argument checks and launches of quip_decode_attention (FP8 false) and quip_decode_attention_fp8 (FP8 true); fn names
+// the entry point in the messages.
+template <bool FP8>
+int decode_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                     float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t nh,
+                     int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
+                 "%s: null pointer", fn);
+  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
+                 "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
+  QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
+                 "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head",
+                 fn, nh, nkv, AD_MAXG);
+  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache) && al16(out) && al16(workspace),
+                 "%s: pointers must be 16-byte aligned", fn);
+  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
+  const int chunk = (int64_t)B * nkv * ceil_div(max_len, AD_CHUNK) < AD_SMALL_GRID ? AD_SMALL_CHUNK : AD_CHUNK;
+  const int nsplit = ceil_div(max_len, chunk);
+  const size_t need = ws_bytes(B, nh, hd, nsplit);
+  QUIP_CHECK_ARG(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+  if (B == 0) return QUIP_OK;
+  float* po = (float*)workspace;
+  float* pml = (float*)((char*)workspace + (((size_t)B * nh * nsplit * hd * sizeof(float) + 255) & ~(size_t)255));
+  const cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(nsplit, nkv, B);
+  const int G = nh / nkv;
+  if (hd == 64) launch_split_g<FP8, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
+  else launch_split_g<FP8, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
+  QUIP_LAUNCHED("attn_decode_split_kernel");
+  attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk);
+  QUIP_LAUNCHED("attn_decode_combine_kernel");
+  return QUIP_OK;
 }
 
 }  // namespace
@@ -270,30 +467,32 @@ extern "C" int quip_decode_attention(const void* q, const void* k_new, const voi
                                      const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
                                      int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
                                      void* stream) {
-  QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace,
-                 "quip_decode_attention: null pointer");
-  QUIP_CHECK_ARG(hd == 64 || hd == 128, "quip_decode_attention: head_dim %d is not 64 or 128", hd);
-  QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
-                 "quip_decode_attention: bad sizes (B %d, nh %d, nkv %d, max_len %d)", B, nh, nkv, max_len);
-  QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
-                 "quip_decode_attention: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head",
-                 nh, nkv, AD_MAXG);
-  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache) && al16(out) && al16(workspace),
-                 "quip_decode_attention: pointers must be 16-byte aligned");
-  const int chunk = (int64_t)B * nkv * ceil_div(max_len, AD_CHUNK) < AD_SMALL_GRID ? AD_SMALL_CHUNK : AD_CHUNK;
-  const int nsplit = ceil_div(max_len, chunk);
-  const size_t need = ws_bytes(B, nh, hd, nsplit);
-  QUIP_CHECK_ARG(workspace_bytes >= need, "quip_decode_attention: workspace of %zu bytes, %zu needed", workspace_bytes, need);
-  if (B == 0) return QUIP_OK;
-  float* po = (float*)workspace;
-  float* pml = (float*)((char*)workspace + (((size_t)B * nh * nsplit * hd * sizeof(float) + 255) & ~(size_t)255));
+  return decode_attention<false>("quip_decode_attention", q, k_new, v_new, k_cache, v_cache, nullptr, nullptr, positions,
+                                 out, B, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache,
+                                         void* v_cache, float* k_scale, float* v_scale, const int64_t* positions,
+                                         void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len,
+                                         float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_attention<true>("quip_decode_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
+                                positions, out, B, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,
+                                    int32_t max_len, int32_t hd, void* stream) {
+  QUIP_CHECK_ARG(src && cache && scales, "quip_kv_quantize_fp8: null pointer");
+  QUIP_CHECK_ARG(hd == 64 || hd == 128, "quip_kv_quantize_fp8: head_dim %d is not 64 or 128", hd);
+  QUIP_CHECK_ARG(B >= 0 && nkv > 0 && P >= 0 && max_len > 0 && P <= max_len,
+                 "quip_kv_quantize_fp8: bad sizes (B %d, nkv %d, P %d, max_len %d): need P <= max_len", B, nkv, P, max_len);
+  QUIP_CHECK_ARG(al16(src) && al16(cache) && al4(scales),
+                 "quip_kv_quantize_fp8: src and cache must be 16-byte aligned, scales 4-byte aligned");
+  const int64_t nvec = (int64_t)B * nkv * P;
+  if (nvec == 0) return QUIP_OK;
+  const unsigned blocks = (unsigned)((nvec + KQ_WARPS - 1) / KQ_WARPS);
   const cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid(nsplit, nkv, B);
-  const int G = nh / nkv;
-  if (hd == 64) launch_split_g<64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
-  else launch_split_g<128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
-  QUIP_LAUNCHED("attn_decode_split_kernel");
-  attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk);
-  QUIP_LAUNCHED("attn_decode_combine_kernel");
+  if (hd == 64) kv_quantize_fp8_kernel<64><<<blocks, KQ_WARPS * 32, 0, st>>>((const __half*)src, (uint8_t*)cache, scales, nvec, P, max_len);
+  else kv_quantize_fp8_kernel<128><<<blocks, KQ_WARPS * 32, 0, st>>>((const __half*)src, (uint8_t*)cache, scales, nvec, P, max_len);
+  QUIP_LAUNCHED("kv_quantize_fp8_kernel");
   return QUIP_OK;
 }

@@ -15,7 +15,10 @@ between them is restated.  Llama (MHA or GQA; torch glue or the kernels of csrc/
 written for, opt.py:431-482: learned positions, LayerNorm with bias, ReLU MLP; torch glue).
 
 `PromptDecoder` is the same step with one position per row and the attention of csrc/attn_decode.cu, filled from a batch
-of prompts by the model's own many-token forward; `generate` runs it greedily from a CUDA graph.
+of prompts by the model's own many-token forward; `generate` runs it greedily from a CUDA graph.  With
+kv_dtype=torch.float8_e4m3fn its cache holds e4m3 keys and values with one fp32 scale per cached head vector (hd + 4
+bytes per vector instead of 2 * hd; the format is in include/quip_b200.h): twice the rows or context in the same memory,
+half the cache bytes a step reads, at the cost of one e4m3 rounding of every cached key and value.
 """
 import math
 
@@ -29,8 +32,11 @@ def _rotate_half(x):
 
 
 class GraphDecoder:
-    def __init__(self, model, max_len=256, batch=1, ops=None, layer_range=None, first=True, last=True):
-        """ops: provider of the fused glue kernels (quip_b200.fused.CudaGlue; picked up automatically when
+    def __init__(self, model, max_len=256, batch=1, ops=None, layer_range=None, first=True, last=True, kv_dtype=None):
+        """kv_dtype: None, torch.float16 or the model's dtype: the cache in the model's dtype (the only cache this
+        class keeps; PromptDecoder also takes torch.float8_e4m3fn).
+
+        ops: provider of the fused glue kernels (quip_b200.fused.CudaGlue; picked up automatically when
         QUIP_FUSED_LAYER=1 on a CUDA device), None for the torch glue.
 
         layer_range=(lo, hi), first, last: one STAGE of a layer pipeline (the reference's opt_multigpu / llama_multigpu
@@ -66,8 +72,7 @@ class GraphDecoder:
         L, B = len(self.layers), self.batch
         self.h_in = None if self.first else torch.zeros(B, 1, cfg.hidden_size, dtype=dt, device=self.dev)
         self.h_out = None if self.last else torch.zeros(B, 1, cfg.hidden_size, dtype=dt, device=self.dev)
-        self.k_cache = torch.zeros(L, B, self.nkv, self.max_len, self.hd, dtype=dt, device=self.dev)
-        self.v_cache = torch.zeros_like(self.k_cache)
+        self._alloc_cache((L, B, self.nkv, self.max_len, self.hd), dt, kv_dtype)
         self.position = torch.zeros(1, dtype=torch.long, device=self.dev)
         self.tokens = torch.zeros(B, dtype=torch.long, device=self.dev)
         self.logits = None
@@ -83,6 +88,16 @@ class GraphDecoder:
             if fused.enabled() and getattr(cfg, 'hidden_act', 'silu') == 'silu' and self.hd % 16 == 0:
                 ops = fused.CudaGlue()
         self.ops = ops
+
+    def _alloc_cache(self, shape, dt, kv_dtype):
+        """k_cache / v_cache of `shape` in the model's dtype dt."""
+        if not (kv_dtype is None or kv_dtype == dt or kv_dtype == torch.float16):
+            raise ValueError(f'{type(self).__name__} keeps its KV cache in the model dtype {dt}: kv_dtype {kv_dtype} '
+                             'is not supported' + (' (PromptDecoder takes float8_e4m3fn)'
+                                                   if kv_dtype == torch.float8_e4m3fn else ''))
+        self.kv_dtype = dt
+        self.k_cache = torch.zeros(shape, dtype=dt, device=self.dev)
+        self.v_cache = torch.zeros_like(self.k_cache)
 
     def _parallel(self, x, mods):
         """[m(x) for m in mods] with every module after the first on its own stream (graph branches when capturing)."""
@@ -350,11 +365,16 @@ class PromptDecoder(GraphDecoder):
         per-row scatter into the cache, SDPA under the mask arange(max_len) <= positions[:, None];
       * `prefill` fills the cache from a batch of prompts with the model's own many-token forward;
       * max_new > 0: greedy selection inside the step -- tokens = argmax(logits), stored in generated[:, t] -- so a
-        host loop only replays the graph.
+        host loop only replays the graph;
+      * kv_dtype=torch.float8_e4m3fn: k_cache / v_cache e4m3 with k_scale / v_scale (L, B, nkv, max_len) fp32, one scale
+        per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
+        (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
+        quantized values of every slot, its own included.  On the CPU the same step in torch: quantize, per-row scatter,
+        dequantize the cache to the compute dtype, SDPA under the mask.
     The whole model, no layer pipeline."""
 
-    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None):
-        super().__init__(model, max_len=max_len, batch=batch, ops=ops)
+    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None):
+        super().__init__(model, max_len=max_len, batch=batch, ops=ops, kv_dtype=kv_dtype)
         B = self.batch
         self.positions = torch.zeros(B, dtype=torch.long, device=self.dev)
         self.max_new = int(max_new)
@@ -364,6 +384,22 @@ class PromptDecoder(GraphDecoder):
         self._pos_host = [0] * B
         self._t_host = 0
         self._kernel = self.dev.type == 'cuda'
+
+    def _alloc_cache(self, shape, dt, kv_dtype):
+        """fp8: e4m3 caches and their fp32 scales, allocated as such (never an fp16 cache first: at the sizes fp8 is for,
+        that one would not fit)."""
+        self.k_scale = self.v_scale = None
+        if kv_dtype != torch.float8_e4m3fn:
+            return super()._alloc_cache(shape, dt, kv_dtype)
+        self.kv_dtype = kv_dtype
+        self.k_cache = torch.zeros(shape, dtype=kv_dtype, device=self.dev)
+        self.v_cache = torch.zeros_like(self.k_cache)
+        self.k_scale = torch.zeros(shape[:-1], dtype=torch.float32, device=self.dev)
+        self.v_scale = torch.zeros_like(self.k_scale)
+
+    @property
+    def _fp8(self):
+        return self.kv_dtype == torch.float8_e4m3fn
 
     def _step_positions(self):
         return self.positions
@@ -375,13 +411,22 @@ class PromptDecoder(GraphDecoder):
         B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
         if self._kernel:
             from . import fused
+            sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
             o = fused.decode_attention(q.reshape(B, nh, hd).contiguous(), k.reshape(B, nkv, hd).contiguous(),
                                        v.reshape(B, nkv, hd).contiguous(), self.k_cache[li], self.v_cache[li],
-                                       self.positions, scale)
+                                       self.positions, scale, **sc)
             return o.view(B, 1, nh * hd)
-        self.k_cache[li][self._rows, :, self.positions] = k[:, :, 0]
-        self.v_cache[li][self._rows, :, self.positions] = v[:, :, 0]
-        kk, vv = self.k_cache[li], self.v_cache[li]
+        if self._fp8:
+            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
+                xq, xs = _e4m3_quantize(x[:, :, 0])
+                cache[self._rows, :, self.positions] = xq
+                scales[self._rows, :, self.positions] = xs
+            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
+            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
+        else:
+            self.k_cache[li][self._rows, :, self.positions] = k[:, :, 0]
+            self.v_cache[li][self._rows, :, self.positions] = v[:, :, 0]
+            kk, vv = self.k_cache[li], self.v_cache[li]
         if nkv != nh:
             kk = kk.repeat_interleave(nh // nkv, dim=1)
             vv = vv.repeat_interleave(nh // nkv, dim=1)
@@ -407,6 +452,9 @@ class PromptDecoder(GraphDecoder):
     def reset(self):
         """Back to an empty cache: every row at position 0, nothing generated."""
         super().reset()
+        if self._fp8:
+            self.k_scale.zero_()
+            self.v_scale.zero_()
         self.positions.zero_()
         self._t.zero_()
         self.generated.zero_()
@@ -437,8 +485,11 @@ class PromptDecoder(GraphDecoder):
             out = self.model.model(input_ids=ids, attention_mask=attn, use_cache=True)
             cache = out.past_key_values
             for li in range(len(self.layers)):
-                self.k_cache[li, :, :, :P].copy_(cache.layers[li].keys)
-                self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
+                if self._fp8:
+                    self._store_fp8(li, cache.layers[li].keys, cache.layers[li].values)
+                else:
+                    self.k_cache[li, :, :, :P].copy_(cache.layers[li].keys)
+                    self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
             logits = self.model.lm_head(out.last_hidden_state[self._rows, lens_t - 1])     # last real token per row
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
@@ -448,6 +499,18 @@ class PromptDecoder(GraphDecoder):
                 self._t.fill_(1)
                 self._t_host = 1
         return logits
+
+    def _store_fp8(self, li, keys, values):
+        """Quantize the prefill's keys / values (B, nkv, P, hd) into slots 0 .. P-1 of layer li's e4m3 cache."""
+        P = keys.shape[2]
+        for x, cache, scales in ((keys, self.k_cache[li], self.k_scale[li]), (values, self.v_cache[li], self.v_scale[li])):
+            if self._kernel:
+                from . import fused
+                fused.kv_quantize(x.to(torch.float16).contiguous(), cache, scales)
+            else:
+                xq, xs = _e4m3_quantize(x)
+                cache[:, :, :P] = xq
+                scales[:, :, :P] = xs
 
     def step(self, tokens=None):
         """One step at every row's own position: tokens (B,) -- or, when generating, the tokens the previous step
@@ -468,15 +531,29 @@ class PromptDecoder(GraphDecoder):
         return self.logits
 
 
+def _e4m3_quantize(x):
+    """The e4m3 format of the fp8 cache (include/quip_b200.h) in torch, for the CPU step: x (..., hd) -> (e4m3 (..., hd),
+    fp32 scales (...))."""
+    x = x.float()
+    amax = x.abs().amax(-1)
+    s = torch.where(amax == 0, torch.ones_like(amax), amax / torch.full_like(amax, 448.0))       # IEEE division
+    return (x / s[..., None]).to(torch.float8_e4m3fn), s
+
+
+def _e4m3_dequantize(q, s, dtype):
+    return (q.float() * s[..., None]).to(dtype)
+
+
 EOS_CHECK_EVERY = 16
 
 
-def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None):
+def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None):
     """Greedy continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of
     new token ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled
     in one many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
     max_len (default: longest prompt + max_new_tokens) is the KV cache length.  Stops early once every row has produced
-    an EOS, checked every EOS_CHECK_EVERY steps."""
+    an EOS, checked every EOS_CHECK_EVERY steps.  kv_dtype=torch.float8_e4m3fn keeps the KV cache in e4m3 with per-vector
+    scales (PromptDecoder); None (the default) keeps it in the model's dtype."""
     prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
     max_new_tokens = int(max_new_tokens)
     if not prompts:
@@ -494,7 +571,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None):
         raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the model')
     eos = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
                                            [int(e) for e in eos_token_id])
-    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens)
+    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()
     dec.prefill(prompts)

@@ -88,10 +88,17 @@ class CudaGlue:
         return out
 
 
-def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale):
+def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None):
     """quip_decode_attention on torch tensors: append k_new / v_new (B, nkv, hd) at slot positions[b] of one layer's
     k_cache / v_cache (B, nkv, max_len, hd) and attend q (B, nh, hd) over slots 0 .. positions[b].  fp16, CUDA,
-    contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream."""
+    contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream.
+
+    Caches of dtype torch.float8_e4m3fn take quip_decode_attention_fp8 and need their per-slot fp32 scales k_scale /
+    v_scale (B, nkv, max_len): k_new / v_new are quantized on append (include/quip_b200.h has the format)."""
+    if k_cache.dtype == torch.float8_e4m3fn:
+        return _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale)
+    if k_scale is not None or v_scale is not None:
+        raise ValueError('decode_attention: k_scale / v_scale go with float8_e4m3fn caches only')
     ts = (q, k_new, v_new, k_cache, v_cache)
     for t in ts + (positions,):
         if not t.is_cuda:
@@ -123,6 +130,69 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale):
                                              max_len, C.c_float(scale), ws.data_ptr(), ws.numel(),
                                              torch.cuda.current_stream(q.device).cuda_stream))
     return out
+
+
+def _check_cuda(fn, ts, dev):
+    for t in ts:
+        if not t.is_cuda:
+            raise RuntimeError(f'{fn} runs on a CUDA device only (there is no CPU fallback)')
+        if t.device != dev:
+            raise ValueError(f'{fn}: all tensors must be on one device')
+        if not t.is_contiguous():
+            raise ValueError(f'{fn} takes contiguous tensors')
+
+
+def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale):
+    if k_scale is None or v_scale is None:
+        raise ValueError('decode_attention: float8_e4m3fn caches need k_scale and v_scale')
+    if (any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or v_cache.dtype != torch.float8_e4m3fn or
+            k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32 or positions.dtype != torch.int64):
+        raise ValueError('decode_attention: an e4m3 step takes fp16 q / k / v, float8_e4m3fn caches, fp32 scales and '
+                         'int64 positions')
+    if q.dim() != 3 or k_cache.dim() != 4:
+        raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
+                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
+    B, nh, hd = q.shape
+    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
+    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+            tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
+            tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape):
+        raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
+                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, scales '
+                         f'{tuple(k_scale.shape)} / {tuple(v_scale.shape)}, positions {tuple(positions.shape)} do not agree')
+    _check_cuda('decode_attention', (q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions), q.device)
+    lib = _lib.load()
+    need = C.c_size_t(0)
+    _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
+    ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
+    out = torch.empty_like(q)
+    with torch.cuda.device(q.device):
+        _lib.check(lib.quip_decode_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                 v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+                                                 positions.data_ptr(), out.data_ptr(), B, nh, nkv, hd, max_len,
+                                                 C.c_float(scale), ws.data_ptr(), ws.numel(),
+                                                 torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
+def kv_quantize(src, cache, scales):
+    """quip_kv_quantize_fp8 on torch tensors: quantize src (B, nkv, P, hd) fp16 into slots 0 .. P-1 of cache
+    (B, nkv, max_len, hd) float8_e4m3fn and scales (B, nkv, max_len) fp32; slots >= P are not touched.  CUDA, one
+    device, contiguous; on the current stream.  Dtypes and shapes are checked before the device."""
+    if src.dtype != torch.float16 or cache.dtype != torch.float8_e4m3fn or scales.dtype != torch.float32:
+        raise ValueError('kv_quantize takes fp16 src, a float8_e4m3fn cache and fp32 scales')
+    if src.dim() != 4 or cache.dim() != 4:
+        raise ValueError(f'kv_quantize: src must be (B, nkv, P, hd) and the cache (B, nkv, max_len, hd), got '
+                         f'{tuple(src.shape)} and {tuple(cache.shape)}')
+    B, nkv, P, hd = src.shape
+    max_len = cache.shape[2]
+    if tuple(cache.shape) != (B, nkv, max_len, hd) or tuple(scales.shape) != (B, nkv, max_len) or P > max_len:
+        raise ValueError(f'kv_quantize: shapes src {tuple(src.shape)}, cache {tuple(cache.shape)}, scales '
+                         f'{tuple(scales.shape)} do not agree')
+    _check_cuda('kv_quantize', (src, cache, scales), src.device)
+    with torch.cuda.device(src.device):
+        _lib.check(_lib.load().quip_kv_quantize_fp8(src.data_ptr(), cache.data_ptr(), scales.data_ptr(), B, nkv, P,
+                                                    max_len, hd, torch.cuda.current_stream(src.device).cuda_stream))
 
 
 def mlp_layout_plan(mlp):
