@@ -40,7 +40,8 @@ def test_ldlq_kernels_reproduce_the_reference_codes():
         assert torch.equal(fn(w, H, int(nbits), int(npasses)), fn(w, H, int(nbits), int(npasses)))      # deterministic
 
 
-@pytest.mark.parametrize('m,d,bits,passes', [(512, 1024, 2, 0), (300, 640, 4, 0), (4096, 4096, 2, 0), (256, 384, 2, 2), (1000, 1408, 3, 1)])
+@pytest.mark.parametrize('m,d,bits,passes', [(512, 1024, 2, 0), (300, 640, 4, 0), (4096, 4096, 2, 0), (256, 384, 2, 2), (1000, 1408, 3, 1),
+                                              (1000, 1416, 3, 1)])
 def test_ldlq_kernels_agree_with_the_torch_loop(m, d, bits, passes):
     """Ragged row counts (not a multiple of the 64-row CTA), a last block shorter than 128 columns, greedy passes."""
     from quip_b200 import quantize as qz
