@@ -168,6 +168,27 @@ int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_ne
 int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,
                          int32_t max_len, int32_t hd, void* stream);
 
+/* Token selection of one generation step: for each row b of logits (B, V) fp16 contiguous (rows need no alignment),
+ * with T = temperature[b], k = top_k[b], p = top_p[b] and s = seed[b] (each (B), device) and t = *step (device; the
+ * index of the token being chosen, 0 for the one after the prompt), tokens[b] (int64) is:
+ *   1. greedy rows (T <= 0, T NaN, or k == 1): the smallest i with x_i = max x (torch.argmax; a NaN counts as the max);
+ *   2. z_i = fp32(x_i) / T, IEEE division;
+ *   3. rank: z descending, equal z by lower index first;
+ *   4. top-k: K = min(k, V) if k > 0, else V; the candidates are the first K tokens in rank order (exactly K);
+ *   5. e_i = exp(z_i - max z);
+ *   6. top-p, if p < 1 (not NaN): keep the shortest rank-order prefix of the candidates whose sum of e is >= p times
+ *      their total; at least one token (p <= 0 keeps the top one);
+ *   7. u = (w >> 8) * 2^-24, w the first word of Philox4x32-10 with key (s low word, s high word) and counter
+ *      (t low word, t high word, 0, 0);
+ *   8. S = sum of e over the kept tokens; walking them in INDEX order, the first whose running sum of e exceeds u * S.
+ * e is fp32 expf, then floor(e * 2^40) as an integer: every sum and comparison after that is exact and independent of
+ * order (u * S exactly), so a token depends only on (row, settings, seed, t) -- not on the batch, the row index or the
+ * launch -- and is bit-identical from run to run.  A row with non-finite logits still gets an index in [0, V).  The
+ * launch depends on (B, V) only: one captured graph serves every step and any settings written between replays.
+ * No workspace.  B >= 0 (0: nothing to do), 1 <= V <= 2^24. */
+int quip_sample(const void* logits, const float* temperature, const int32_t* top_k, const float* top_p,
+                const uint64_t* seed, const int64_t* step, int64_t* tokens, int32_t B, int32_t V, void* stream);
+
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout
  * (bits 3: int32 (K*3/32, N) as Quant3Linear.pack writes it; bits 4: (K/8, N); bits 2: (K/16, N)):

@@ -66,6 +66,8 @@ EXPORTS = {
                                             C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     'quip_kv_quantize_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, C.c_void_p]),
+    'quip_sample': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.c_int32, C.c_int32, C.c_void_p]),
     'quip_pack_codes': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     'quip_unpack_codes': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     'quip_convert_ref': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),

@@ -18,7 +18,9 @@ written for, opt.py:431-482: learned positions, LayerNorm with bias, ReLU MLP; t
 of prompts by the model's own many-token forward; `generate` runs it greedily from a CUDA graph.  With
 kv_dtype=torch.float8_e4m3fn its cache holds e4m3 keys and values with one fp32 scale per cached head vector (hd + 4
 bytes per vector instead of 2 * hd; the format is in include/quip_b200.h): twice the rows or context in the same memory,
-half the cache bytes a step reads, at the cost of one e4m3 rounding of every cached key and value.
+half the cache bytes a step reads, at the cost of one e4m3 rounding of every cached key and value.  With sampling=True
+its step selects by temperature, top-k and top-p with a per-row seed (quip_sample, csrc/sample.cu; the rule is in
+include/quip_b200.h) instead of argmax, from settings held in device buffers, so one captured graph serves any settings.
 """
 import math
 
@@ -364,8 +366,11 @@ class PromptDecoder(GraphDecoder):
         kernel, slots 0 .. positions[b] read and no others, GQA without copies.  On the CPU the same step in torch:
         per-row scatter into the cache, SDPA under the mask arange(max_len) <= positions[:, None];
       * `prefill` fills the cache from a batch of prompts with the model's own many-token forward;
-      * max_new > 0: greedy selection inside the step -- tokens = argmax(logits), stored in generated[:, t] -- so a
-        host loop only replays the graph;
+      * max_new > 0: selection inside the step -- tokens = argmax(logits), stored in generated[:, t] -- so a host loop
+        only replays the graph;
+      * sampling=True: the selection is quip_sample (csrc/sample.cu) over the device buffers temperature, top_k, top_p
+        and seed (B each, filled by set_sampling) at step t = _t, the index of the token in generated; a row's token
+        depends on its logits, settings, seed and t only.  On the CPU the same rule in torch (_sample_torch);
       * kv_dtype=torch.float8_e4m3fn: k_cache / v_cache e4m3 with k_scale / v_scale (L, B, nkv, max_len) fp32, one scale
         per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
         (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
@@ -373,7 +378,7 @@ class PromptDecoder(GraphDecoder):
         dequantize the cache to the compute dtype, SDPA under the mask.
     The whole model, no layer pipeline."""
 
-    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None):
+    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False):
         super().__init__(model, max_len=max_len, batch=batch, ops=ops, kv_dtype=kv_dtype)
         B = self.batch
         self.positions = torch.zeros(B, dtype=torch.long, device=self.dev)
@@ -384,6 +389,49 @@ class PromptDecoder(GraphDecoder):
         self._pos_host = [0] * B
         self._t_host = 0
         self._kernel = self.dev.type == 'cuda'
+        self.sampling = bool(sampling)
+        if self.sampling:
+            self.temperature = torch.ones(B, dtype=torch.float32, device=self.dev)
+            self.top_k = torch.zeros(B, dtype=torch.int32, device=self.dev)
+            self.top_p = torch.ones(B, dtype=torch.float32, device=self.dev)
+            self.seed = torch.zeros(B, dtype=torch.int64, device=self.dev)
+
+    def set_sampling(self, temperature=1.0, top_k=0, top_p=1.0, seed=0):
+        """Write the sampling settings into the device buffers a captured step reads: each a scalar for every row or one
+        value per row.  seed: ints in [0, 2^64), or an int64 tensor holding their two's-complement bits.  Temperature 0 or
+        top_k 1 makes a row greedy (argmax)."""
+        if not self.sampling:
+            raise ValueError('set_sampling needs a PromptDecoder made with sampling=True')
+        B = self.batch
+
+        def rows(v):
+            v = v.tolist() if torch.is_tensor(v) else v
+            v = list(v) if isinstance(v, (list, tuple)) else [v] * B
+            if len(v) != B:
+                raise ValueError(f'{len(v)} values for a decoder of batch {B}')
+            return v
+        if torch.is_tensor(seed) and seed.dtype == torch.int64:
+            seeds = rows(seed)
+        else:
+            seeds = [int(x) for x in rows(seed)]
+            if any(not 0 <= x < 2 ** 64 for x in seeds):
+                raise ValueError('seeds must lie in [0, 2^64)')
+            seeds = [x - 2 ** 64 if x >= 2 ** 63 else x for x in seeds]
+        self.temperature.copy_(torch.tensor(rows(temperature), dtype=torch.float32))
+        self.top_k.copy_(torch.tensor(rows(top_k), dtype=torch.int32))
+        self.top_p.copy_(torch.tensor(rows(top_p), dtype=torch.float32))
+        self.seed.copy_(torch.tensor(seeds, dtype=torch.int64))
+
+    def _select(self, logits):
+        """tokens = the token chosen for each row from logits (B, vocab) at step _t: argmax, or with sampling the rule of
+        quip_sample."""
+        if not self.sampling:
+            self.tokens.copy_(logits.argmax(-1))
+        elif self._kernel:
+            from . import fused
+            fused.sample(logits, self.temperature, self.top_k, self.top_p, self.seed, self._t, self.tokens)
+        else:
+            self.tokens.copy_(_sample_torch(logits, self.temperature, self.top_k, self.top_p, self.seed, int(self._t)))
 
     def _alloc_cache(self, shape, dt, kv_dtype):
         """fp8: e4m3 caches and their fp32 scales, allocated as such (never an fp16 cache first: at the sizes fp8 is for,
@@ -436,7 +484,7 @@ class PromptDecoder(GraphDecoder):
     def _advance(self):
         self.positions.add_(1)
         if self.max_new:
-            self.tokens.copy_(self.logits.argmax(-1))
+            self._select(self.logits)
             self.generated.index_copy_(1, self._t, self.tokens[:, None])
             self._t.add_(1)
 
@@ -466,7 +514,8 @@ class PromptDecoder(GraphDecoder):
         forward (`model.model(ids, attention_mask=..., use_cache=True)`, the packed linears at M = B * P), its keys and
         values copied to the cache slots 0 .. P-1.  Slots past a row's length hold padding; the step overwrites them in
         turn and never reads past positions[b].  Returns the logits after each prompt's last token (B, vocab); with
-        max_new > 0 their argmax is the first generated token and the next step's input."""
+        max_new > 0 the token selected from them (argmax, or sampled at t = 0) is the first generated token and the next
+        step's input."""
         B = self.batch
         if len(prompts) != B:
             raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
@@ -494,7 +543,8 @@ class PromptDecoder(GraphDecoder):
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
             if self.max_new:
-                self.tokens.copy_(logits.argmax(-1))
+                self._t.zero_()
+                self._select(logits)
                 self.generated[:, 0].copy_(self.tokens)
                 self._t.fill_(1)
                 self._t_host = 1
@@ -544,16 +594,98 @@ def _e4m3_dequantize(q, s, dtype):
     return (q.float() * s[..., None]).to(dtype)
 
 
+def _philox_uniform(seed, t):
+    """u = (w >> 8) * 2^-24, w the first word of Philox4x32-10 of counter (t lo, t hi, 0, 0) under key (seed lo, seed hi);
+    seed and t are Python ints taken mod 2^64."""
+    M = 0xFFFFFFFF
+    seed, t = seed % 2 ** 64, t % 2 ** 64
+    c0, c1, c2, c3 = t & M, t >> 32, 0, 0
+    k0, k1 = seed & M, seed >> 32
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + 0x9E3779B9) & M, (k1 + 0xBB67AE85) & M
+        p0, p1 = 0xD2511F53 * c0, 0xCD9E8D57 * c2
+        c0, c1, c2, c3 = (p1 >> 32) ^ c1 ^ k0, p1 & M, (p0 >> 32) ^ c3 ^ k1, p0 & M
+    return (c0 >> 8) * 2.0 ** -24
+
+
+def _sample_torch(logits, temperature, top_k, top_p, seed, t):
+    """The rule of quip_sample (include/quip_b200.h) in torch, one row at a time: the CPU step of a sampling
+    PromptDecoder.  z is fp32 as the kernel has it (same ranking, same top-k set); e and its sums are float64."""
+    B, V = logits.shape
+    out = torch.empty(B, dtype=torch.long)
+    for b in range(B):
+        x = logits[b].detach().float().cpu()
+        T, k, p = float(temperature[b]), int(top_k[b]), float(top_p[b])
+        if not T > 0 or k == 1:
+            out[b] = x.argmax()
+            continue
+        z = x / torch.tensor(T, dtype=torch.float32)
+        order = torch.sort(z, descending=True, stable=True).indices
+        cand = order[:min(k, V) if k > 0 else V]
+        e = torch.exp(z[cand].double() - float(z[order[0]]))
+        n = cand.numel()
+        if p < 1:
+            cs = torch.cumsum(e, 0)
+            n = min(n, max(1, int(torch.searchsorted(cs, torch.tensor([p * float(cs[-1])], dtype=torch.float64))) + 1))
+        kept, ek = cand[:n], e[:n]
+        idx = torch.argsort(kept, stable=True)                     # index order
+        run = torch.cumsum(ek[idx], 0)
+        thr = _philox_uniform(int(seed[b]), t) * float(run[-1])
+        j = min(int(torch.searchsorted(run, torch.tensor([thr], dtype=torch.float64), right=True)), n - 1)
+        out[b] = kept[idx[j]]
+    return out.to(logits.device)
+
+
 EOS_CHECK_EVERY = 16
 
 
-def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None):
-    """Greedy continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of
-    new token ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled
-    in one many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
+def _per_prompt(name, v, n):
+    """A generate() setting as one value per prompt: a scalar for all, or a list / 1-D tensor of n."""
+    if torch.is_tensor(v):
+        v = v.tolist()
+    if isinstance(v, (list, tuple)):
+        if len(v) != n:
+            raise ValueError(f'{name}: {len(v)} values for {n} prompts')
+        return list(v)
+    return [v] * n
+
+
+def _sampling_settings(n, temperature, top_k, top_p, seed):
+    """Validated per-prompt (temperature, top_k, top_p, seeds) for n prompts; an int seed gives prompt b the seed
+    seed + b (mod 2^64)."""
+    temps = [float(t) for t in _per_prompt('temperature', temperature, n)]
+    if any(not (math.isfinite(t) and t >= 0) for t in temps):
+        raise ValueError(f'temperature must be finite and >= 0, got {temperature}')
+    ks = _per_prompt('top_k', top_k, n)
+    if any(int(k) != k or k < 0 for k in ks):
+        raise ValueError(f'top_k must be an integer >= 0, got {top_k}')
+    ps = [float(p) for p in _per_prompt('top_p', top_p, n)]
+    if any(not 0 < p <= 1 for p in ps):
+        raise ValueError(f'top_p must lie in (0, 1], got {top_p}')
+    explicit = torch.is_tensor(seed) or isinstance(seed, (list, tuple))
+    seeds = _per_prompt('seed', seed, n) if explicit else [seed]
+    if any(int(x) != x or not 0 <= x < 2 ** 64 for x in seeds):
+        raise ValueError(f'seeds must be integers in [0, 2^64), got {seed}')
+    if not explicit:
+        seeds = [(int(seed) + b) % 2 ** 64 for b in range(n)]
+    return temps, [int(k) for k in ks], ps, [int(x) for x in seeds]
+
+
+def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
+             temperature=1.0, top_k=0, top_p=1.0, seed=0):
+    """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
+    ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
+    many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
     max_len (default: longest prompt + max_new_tokens) is the KV cache length.  Stops early once every row has produced
     an EOS, checked every EOS_CHECK_EVERY steps.  kv_dtype=torch.float8_e4m3fn keeps the KV cache in e4m3 with per-vector
-    scales (PromptDecoder); None (the default) keeps it in the model's dtype."""
+    scales (PromptDecoder); None (the default) keeps it in the model's dtype.
+
+    Greedy (argmax) unless do_sample=True, which samples by the rule of include/quip_b200.h (quip_sample): temperature
+    (>= 0, finite; 0 is greedy), top_k (0: off; exactly k candidates, ties by lower id), top_p (in (0, 1]) and seed, each
+    a scalar or one value per prompt.  An int seed gives prompt b the seed seed + b (mod 2^64); a list gives each prompt
+    its own, and then a prompt's continuation is the same alone or in any batch.  A sampling setting other than the
+    default without do_sample=True raises ValueError."""
     prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
     max_new_tokens = int(max_new_tokens)
     if not prompts:
@@ -571,7 +703,16 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the model')
     eos = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
                                            [int(e) for e in eos_token_id])
-    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype)
+    if not do_sample:
+        for name, v, d in (('temperature', temperature, 1.0), ('top_k', top_k, 0), ('top_p', top_p, 1.0), ('seed', seed, 0)):
+            if torch.is_tensor(v) or isinstance(v, (list, tuple)) or v != d:
+                raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
+    else:
+        settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
+    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype,
+                        sampling=bool(do_sample))
+    if do_sample:
+        dec.set_sampling(*settings)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()
     dec.prefill(prompts)

@@ -195,6 +195,30 @@ def kv_quantize(src, cache, scales):
                                                     max_len, hd, torch.cuda.current_stream(src.device).cuda_stream))
 
 
+def sample(logits, temperature, top_k, top_p, seed, step, out):
+    """quip_sample on torch tensors: one token per row of logits (B, V) fp16 into out (B,) int64, by the rule of
+    include/quip_b200.h (greedy rows T <= 0 or k == 1; else temperature, top-k, top-p and a Philox draw of (seed, step)).
+    temperature / top_p (B,) fp32, top_k (B,) int32, seed (B,) int64 (the seeds' two's-complement bits, read as uint64)
+    or uint64, step (1,) int64.  CUDA, one device, contiguous; on the current stream.  Returns out."""
+    B = logits.shape[0] if logits.dim() == 2 else -1
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'sample: logits must be (B, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    for name, t, dts in (('temperature', temperature, (torch.float32,)), ('top_k', top_k, (torch.int32,)),
+                         ('top_p', top_p, (torch.float32,)), ('seed', seed, (torch.int64, torch.uint64)),
+                         ('out', out, (torch.int64,))):
+        if t.dtype not in dts or tuple(t.shape) != (B,):
+            raise ValueError(f'sample: {name} must be ({B},) {" or ".join(str(d) for d in dts)}, got '
+                             f'{tuple(t.shape)} {t.dtype}')
+    if step.dtype != torch.int64 or step.numel() != 1:
+        raise ValueError(f'sample: step must be one int64, got {tuple(step.shape)} {step.dtype}')
+    _check_cuda('sample', (logits, temperature, top_k, top_p, seed, step, out), logits.device)
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(),
+                                           seed.data_ptr(), step.data_ptr(), out.data_ptr(), B, logits.shape[1],
+                                           torch.cuda.current_stream(logits.device).cuda_stream))
+    return out
+
+
 def mlp_layout_plan(mlp):
     """The combined index of the three permutations around SiLU(gate) * up of a packed Llama MLP -- the output gathers of
     gate_proj / up_proj (y[j] = layout[u_idx[j]]) and the input gather of down_proj (layout[l] = x[v_idx[l]]) -- so that one

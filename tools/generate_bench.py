@@ -4,13 +4,19 @@ GQA) against PromptDecoder (per-row positions, csrc/attn_decode.cu), and the dec
 HBM bandwidth of the H100 SXM data sheet (3.35 TB/s).  Needs a CUDA device.
 
     python tools/generate_bench.py --out DIR [--models llama7b,llama70b] [--layers70b 80] [--steps 16]
-                                   [--sections kernel,prefill,decode,fp8]      (fp8kernel: the fp8 kernel rows only)
+                                   [--sections kernel,prefill,decode,fp8]      (fp8kernel: the fp8 kernel rows only;
+                                                                                sample: the sampling rows)
 
 Section fp8 measures the e4m3 KV cache (PromptDecoder(kv_dtype=torch.float8_e4m3fn)): the fp8 kernel alone next to the
 fp16 one (bytes: hd per cached K / V vector plus its 4-byte scale), PromptDecoder steps fp16 against fp8 at B = 32 and
 contexts 2048 / 4096 (alternating in one process, one decoder allocated at a time, both caches filled from the same
 values; logits compared), and configurations whose fp16 cache does not fit the card, run with fp8 or listed with the
 bytes they need.
+
+Section sample times quip_sample (csrc/sample.cu) alone for B in {1, 32, 128} x V in {32000, 50272, 128256} at
+T = 0.7, k = 50, p = 0.9 and at k = 0, p = 0.9, next to torch.argmax and the torch warper chain (temperature, top-k, sort,
+softmax, cumsum, top-p mask, multinomial) on the same rows, and a 7B PromptDecoder step at B = 32, context 2048, greedy
+against sampling, alternated over three trials.
 
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
@@ -249,6 +255,73 @@ def decode_steps_fp8(model, B, ctx, steps, trials=2, kinds=('fp16', 'fp8')):
     return out
 
 
+def torch_warpers(x, T, k, p):
+    """HF-style sampling chain in torch ops: temperature, top-k, top-p over a descending sort, multinomial."""
+    z = x.float() / T
+    if k:
+        kth = torch.topk(z, k, dim=-1).values[:, -1:]
+        z = z.masked_fill(z < kth, float('-inf'))
+    s, idx = torch.sort(z, descending=True, dim=-1)
+    cs = torch.softmax(s, -1).cumsum(-1)
+    drop = (cs - torch.softmax(s, -1)) >= p                             # mass ranked strictly above is >= p
+    s = s.masked_fill(drop, float('-inf'))
+    pick = torch.multinomial(torch.softmax(s, -1), 1)
+    return idx.gather(-1, pick)[:, 0]
+
+
+def sample_alone(B, V, k, p, reps):
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(0)
+    x = (torch.randn(B, V, generator=g, device='cuda') * 3).half()
+    T = torch.full((B,), 0.7, device='cuda')
+    kk = torch.full((B,), k, dtype=torch.int32, device='cuda')
+    pp = torch.full((B,), p, device='cuda')
+    sd = torch.arange(B, dtype=torch.int64, device='cuda')
+    step = torch.zeros(1, dtype=torch.int64, device='cuda')
+    out = torch.empty(B, dtype=torch.int64, device='cuda')
+    ms = events_ms(lambda: fused.sample(x, T, kk, pp, sd, step, out), reps)
+    ms_argmax = events_ms(lambda: x.argmax(-1), reps)
+    ms_chain = events_ms(lambda: torch_warpers(x, 0.7, k, p), max(reps // 4, 5))
+    return dict(B=B, V=V, T=0.7, top_k=k, top_p=p, kernel_ms=ms, torch_argmax_ms=ms_argmax, torch_warpers_ms=ms_chain)
+
+
+def sample_steps(model, B, ctx, steps, trials=3):
+    """Per-step ms of a captured PromptDecoder generating greedily and one sampling (T 0.7, k 50, p 0.9) at every row's
+    position ctx .. ctx+steps-1, alternating trial by trial."""
+    from quip_b200.decode import PromptDecoder
+    max_len = ctx + steps + 1
+    res = {'greedy': [], 'sampling': []}
+    for t in range(trials + 1):
+        for kind in ('greedy', 'sampling'):
+            dec = PromptDecoder(model, max_len=max_len, batch=B, max_new=steps + 1, sampling=kind == 'sampling')
+            if kind == 'sampling':
+                dec.set_sampling(temperature=0.7, top_k=50, top_p=0.9, seed=list(range(B)))
+            dec.k_cache.normal_(0.0, 0.5)
+            dec.v_cache.normal_(0.0, 0.5)
+            dec.capture()
+            with torch.no_grad():
+                for rep in range(2):
+                    dec.positions.fill_(ctx)
+                    dec._pos_host = [ctx] * B
+                    dec._t.fill_(1)
+                    dec._t_host = 1
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(steps):
+                        dec.step()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    if rep and t:
+                        res[kind].append(e0.elapsed_time(e1) / steps)
+            del dec
+            torch.cuda.empty_cache()
+    out = dict(B=B, context=ctx, trials_ms=res)
+    for kind in res:
+        out[f'{kind}_ms'] = sorted(res[kind])[len(res[kind]) // 2]
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -286,7 +359,17 @@ def main():
                     print(f'{name} fp8 kernel B={B} ctx={ctx}: {r["kernel_ms"]:.4f} ms, {r["bytes_per_s"] / 1e12:.2f} TB/s '
                           f'({100 * r["share_of_3_35_TBps"]:.0f}% of 3.35), rel err vs fp16 kernel {r["rel_err_vs_fp16"]:.1e}',
                           flush=True)
-        if not sections & {'prefill', 'decode', 'fp8'}:
+        if 'sample' in sections and name == 'llama7b':
+            rec['sample'] = []
+            for B in (1, 32, 128):
+                for V in (32000, 50272, 128256):
+                    for k, p in ((50, 0.9), (0, 0.9)):
+                        r = sample_alone(B, V, k, p, a.kernel_reps)
+                        rec['sample'].append(r)
+                        print(f'sample B={B} V={V} k={k} p={p}: kernel {1e3 * r["kernel_ms"]:.1f} us, torch argmax '
+                              f'{1e3 * r["torch_argmax_ms"]:.1f} us, torch warpers {1e3 * r["torch_warpers_ms"]:.1f} us',
+                              flush=True)
+        if not sections & {'prefill', 'decode', 'fp8', 'sample'}:
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
@@ -306,6 +389,11 @@ def main():
                 print(f'{name} decode B={B} ctx={ctx}: GraphDecoder {r["graph_decoder_ms"]:.3f} ms/step '
                       f'({r["graph_decoder_tok_s"]:.0f} tok/s), PromptDecoder {r["prompt_decoder_ms"]:.3f} ms/step '
                       f'({r["prompt_decoder_tok_s"]:.0f} tok/s), logits rel err {r["logits_rel_err"]:.1e}', flush=True)
+        if 'sample' in sections and name == 'llama7b':
+            r = sample_steps(model, 32, 2048, a.steps)
+            rec['sample_decode'] = r
+            print(f'{name} PromptDecoder B=32 ctx=2048: greedy {r["greedy_ms"]:.3f} ms/step, sampling '
+                  f'{r["sampling_ms"]:.3f} ms/step', flush=True)
         # fp16 against fp8 at B = 32, then the configurations only an e4m3 cache fits (7B 48 x 4096, 70B 64 x 4096)
         runs = [(32, 2048, ('fp16', 'fp8')), (32, 4096, ('fp16', 'fp8'))] if 'fp8' in sections else []
         if 'fp8' in sections:
