@@ -162,6 +162,48 @@ int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_ne
                               float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
                               int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
                               size_t workspace_bytes, void* stream);
+/* One attention step with T new tokens per row (speculative verification), each row at its own position, on one layer
+ * of the static KV cache.  q (B, T, nh, hd) fp16 token-major, rotary applied; k_new / v_new (B, T, nkv, hd) fp16;
+ * caches (B, nkv, max_len, hd); positions (B) int64 on the device; out (B, T, nh, hd) fp16.  Token i of row b is written
+ * at slot positions[b] + i, and
+ *   out[b][i][h] = softmax_j(scale * q[b][i][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b] + i,
+ * causal inside the new tokens.  No slot past positions[b] + T - 1 is read.  Scores and softmax in fp32; Q.K^T and P.V
+ * on tensor cores (fp16 operands, fp32 accumulation; p rounded once to fp16); one fp16 rounding of the output.  1 <= T
+ * <= 8, hd in {64, 128}, nh % nkv == 0, nh / nkv <= 8; pointers 16-byte aligned; fp32 scratch from
+ * quip_extend_attention_workspace_bytes.  The grid depends on (B, T, nkv, max_len) only.  A row with positions[b] < 0
+ * or positions[b] + T > max_len writes nothing and gets NaN outputs.  Deterministic, and a row's result does not depend
+ * on the other rows.  T = 1 computes what quip_decode_attention does, to within its rounding of p. */
+int quip_extend_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                          const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
+                          int32_t max_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+int quip_extend_attention_workspace_bytes(int32_t B, int32_t T, int32_t nh, int32_t hd, int32_t max_len,
+                                          size_t* out_bytes);
+/* The same on an e4m3 cache with per-slot scales (the format of quip_decode_attention_fp8): the new keys and values are
+ * quantized on append and attended over as quantized values.  A slot's k scale multiplies its score column; its v scale
+ * multiplies p before p is rounded to fp16 (normalised by the chunk's largest v scale, which multiplies the chunk's
+ * P.V). */
+int quip_extend_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                              float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t T,
+                              int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
+/* Prompt-lookup drafts.  hist (B, max_len) int64 holds each row's tokens by position; the current token is at
+ * c = positions[b].  For e < c let L(e) be the length of the common suffix of hist[b, ..e] and hist[b, ..c], capped at
+ * n_max.  The match is the e with the largest L(e) >= n_min, the largest such e on ties (longest n-gram first, then the
+ * most recent).  tokens (B, 1 + k): column 0 is hist[b, c]; the drafts d_i = u[e + i], i = 1..k, with u = hist[b, 0..c]
+ * followed by d itself (an overlapping copy, so a period shorter than k still fills k drafts).  No match: every d_i is
+ * the current token.  A row with c outside [0, max_len) gets zeros.  1 <= n_min <= n_max; O(c * n_max) reads. */
+int quip_ngram_draft(const int64_t* hist, const int64_t* positions, int64_t* tokens, int32_t B, int32_t max_len,
+                     int32_t k, int32_t n_min, int32_t n_max, void* stream);
+/* Acceptance of a verified speculative step.  tokens (B, T) are the step's inputs (the current token, then T - 1 drafts),
+ * targets (B, T) the tokens selected from the step's logits.  For each row with n_gen[b] < max_new: a = the length of the
+ * longest prefix with tokens[b][i] == targets[b][i - 1] (i = 1 ..); e = min(a + 1, max_new - n_gen[b]); targets[b][0 ..
+ * e-1] are written to generated[b][n_gen ..] (rows of gen_cols >= max_new) and hist[b][positions + 1 ..] (slots below
+ * max_len); positions and n_gen advance by e, accepted by e - 1.  Finished rows are left alone. */
+int quip_spec_accept(const int64_t* tokens, const int64_t* targets, int64_t* generated, int64_t* hist,
+                     int64_t* positions, int64_t* n_gen, int64_t* accepted, int32_t B, int32_t T, int32_t max_new,
+                     int32_t gen_cols, int32_t max_len, void* stream);
+
 /* Prefill of an e4m3 cache: src (B, nkv, P, hd) fp16 quantized as above into slots 0 .. P-1 of cache
  * (B, nkv, max_len, hd) e4m3fn and scales (B, nkv, max_len) fp32; slots >= P are not touched.  hd in {64, 128},
  * P <= max_len; src and cache 16-byte aligned, scales 4-byte aligned. */
@@ -188,6 +230,12 @@ int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B,
  * No workspace.  B >= 0 (0: nothing to do), 1 <= V <= 2^24. */
 int quip_sample(const void* logits, const float* temperature, const int32_t* top_k, const float* top_p,
                 const uint64_t* seed, const int64_t* step, int64_t* tokens, int32_t B, int32_t V, void* stream);
+/* The same rule over logits (B * T, V): row b * T + i takes the settings and seed of row b (each (B)) and
+ * t = steps[b] + i, steps (B) int64 on the device.  Row b * T + i's token is what quip_sample gives for that logits row
+ * with those settings at step t. */
+int quip_sample_at(const void* logits, const float* temperature, const int32_t* top_k, const float* top_p,
+                   const uint64_t* seed, const int64_t* steps, int64_t* tokens, int32_t B, int32_t T, int32_t V,
+                   void* stream);
 
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout

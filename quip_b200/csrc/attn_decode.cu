@@ -332,19 +332,20 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   }
 }
 
-// One CTA per (row, head), one thread per dim: merge the chunks 0 .. positions[b] / chunk in ascending order.
+// One CTA per (row, token, head), one thread per dim: merge the chunks 0 .. (positions[b] + i) / chunk of token i in
+// ascending order.  T = 1 is the decode step; a row with positions[b] + T > max_len gets NaN.
 __global__ void __launch_bounds__(128)
 attn_decode_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
                            const int64_t* __restrict__ positions, __half* __restrict__ out, int nh, int hd, int max_len,
-                           int nsplit, int chunk) {
+                           int nsplit, int chunk, int T) {
   const int bh = blockIdx.x, d = threadIdx.x;
-  const int b = bh / nh;
+  const int bt = bh / nh, b = bt / T;
   const int64_t pos = positions[b];
-  if (pos < 0 || pos >= max_len) {
+  if (pos < 0 || pos > (int64_t)max_len - T) {
     out[(int64_t)bh * hd + d] = __float2half_rn(NAN);
     return;
   }
-  const int ns = (int)(pos / chunk) + 1;
+  const int ns = (int)((pos + bt % T) / chunk) + 1;
   const float* ml = part_ml + (int64_t)bh * nsplit * 2;
   const float* po = part_o + (int64_t)bh * nsplit * hd + d;
   float M = -INFINITY;
@@ -356,6 +357,277 @@ attn_decode_combine_kernel(const float* __restrict__ part_o, const float* __rest
     O = fmaf(po[(int64_t)s * hd], w, O);
   }
   out[(int64_t)bh * hd + d] = __float2half_rn(O / L);
+}
+
+// ---- Extend attention: T <= 8 new tokens per row (speculative verification), on tensor cores.
+//
+// CTA (split, kv head, row) owns one AX_CHUNK-slot chunk and the R = G * T query rows (token i, head g) -> r = i * G + g
+// of its kv head, padded to MT = ceil(R / 16) m16 tiles.  The chunk's K and V (e4m3: converted exactly to fp16) and Q
+// are staged in shared memory; S = Q.K^T and O = P.V run as mma.sync m16n8k16 (fp16 in, fp32 accumulate).  Token i
+// sees slots j <= positions[b] + i.  Scores are fp32 (e4m3: times the slot's k scale), the chunk softmax is fp32 and P
+// is rounded once to fp16 for the MMA; e4m3 folds the slot's v scale into p before that rounding, normalised by the
+// largest v scale among the row's visible slots of the chunk (multiplied back into O) so that p * s_v keeps fp16's
+// normal range and a token's result does not depend on the slots it cannot see.  New slot
+// positions[b] + i is written by the CTA whose chunk holds it, which computes with the new (quantized) values directly.
+constexpr int AX_CHUNK = 64;
+constexpr int AX_THREADS = 128;
+constexpr int AX_MAXT = 8;
+constexpr int AX_ROWS = AD_MAXG * AX_MAXT;   // query rows per CTA at most
+
+template <int HD>
+struct AxLayout {
+  static constexpr int QS = HD + 8;          // row stride (halves) of the Q, K and V tiles: conflict-free fragments
+  static constexpr int PS = AX_CHUNK + 8;    // row stride (halves) of the P tile
+  static constexpr int SS = AX_CHUNK + 4;    // row stride (floats) of the score tile (aliases the Q tile)
+  static constexpr size_t QB = (size_t)AX_ROWS * QS * 2, SB = (size_t)AX_ROWS * SS * 4;
+  static constexpr size_t K_OFF = ((QB > SB ? QB : SB) + 15) & ~(size_t)15;
+  static constexpr size_t V_OFF = K_OFF + (size_t)AX_CHUNK * QS * 2;
+  static constexpr size_t P_OFF = V_OFF + (size_t)AX_CHUNK * QS * 2;
+  static constexpr size_t F_OFF = P_OFF + (size_t)AX_ROWS * PS * 2;   // k scales, v scales, each row's max v scale
+  static constexpr size_t BYTES = F_OFF + (2 * AX_CHUNK + AX_ROWS) * sizeof(float);
+};
+
+// 8 e4m3 bytes -> 8 fp16 (exact)
+__device__ __forceinline__ uint4 e4m3x8_to_h8(const uint2& u) {
+  AH8 t;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t w = i < 2 ? u.x : u.y;
+    t.h2[i] = __half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)((w >> (16 * (i & 1))) & 0xFFFFu), __NV_E4M3));
+  }
+  return t.v;
+}
+
+__device__ __forceinline__ uint32_t h2_pack(__half lo, __half hi) {
+  return (uint32_t)__half_as_ushort(lo) | ((uint32_t)__half_as_ushort(hi) << 16);
+}
+
+// Partials: o [B][T][nh][nsplit][HD], ml [B][T][nh][nsplit][2], the layout of the decode kernel with B * T rows.
+template <bool FP8, int HD, int G>
+__global__ void __launch_bounds__(AX_THREADS)
+attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict__ k_new, const __half* __restrict__ v_new,
+                         void* __restrict__ kc, void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
+                         const int64_t* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml,
+                         int nh, int nkv, int max_len, int nsplit, int T, float scale) {
+  using L = AxLayout<HD>;
+  using CT = std::conditional_t<FP8, uint8_t, __half>;
+  constexpr int QS = L::QS, PS = L::PS, SS = L::SS;
+  constexpr int SEG = HD / 8;                 // 16-byte fp16 segments of a head vector
+  constexpr int NT = HD / 32;                 // n8 tiles of a warp's quarter of the P.V output
+  extern __shared__ __align__(16) unsigned char ax_smem[];
+  __half* sq = reinterpret_cast<__half*>(ax_smem);
+  float* ss = reinterpret_cast<float*>(ax_smem);
+  __half* sk = reinterpret_cast<__half*>(ax_smem + L::K_OFF);
+  __half* sv = reinterpret_cast<__half*>(ax_smem + L::V_OFF);
+  __half* sp = reinterpret_cast<__half*>(ax_smem + L::P_OFF);
+  float* sks = reinterpret_cast<float*>(ax_smem + L::F_OFF);
+  float* svs = sks + AX_CHUNK;
+  float* svmax = svs + AX_CHUNK;              // per query row
+
+  const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
+  const int64_t pos = positions[b];
+  const int start = split * AX_CHUNK;
+  if (pos < 0 || pos > (int64_t)max_len - T || start > pos + T - 1) return;
+  const int n = (int)min((int64_t)AX_CHUNK, pos + T - start);          // slots start .. start + n - 1
+  const int nold = (int)max((int64_t)0, min((int64_t)n, pos - start));  // of which cached (the rest are new)
+  const int R = G * T, MT = (R + 15) / 16;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
+
+  const int64_t row = (int64_t)b * nkv + kvh;
+  CT* kr = reinterpret_cast<CT*>(kc) + row * (int64_t)max_len * HD;
+  CT* vr = reinterpret_cast<CT*>(vc) + row * (int64_t)max_len * HD;
+  auto new_vec = [&](const __half* x, int j) {  // the new key / value of chunk slot j
+    return x + (((int64_t)b * T + (start + j - pos)) * nkv + kvh) * HD;
+  };
+
+  // ---- stage Q (rows >= R zero), the chunk's K / V (rows >= n zero) and, e4m3, the slot scales
+  for (int i = tid; i < MT * 16 * SEG; i += AX_THREADS) {
+    const int r = i / SEG, c = i % SEG;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (r < R) v = __ldg(reinterpret_cast<const uint4*>(q + (((int64_t)b * T + r / G) * nh + (int64_t)kvh * G + r % G) * HD) + c);
+    reinterpret_cast<uint4*>(sq + r * QS)[c] = v;
+  }
+  for (int i = tid; i < AX_CHUNK * SEG; i += AX_THREADS) {
+    const int j = i / SEG, c = i % SEG;
+    uint4 kv = make_uint4(0, 0, 0, 0), vv = kv;
+    if (j < nold) {
+      if constexpr (FP8) {
+        kv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(kr + (int64_t)(start + j) * HD) + c));
+        vv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(vr + (int64_t)(start + j) * HD) + c));
+      } else {
+        kv = ldg_nc_v4(reinterpret_cast<const uint4*>(kr + (int64_t)(start + j) * HD) + c);
+        vv = ldg_nc_v4(reinterpret_cast<const uint4*>(vr + (int64_t)(start + j) * HD) + c);
+      }
+    } else if (j < n && !FP8) {               // append: this CTA owns slot start + j
+      kv = reinterpret_cast<const uint4*>(new_vec(k_new, j))[c];
+      vv = reinterpret_cast<const uint4*>(new_vec(v_new, j))[c];
+      reinterpret_cast<uint4*>(kr + (int64_t)(start + j) * HD)[c] = kv;
+      reinterpret_cast<uint4*>(vr + (int64_t)(start + j) * HD)[c] = vv;
+    } else if (j < n) {
+      continue;                               // e4m3 append below
+    }
+    reinterpret_cast<uint4*>(sk + j * QS)[c] = kv;
+    reinterpret_cast<uint4*>(sv + j * QS)[c] = vv;
+  }
+  if constexpr (FP8) {
+    for (int j = tid; j < nold; j += AX_THREADS) {
+      sks[j] = ksc[row * max_len + start + j];
+      svs[j] = vsc[row * max_len + start + j];
+    }
+    // append: one warp per new vector (k of slot j, then v), quantized, stored, and staged as fp16
+    constexpr int E = HD / 32;
+    for (int v = warp; v < 2 * (n - nold); v += AX_THREADS / 32) {
+      const int isv = v & 1, j = nold + v / 2;
+      float s;
+      const uint32_t w = e4m3_quantize_warp<HD>(new_vec(isv ? v_new : k_new, j), lane, s);
+      e4m3_store_warp<HD>((isv ? vr : kr) + (int64_t)(start + j) * HD, lane, w);
+      __half* t = (isv ? sv : sk) + j * QS + lane * E;
+#pragma unroll
+      for (int e = 0; e < E / 2; ++e)
+        reinterpret_cast<__half2*>(t)[e] =
+            __half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)((w >> (16 * e)) & 0xFFFFu), __NV_E4M3));
+      if (lane == 0) {
+        (isv ? vsc : ksc)[row * max_len + start + j] = s;
+        (isv ? svs : sks)[j] = s;
+      }
+    }
+  }
+  __syncthreads();
+
+  // ---- S = Q.K^T: warp w takes slots 16w .. 16w + 15 of every m tile
+  float acc[4][2][4];
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.f;
+  if (warp * 16 < n) {
+#pragma unroll
+    for (int kk = 0; kk < HD; kk += 16) {
+      uint32_t bf[2][2];
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt) {
+        const __half* kp = sk + (warp * 16 + nt * 8 + gid) * QS + kk + tig * 2;
+        bf[nt][0] = *reinterpret_cast<const uint32_t*>(kp);
+        bf[nt][1] = *reinterpret_cast<const uint32_t*>(kp + 8);
+      }
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt) {
+        if (mt < MT) {
+          const __half* qp = sq + (mt * 16 + gid) * QS + kk + tig * 2;
+          const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(qp), *reinterpret_cast<const uint32_t*>(qp + 8 * QS),
+                                 *reinterpret_cast<const uint32_t*>(qp + 8),
+                                 *reinterpret_cast<const uint32_t*>(qp + 8 * QS + 8)};
+#pragma unroll
+          for (int nt = 0; nt < 2; ++nt) mma16816(acc[mt][nt], a, bf[nt]);
+        }
+      }
+    }
+  }
+  __syncthreads();                            // the score tile overwrites the Q tile
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt) {
+    if (mt < MT) {
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int r = mt * 16 + gid + (e >> 1) * 8, j = warp * 16 + nt * 8 + tig * 2 + (e & 1);
+          float s = acc[mt][nt][e] * scale;
+          if constexpr (FP8) s = j < n ? s * sks[j] : s;
+          const bool ok = r < R && j < n && (int64_t)start + j <= pos + r / G;
+          ss[r * SS + j] = ok ? s : -INFINITY;
+        }
+    }
+  }
+  __syncthreads();
+
+  // ---- chunk softmax per query row (one warp per row, fixed order); P (fp16) for the MMA
+  for (int r = warp; r < MT * 16; r += AX_THREADS / 32) {
+    float p0 = 0.f, p1 = 0.f;
+    if (r < R) {
+      const float s0 = ss[r * SS + lane], s1 = ss[r * SS + lane + 32];
+      float m = fmaxf(s0, s1);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+      if (m != -INFINITY) {
+        p0 = expf(s0 - m);
+        p1 = expf(s1 - m);
+      }
+      float l = p0 + p1;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+      if (lane == 0) {
+        float* ml = part_ml + ((((int64_t)b * T + r / G) * nh + (int64_t)kvh * G + r % G) * nsplit + split) * 2;
+        ml[0] = m;
+        ml[1] = l;
+      }
+      if constexpr (FP8) {                    // p0 / p1 are 0 at the slots the row does not see
+        const int64_t last = pos + r / G - start;
+        float sm = fmaxf(lane <= last && lane < n ? svs[lane] : 0.f, lane + 32 <= last && lane + 32 < n ? svs[lane + 32] : 0.f);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sm = fmaxf(sm, __shfl_xor_sync(0xffffffffu, sm, o));
+        sm = sm > 0.f ? sm : 1.f;
+        const float vnorm = 1.f / sm;
+        p0 = p0 > 0.f ? p0 * (svs[lane] * vnorm) : 0.f;
+        p1 = p1 > 0.f ? p1 * (svs[lane + 32] * vnorm) : 0.f;
+        if (lane == 0) svmax[r] = sm;
+      }
+    }
+    sp[r * PS + lane] = __float2half_rn(p0);
+    sp[r * PS + lane + 32] = __float2half_rn(p1);
+  }
+  __syncthreads();
+
+  // ---- O = P.V: warp w takes dims w * HD / 4 .. of every m tile; k steps past n hold P = V = 0 and are skipped
+  float o[4][NT][4];
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[mt][nt][e] = 0.f;
+#pragma unroll
+  for (int kk = 0; kk < AX_CHUNK; kk += 16) {
+    if (kk < n) {
+      uint32_t bf[NT][2];
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) {
+        const __half* vp = sv + (kk + tig * 2) * QS + warp * (HD / 4) + nt * 8 + gid;
+        bf[nt][0] = h2_pack(vp[0], vp[QS]);
+        bf[nt][1] = h2_pack(vp[8 * QS], vp[9 * QS]);
+      }
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt) {
+        if (mt < MT) {
+          const __half* pp = sp + (mt * 16 + gid) * PS + kk + tig * 2;
+          const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(pp), *reinterpret_cast<const uint32_t*>(pp + 8 * PS),
+                                 *reinterpret_cast<const uint32_t*>(pp + 8),
+                                 *reinterpret_cast<const uint32_t*>(pp + 8 * PS + 8)};
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) mma16816(o[mt][nt], a, bf[nt]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt) {
+    if (mt < MT) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = mt * 16 + gid + 8 * h;
+        if (r < R) {
+          const float oscale = FP8 ? svmax[r] : 1.f;
+          float* dst = part_o + ((((int64_t)b * T + r / G) * nh + (int64_t)kvh * G + r % G) * nsplit + split) * HD +
+                       warp * (HD / 4) + tig * 2;
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt)
+            *reinterpret_cast<float2*>(dst + nt * 8) = make_float2(o[mt][nt][2 * h] * oscale, o[mt][nt][2 * h + 1] * oscale);
+        }
+      }
+    }
+  }
 }
 
 // Prefill: one warp per head vector v = (row, p) of src (rows, P, HD) fp16 -> e4m3 slot p of cache (rows, max_len, HD)
@@ -443,7 +715,76 @@ int decode_attention(const char* fn, const void* q, const void* k_new, const voi
   if (hd == 64) launch_split_g<FP8, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
   else launch_split_g<FP8, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
   QUIP_LAUNCHED("attn_decode_split_kernel");
-  attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk);
+  attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk, 1);
+  QUIP_LAUNCHED("attn_decode_combine_kernel");
+  return QUIP_OK;
+}
+
+template <bool FP8, int HD, int G>
+int launch_extend(dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
+                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
+                  int nsplit, int T, float scale) {
+  constexpr size_t smem = AxLayout<HD>::BYTES;
+  auto kern = attn_extend_split_kernel<FP8, HD, G>;
+  if (smem > 48 * 1024) QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<grid, AX_THREADS, smem, st>>>((const __half*)q, (const __half*)kn, (const __half*)vn, kc, vc, ksc, vsc, pos, po,
+                                       pml, nh, nkv, max_len, nsplit, T, scale);
+  QUIP_LAUNCHED("attn_extend_split_kernel");
+  return QUIP_OK;
+}
+
+template <bool FP8, int HD>
+int launch_extend_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc,
+                    void* vc, float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv,
+                    int max_len, int nsplit, int T, float scale) {
+#define AX_LAUNCH(g) \
+  return launch_extend<FP8, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, nh, nkv, max_len, nsplit, T, scale)
+  switch (G) {
+    case 1: AX_LAUNCH(1);
+    case 2: AX_LAUNCH(2);
+    case 3: AX_LAUNCH(3);
+    case 4: AX_LAUNCH(4);
+    case 5: AX_LAUNCH(5);
+    case 6: AX_LAUNCH(6);
+    case 7: AX_LAUNCH(7);
+    default: AX_LAUNCH(8);
+  }
+#undef AX_LAUNCH
+}
+
+// Argument checks and launches of quip_extend_attention (FP8 false) and quip_extend_attention_fp8 (FP8 true).
+template <bool FP8>
+int extend_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                     float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t T,
+                     int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
+                 "%s: null pointer", fn);
+  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(T >= 1 && T <= AX_MAXT, "%s: %d tokens per row: need 1 <= T <= %d", fn, T, AX_MAXT);
+  QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
+                 "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
+  QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
+                 "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head",
+                 fn, nh, nkv, AD_MAXG);
+  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache) && al16(out) && al16(workspace),
+                 "%s: pointers must be 16-byte aligned", fn);
+  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
+  const int nsplit = ceil_div(max_len, AX_CHUNK);
+  const size_t need = ws_bytes((int64_t)B * T, nh, hd, nsplit);
+  QUIP_CHECK_ARG(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+  if (B == 0) return QUIP_OK;
+  float* po = (float*)workspace;
+  float* pml = (float*)((char*)workspace + (((size_t)B * T * nh * nsplit * hd * sizeof(float) + 255) & ~(size_t)255));
+  const cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(nsplit, nkv, B);
+  const int G = nh / nkv;
+  const int e = hd == 64
+      ? launch_extend_g<FP8, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, T, scale)
+      : launch_extend_g<FP8, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, T, scale);
+  if (e != QUIP_OK) return e;
+  attn_decode_combine_kernel<<<(unsigned)((int64_t)B * T * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd,
+                                                                             max_len, nsplit, AX_CHUNK, T);
   QUIP_LAUNCHED("attn_decode_combine_kernel");
   return QUIP_OK;
 }
@@ -477,6 +818,33 @@ extern "C" int quip_decode_attention_fp8(const void* q, const void* k_new, const
                                          float scale, void* workspace, size_t workspace_bytes, void* stream) {
   return decode_attention<true>("quip_decode_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
                                 positions, out, B, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int quip_extend_attention_workspace_bytes(int32_t B, int32_t T, int32_t nh, int32_t hd, int32_t max_len,
+                                                     size_t* out_bytes) {
+  QUIP_CHECK_ARG(out_bytes, "quip_extend_attention_workspace_bytes: null pointer");
+  QUIP_CHECK_ARG(B >= 0 && T >= 1 && T <= AX_MAXT && nh > 0 && max_len > 0,
+                 "quip_extend_attention_workspace_bytes: bad sizes (B %d, T %d, nh %d, max_len %d)", B, T, nh, max_len);
+  QUIP_CHECK_ARG(hd == 64 || hd == 128, "quip_extend_attention_workspace_bytes: head_dim %d is not 64 or 128", hd);
+  *out_bytes = ws_bytes((int64_t)B * T, nh, hd, ceil_div(max_len, AX_CHUNK));
+  return QUIP_OK;
+}
+
+extern "C" int quip_extend_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                                     const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
+                                     int32_t hd, int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  return extend_attention<false>("quip_extend_attention", q, k_new, v_new, k_cache, v_cache, nullptr, nullptr, positions,
+                                 out, B, T, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int quip_extend_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache,
+                                         void* v_cache, float* k_scale, float* v_scale, const int64_t* positions,
+                                         void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
+                                         int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+  return extend_attention<true>("quip_extend_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
+                                positions, out, B, T, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
 }
 
 extern "C" int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,

@@ -21,6 +21,10 @@
 // The kept set always has the form {key > tau} + {the first m keys == tau in index order}.  Every pass recomputes z from
 // the fp16 row (re-read from L2); nothing depends on V fitting shared memory.  The launch reads the settings and the step
 // from device memory, so a captured graph serves every step and every setting written between replays.
+//
+// quip_sample_at is the same kernel over B * T logits rows: row b * T + i takes the settings and seed of b and the step
+// steps[b] + i (speculative verification: token i of row b lands at index steps[b] + i of the row's output).
+// quip_sample is its T = 1 case with one step shared by every row.
 #include <math.h>
 
 #include "common.cuh"
@@ -181,13 +185,15 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const __half* __r
                                                             const float* __restrict__ top_p,
                                                             const uint64_t* __restrict__ seed,
                                                             const int64_t* __restrict__ step,
-                                                            int64_t* __restrict__ tokens, int V) {
+                                                            int64_t* __restrict__ tokens, int V, int per_set,
+                                                            int step_stride) {
   __shared__ SampleSmem s;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int bs = b / per_set;                              // the row's settings (per_set logits rows each)
   const __half* x = logits + (size_t)b * V;
-  const float T = temperature[b];
-  const int32_t k = top_k[b];
-  const float p = top_p[b];
+  const float T = temperature[bs];
+  const int32_t k = top_k[bs];
+  const float p = top_p[bs];
   const bool greedy = !(T > 0.f) || k == 1;
   const uint32_t K = (k > 0 && k < V) ? (uint32_t)k : (uint32_t)V;
   auto key_of = [&](__half h) {
@@ -339,8 +345,8 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const __half* __r
       tot[w] = s.wtot[w] + (unsigned long long)kept * wt;
       S += tot[w];
     }
-    const int64_t t = *step;
-    const uint64_t sd = seed[b];
+    const int64_t t = step[(int64_t)bs * step_stride] + b % per_set;
+    const uint64_t sd = seed[bs];
     const uint32_t w24 = philox_word0((uint32_t)t, (uint32_t)((uint64_t)t >> 32), (uint32_t)sd, (uint32_t)(sd >> 32)) >> 8;
     // thr = floor(u * S), u = w24 / 2^24, exactly (S < 2^57)
     const unsigned long long lo64 = S * (unsigned long long)w24, hi64 = __umul64hi(S, (unsigned long long)w24);
@@ -405,7 +411,20 @@ extern "C" int quip_sample(const void* logits, const float* temperature, const i
   QUIP_CHECK_ARG(logits && temperature && top_k && top_p && seed && step && tokens, "quip_sample: null pointer");
   if (B == 0) return QUIP_OK;
   sample_kernel<<<(unsigned)B, SP_THREADS, 0, (cudaStream_t)stream>>>((const __half*)logits, temperature, top_k, top_p,
-                                                                      seed, step, tokens, V);
+                                                                      seed, step, tokens, V, 1, 0);
+  QUIP_LAUNCHED("sample_kernel");
+  return QUIP_OK;
+}
+
+extern "C" int quip_sample_at(const void* logits, const float* temperature, const int32_t* top_k, const float* top_p,
+                              const uint64_t* seed, const int64_t* steps, int64_t* tokens, int32_t B, int32_t T,
+                              int32_t V, void* stream) {
+  QUIP_CHECK_ARG(B >= 0 && T >= 1 && (int64_t)B * T <= 0x7FFFFFFF && V >= 1 && V <= SP_MAX_V,
+                 "quip_sample_at: bad sizes (B %d, T %d, V %d): need B >= 0, T >= 1 and 1 <= V <= %d", B, T, V, SP_MAX_V);
+  QUIP_CHECK_ARG(logits && temperature && top_k && top_p && seed && steps && tokens, "quip_sample_at: null pointer");
+  if (B == 0) return QUIP_OK;
+  sample_kernel<<<(unsigned)(B * T), SP_THREADS, 0, (cudaStream_t)stream>>>((const __half*)logits, temperature, top_k,
+                                                                            top_p, seed, steps, tokens, V, T, 1);
   QUIP_LAUNCHED("sample_kernel");
   return QUIP_OK;
 }

@@ -21,6 +21,9 @@ bytes per vector instead of 2 * hd; the format is in include/quip_b200.h): twice
 half the cache bytes a step reads, at the cost of one e4m3 rounding of every cached key and value.  With sampling=True
 its step selects by temperature, top-k and top-p with a per-row seed (quip_sample, csrc/sample.cu; the rule is in
 include/quip_b200.h) instead of argmax, from settings held in device buffers, so one captured graph serves any settings.
+`SpecDecoder` (generate(..., prompt_lookup_num_tokens=k)) verifies k prompt-lookup drafts per row in each captured step:
+T = k + 1 tokens per row through the same layer loops, attention by csrc/attn_decode.cu's extend kernel, drafting and
+acceptance by csrc/spec.cu.
 """
 import math
 
@@ -53,6 +56,7 @@ class GraphDecoder:
         self.nh = cfg.num_attention_heads
         dt = model.get_input_embeddings().weight.dtype     # fp16 on the GPU path; fp32 in the CPU tests
         self.first, self.last = bool(first), bool(last)
+        self.T = 1                                         # tokens per row in a step (SpecDecoder: 1 + drafts)
         if self.family == 'llama':
             self.layers = list(model.model.layers)
             self.nkv = getattr(cfg, 'num_key_value_heads', None) or self.nh
@@ -149,6 +153,13 @@ class GraphDecoder:
         o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
         return o.transpose(1, 2).reshape(B, 1, nh * hd)
 
+    def _rope_rows(self, pos):
+        """Rotary cos / sin rows of the step's tokens: (1 or B, hd) at T = 1; (B * T, hd), token i of row b at position
+        pos[b] + i, otherwise."""
+        if self.T > 1:
+            pos = (pos[:, None] + self._tarange).reshape(-1)
+        return self.cos.index_select(0, pos), self.sin.index_select(0, pos)
+
     def _advance(self):
         self.position.add_(1)
 
@@ -159,11 +170,12 @@ class GraphDecoder:
     # graph node); the residual add of a branch rides on the next RMSNorm
     def _layers_fused(self, h):
         ops = self.ops
-        B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
+        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
         pos = self._step_positions()
         h = h.contiguous()
-        cos = self.cos.index_select(0, pos).expand(B, hd).contiguous()                     # one row per sequence
-        sin = self.sin.index_select(0, pos).expand(B, hd).contiguous()
+        cos, sin = self._rope_rows(pos)
+        cos = cos.expand(B * T, hd).contiguous()                                          # one row per token
+        sin = sin.expand(B * T, hd).contiguous()
         mask = self._attn_mask(pos)
         pend = None
         for li, layer in enumerate(self.layers):
@@ -175,26 +187,29 @@ class GraphDecoder:
                 h, x = ops.rmsnorm(h, n1.weight, n1.variance_epsilon, residual=pend)
             q, k, v = self._parallel(x, [a.q_proj, a.k_proj, a.v_proj])
             ops.rope_(q, k, cos, sin, hd)
-            o = self._attend(li, q.view(B, 1, nh, hd).transpose(1, 2), k.view(B, 1, nkv, hd).transpose(1, 2),
-                             v.view(B, 1, nkv, hd).transpose(1, 2), mask, 1.0 / math.sqrt(hd))
+            o = self._attend(li, q.view(B, T, nh, hd).transpose(1, 2), k.view(B, T, nkv, hd).transpose(1, 2),
+                             v.view(B, T, nkv, hd).transpose(1, 2), mask, 1.0 / math.sqrt(hd))
             h, x = ops.rmsnorm(h, n2.weight, n2.variance_epsilon, residual=a.o_proj(o))
             gate, up = self._parallel(x, [mlp.gate_proj, mlp.up_proj])
             pend = mlp.down_proj(ops.silu_mul(gate, up))
         return h, pend
 
     def _layers_llama(self, h):
-        B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
+        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
         pos = self._step_positions()
-        cos = self.cos.index_select(0, pos)[:, None, None]                                 # (1 or B, 1, 1, hd)
-        sin = self.sin.index_select(0, pos)[:, None, None]
+        cos, sin = self._rope_rows(pos)
+        if T == 1:
+            cos, sin = cos[:, None, None], sin[:, None, None]                              # (1 or B, 1, 1, hd)
+        else:
+            cos, sin = cos.view(B, 1, T, hd), sin.view(B, 1, T, hd)
         mask = self._attn_mask(pos)
         for li, layer in enumerate(self.layers):
             a = layer.self_attn
             x = layer.input_layernorm(h)
             q, k, v = self._parallel(x, [a.q_proj, a.k_proj, a.v_proj])
-            q = q.view(B, 1, nh, hd).transpose(1, 2)                                       # (B, nh, 1, hd)
-            k = k.view(B, 1, nkv, hd).transpose(1, 2)
-            v = v.view(B, 1, nkv, hd).transpose(1, 2)
+            q = q.view(B, T, nh, hd).transpose(1, 2)                                       # (B, nh, T, hd)
+            k = k.view(B, T, nkv, hd).transpose(1, 2)
+            v = v.view(B, T, nkv, hd).transpose(1, 2)
             q = q * cos + _rotate_half(q) * sin
             k = k * cos + _rotate_half(k) * sin
             o = self._attend(li, q, k, v, mask, 1.0 / math.sqrt(hd))
@@ -208,14 +223,14 @@ class GraphDecoder:
     # OPT (modeling_opt.OPTDecoderLayer): pre- or post-LayerNorm, q scaled before the dot product, ReLU between fc1 and fc2;
     # biases live inside the (Quant)Linear modules
     def _layers_opt(self, h):
-        B, nh, hd = self.batch, self.nh, self.hd
+        B, T, nh, hd = self.batch, self.T, self.nh, self.hd
         mask = self._attn_mask(self._step_positions())
         for li, layer in enumerate(self.layers):
             a, before = layer.self_attn, layer.do_layer_norm_before
             x = layer.self_attn_layer_norm(h) if before else h
             q, k, v = self._parallel(x, [a.q_proj, a.k_proj, a.v_proj])
-            q = (q * a.scaling).view(B, 1, nh, hd).transpose(1, 2)                         # scaled first, as the HF module does
-            o = self._attend(li, q, k.view(B, 1, nh, hd).transpose(1, 2), v.view(B, 1, nh, hd).transpose(1, 2), mask, 1.0)
+            q = (q * a.scaling).view(B, T, nh, hd).transpose(1, 2)                         # scaled first, as the HF module does
+            o = self._attend(li, q, k.view(B, T, nh, hd).transpose(1, 2), v.view(B, T, nh, hd).transpose(1, 2), mask, 1.0)
             h = h + a.out_proj(o)
             if not before:
                 h = layer.self_attn_layer_norm(h)
@@ -226,17 +241,23 @@ class GraphDecoder:
         return h, None
 
     def _embed(self):
-        """Token (and, for OPT, learned position: index position + 2) embeddings of the step: (B, 1, hidden)."""
+        """Token (and, for OPT, learned position: index position + 2) embeddings of the step: (B, T, hidden); tokens is
+        (B,) at T = 1 and (B, T) otherwise."""
+        multi = self.T > 1
         if self.family == 'llama':
-            return self.model.model.embed_tokens(self.tokens)[:, None, :]
+            return self.model.model.embed_tokens(self.tokens) if multi else self.model.model.embed_tokens(self.tokens)[:, None, :]
         d = self.model.model.decoder
-        h = d.embed_tokens(self.tokens)[:, None, :]
+        h = d.embed_tokens(self.tokens) if multi else d.embed_tokens(self.tokens)[:, None, :]
         if d.project_in is not None:
             h = d.project_in(h)
-        return h + F.embedding(self._step_positions() + d.embed_positions.offset, d.embed_positions.weight)[:, None]
+        pos = self._step_positions()
+        if multi:
+            return h + F.embedding(pos[:, None] + self._tarange + d.embed_positions.offset, d.embed_positions.weight)
+        return h + F.embedding(pos + d.embed_positions.offset, d.embed_positions.weight)[:, None]
 
     def _head(self, h, pend):
-        """Final norm (fused with the pending residual add on the glue-kernel path) -> lm_head: logits (B, vocab)."""
+        """Final norm (fused with the pending residual add on the glue-kernel path) -> lm_head: logits (B, vocab), or
+        (B, T, vocab) for a step of T > 1 tokens per row."""
         if self.family == 'llama':
             fn = self.model.model.norm
             if self.ops is not None:
@@ -249,7 +270,8 @@ class GraphDecoder:
                 h = d.final_layer_norm(h)
             if d.project_out is not None:
                 h = d.project_out(h)
-        return self.model.lm_head(h)[:, 0, :]
+        logits = self.model.lm_head(h)
+        return logits if self.T > 1 else logits[:, 0, :]
 
     # one decode step of the stage on the static buffers (what the graph records)
     def _step(self):
@@ -422,16 +444,17 @@ class PromptDecoder(GraphDecoder):
         self.top_p.copy_(torch.tensor(rows(top_p), dtype=torch.float32))
         self.seed.copy_(torch.tensor(seeds, dtype=torch.int64))
 
-    def _select(self, logits):
-        """tokens = the token chosen for each row from logits (B, vocab) at step _t: argmax, or with sampling the rule of
-        quip_sample."""
+    def _select(self, logits, out=None):
+        """out (default: tokens) = the token chosen for each row from logits (B, vocab) at step _t: argmax, or with
+        sampling the rule of quip_sample."""
+        out = self.tokens if out is None else out
         if not self.sampling:
-            self.tokens.copy_(logits.argmax(-1))
+            out.copy_(logits.argmax(-1))
         elif self._kernel:
             from . import fused
-            fused.sample(logits, self.temperature, self.top_k, self.top_p, self.seed, self._t, self.tokens)
+            fused.sample(logits, self.temperature, self.top_k, self.top_p, self.seed, self._t, out)
         else:
-            self.tokens.copy_(_sample_torch(logits, self.temperature, self.top_k, self.top_p, self.seed, int(self._t)))
+            out.copy_(_sample_torch(logits, self.temperature, self.top_k, self.top_p, self.seed, int(self._t)))
 
     def _alloc_cache(self, shape, dt, kv_dtype):
         """fp8: e4m3 caches and their fp32 scales, allocated as such (never an fp16 cache first: at the sizes fp8 is for,
@@ -453,10 +476,16 @@ class PromptDecoder(GraphDecoder):
         return self.positions
 
     def _attn_mask(self, pos):
-        return None if self._kernel else (self._arange[None] <= pos[:, None])[:, None, None, :]     # (B, 1, 1, max_len)
+        if self._kernel:
+            return None
+        if self.T > 1:                                                                 # (B, 1, T, max_len), causal
+            return (self._arange[None, None] <= (pos[:, None] + self._tarange)[:, :, None])[:, None]
+        return (self._arange[None] <= pos[:, None])[:, None, None, :]                  # (B, 1, 1, max_len)
 
     def _attend(self, li, q, k, v, mask, scale):
         B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
+        if self.T > 1:
+            return self._attend_multi(li, q, k, v, mask, scale)
         if self._kernel:
             from . import fused
             sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
@@ -480,6 +509,37 @@ class PromptDecoder(GraphDecoder):
             vv = vv.repeat_interleave(nh // nkv, dim=1)
         o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
         return o.transpose(1, 2).reshape(B, 1, nh * hd)
+
+    def _attend_multi(self, li, q, k, v, mask, scale):
+        """_attend for T > 1 tokens per row (q (B, nh, T, hd), k / v (B, nkv, T, hd)): token i appended at slot
+        positions[b] + i and attending over slots 0 .. positions[b] + i.  CUDA: quip_extend_attention(_fp8), token-major
+        operands; CPU: per-row scatter of the T slots, SDPA under the causal mask.  Returns (B, T, nh * hd)."""
+        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
+        if self._kernel:
+            from . import fused
+            sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
+            o = fused.extend_attention(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous(),
+                                       v.transpose(1, 2).contiguous(), self.k_cache[li], self.v_cache[li],
+                                       self.positions, scale, **sc)
+            return o.view(B, T, nh * hd)
+        rows = self._rows[:, None].expand(B, T)
+        slots = self.positions[:, None] + self._tarange                                 # (B, T)
+        if self._fp8:
+            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
+                xq, xs = _e4m3_quantize(x.transpose(1, 2))                              # (B, T, nkv, hd), (B, T, nkv)
+                cache[rows, :, slots] = xq
+                scales[rows, :, slots] = xs
+            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
+            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
+        else:
+            self.k_cache[li][rows, :, slots] = k.transpose(1, 2)
+            self.v_cache[li][rows, :, slots] = v.transpose(1, 2)
+            kk, vv = self.k_cache[li], self.v_cache[li]
+        if nkv != nh:
+            kk = kk.repeat_interleave(nh // nkv, dim=1)
+            vv = vv.repeat_interleave(nh // nkv, dim=1)
+        o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
+        return o.transpose(1, 2).reshape(B, T, nh * hd)
 
     def _advance(self):
         self.positions.add_(1)
@@ -543,12 +603,16 @@ class PromptDecoder(GraphDecoder):
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
             if self.max_new:
-                self._t.zero_()
-                self._select(logits)
-                self.generated[:, 0].copy_(self.tokens)
-                self._t.fill_(1)
-                self._t_host = 1
+                self._first_token(logits)
         return logits
+
+    def _first_token(self, logits):
+        """Select the first generated token from the prefill's logits (B, vocab), at t = 0."""
+        self._t.zero_()
+        self._select(logits)
+        self.generated[:, 0].copy_(self.tokens)
+        self._t.fill_(1)
+        self._t_host = 1
 
     def _store_fp8(self, li, keys, values):
         """Quantize the prefill's keys / values (B, nkv, P, hd) into slots 0 .. P-1 of layer li's e4m3 cache."""
@@ -580,6 +644,183 @@ class PromptDecoder(GraphDecoder):
             self.graph.replay()
         return self.logits
 
+
+
+class SpecDecoder(PromptDecoder):
+    """PromptDecoder whose step verifies prompt-lookup drafts: T = 1 + draft_tokens tokens per row in one step.
+
+    One captured step runs
+      * draft: tokens (B, T) = the current token hist[b, positions[b]] and k drafts by n-gram lookup in the row's own
+        prompt and output (quip_ngram_draft; the rule is in include/quip_b200.h);
+      * the model on the B * T tokens: token i of row b at position positions[b] + i, attention by
+        quip_extend_attention(_fp8) (causal inside the new tokens);
+      * select: targets (B, T) from the step's logits (B, T, vocab): argmax, or with sampling the rule of quip_sample at
+        t = n_gen[b] + i (quip_sample_at), the index the token would take in generated -- so a token is the one the
+        non-speculative decoder chooses from the same logits;
+      * accept: the longest prefix of drafts that equals the targets before them, plus one target (quip_spec_accept),
+        appended to generated and hist; positions and n_gen advance by that count, accepted by the drafts taken.
+    Rejected drafts leave keys and values in slots past positions[b]; no step reads there before overwriting them.
+    A row with max_new tokens does not advance.  On the CPU the same step in torch (_ngram_draft_torch,
+    _spec_accept_torch, per-row scatter of the T slots and SDPA under the causal mask).  Needs max_len >= the longest
+    prompt + max_new + draft_tokens (a finished row's step still writes its T slots)."""
+
+    def __init__(self, model, max_len=256, batch=1, max_new=1, draft_tokens=4, max_ngram=3, ops=None, kv_dtype=None,
+                 sampling=False):
+        k, n_max = int(draft_tokens), int(max_ngram)
+        if not 1 <= k <= 7:
+            raise ValueError(f'draft_tokens must lie in [1, 7], got {draft_tokens}')
+        if n_max < 1:
+            raise ValueError(f'max_ngram must be at least 1, got {max_ngram}')
+        if int(max_new) < 1:
+            raise ValueError(f'a SpecDecoder selects inside its step: max_new must be at least 1, got {max_new}')
+        if int(max_len) < k + 2:
+            raise ValueError(f'max_len {max_len} leaves no room for a step of {k + 1} tokens')
+        super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
+                         sampling=sampling)
+        B, dev = self.batch, self.dev
+        self.k, self.n_min, self.n_max = k, 1, n_max
+        self.T = k + 1
+        self._tarange = torch.arange(self.T, device=dev)
+        self.tokens = torch.zeros(B, self.T, dtype=torch.long, device=dev)
+        self.targets = torch.zeros(B, self.T, dtype=torch.long, device=dev)
+        self.hist = torch.zeros(B, self.max_len, dtype=torch.long, device=dev)
+        self.n_gen = torch.zeros(B, dtype=torch.long, device=dev)
+        self.accepted = torch.zeros(B, dtype=torch.long, device=dev)
+        self._first = torch.zeros(B, dtype=torch.long, device=dev)
+        self._steps_host = 0
+
+    def _step(self):
+        self._draft()
+        super()._step()
+
+    def _draft(self):
+        if self._kernel:
+            from . import fused
+            fused.ngram_draft(self.hist, self.positions, self.tokens, self.n_min, self.n_max)
+        else:
+            self.tokens.copy_(_ngram_draft_torch(self.hist, self.positions, self.k, self.n_min, self.n_max))
+
+    def _advance(self):
+        logits = self.logits                                                            # (B, T, vocab)
+        if not self.sampling:
+            self.targets.copy_(logits.argmax(-1))
+        elif self._kernel:
+            from . import fused
+            fused.sample_at(logits, self.temperature, self.top_k, self.top_p, self.seed, self.n_gen, self.targets)
+        else:
+            self.targets.copy_(_sample_torch_at(logits, self.temperature, self.top_k, self.top_p, self.seed, self.n_gen))
+        if self._kernel:
+            from . import fused
+            fused.spec_accept(self.tokens, self.targets, self.generated, self.hist, self.positions, self.n_gen,
+                              self.accepted, self.max_new)
+        else:
+            _spec_accept_torch(self.tokens, self.targets, self.generated, self.hist, self.positions, self.n_gen,
+                               self.accepted, self.max_new)
+
+    def _capture_state(self):
+        return super()._capture_state() + [self.targets, self.hist, self.n_gen, self.accepted]
+
+    def _counters_in_range(self):
+        # a warm-up step writes slots positions[b] .. positions[b] + k: keep them inside the cache
+        super()._counters_in_range()
+        self.positions.clamp_(max=self.max_len - self.T)
+
+    def reset(self):
+        super().reset()
+        for t in (self.tokens, self.targets, self.hist, self.n_gen, self.accepted):
+            t.zero_()
+        self._steps_host = 0
+
+    def prefill(self, prompts):
+        """PromptDecoder.prefill, plus the history: each prompt and its first generated token in hist, n_gen = 1."""
+        lens = [int(torch.as_tensor(p).numel()) for p in prompts]
+        if lens and max(lens) + self.max_new + self.k > self.max_len:
+            raise ValueError(f'a prompt of {max(lens)} tokens, {self.max_new} new ones and {self.k} drafts exceed the '
+                             f'cache of {self.max_len} positions')
+        logits = super().prefill(prompts)
+        with torch.no_grad():
+            for b, p in enumerate(prompts):
+                self.hist[b, :lens[b]] = torch.as_tensor(p).reshape(-1).to(self.dev)
+        self.accepted.zero_()
+        self._steps_host = 0
+        return logits
+
+    def _first_token(self, logits):
+        self._t.zero_()
+        self._select(logits, out=self._first)
+        self.generated[:, 0].copy_(self._first)
+        self.hist[self._rows, self.positions] = self._first
+        self.n_gen.fill_(1)
+        self._t.fill_(1)
+        self._t_host = 1
+
+    def step(self, tokens=None):
+        """One speculative step for every row that has fewer than max_new tokens; returns the logits (B, T, vocab).
+        Every row is done after max_new - 1 steps (each gives an unfinished row at least one token)."""
+        if tokens is not None:
+            raise ValueError('a SpecDecoder step feeds its own tokens (the current one and its drafts)')
+        if self._steps_host >= self.max_new - 1:
+            raise ValueError(f'{self.max_new} tokens generated already')
+        self._steps_host += 1
+        if self.graph is None:
+            with torch.no_grad():
+                self._step()
+        else:
+            self.graph.replay()
+        return self.logits
+
+
+def _ngram_draft_torch(hist, positions, k, n_min, n_max):
+    """The rule of quip_ngram_draft (include/quip_b200.h) in torch, one row at a time: (B, 1 + k)."""
+    B, max_len = hist.shape
+    out = torch.zeros(B, k + 1, dtype=torch.long)
+    for b in range(B):
+        c = int(positions[b])
+        if not 0 <= c < max_len:
+            continue
+        h = hist[b, :c + 1].cpu()
+        e = torch.arange(c)
+        length = torch.zeros(c, dtype=torch.long)
+        alive = torch.ones(c, dtype=torch.bool)
+        for t in range(min(n_max, c)):                               # suffix element t: h[e - t] == h[c - t]
+            alive = alive & (e >= t) & (h[(e - t).clamp(min=0)] == h[c - t])
+            length += alive.long()
+        key = torch.where(length >= n_min, length * (c + 1) + e, torch.full_like(e, -1))   # longest, then latest
+        u = h.tolist()
+        best = int(key.argmax()) if c and int(key.max()) >= 0 else -1
+        for i in range(1, k + 1):
+            u.append(u[c] if best < 0 else u[best + i])
+        out[b] = torch.tensor(u[c:])
+    return out.to(hist.device)
+
+
+def _spec_accept_torch(tokens, targets, generated, hist, positions, n_gen, accepted, max_new):
+    """The rule of quip_spec_accept (include/quip_b200.h) in torch, in place."""
+    B, T = tokens.shape
+    a = (tokens[:, 1:] == targets[:, :-1]).long().cumprod(1).sum(1)
+    live = n_gen < max_new
+    e = torch.where(live, torch.minimum(a + 1, max_new - n_gen), torch.zeros_like(a))
+    j = torch.arange(T, device=tokens.device)
+    w = j[None] < e[:, None]
+    rows = torch.arange(B, device=tokens.device)[:, None].expand(B, T)
+    gcol, hcol = n_gen[:, None] + j, positions[:, None] + 1 + j
+    generated[rows[w], gcol[w]] = targets[w]
+    hw = w & (hcol >= 0) & (hcol < hist.shape[1])
+    hist[rows[hw], hcol[hw]] = targets[hw]
+    positions += e
+    n_gen += e
+    accepted += torch.where(live, e - 1, torch.zeros_like(e))
+
+
+def _sample_torch_at(logits, temperature, top_k, top_p, seed, steps):
+    """_sample_torch over logits (B, T, vocab): token i of row b with row b's settings at step steps[b] + i."""
+    B, T, _ = logits.shape
+    out = torch.empty(B, T, dtype=torch.long)
+    for b in range(B):
+        for i in range(T):
+            out[b, i] = _sample_torch(logits[b, i][None], temperature[b:b + 1], top_k[b:b + 1], top_p[b:b + 1],
+                                      seed[b:b + 1], int(steps[b]) + i)[0]
+    return out.to(logits.device)
 
 def _e4m3_quantize(x):
     """The e4m3 format of the fp8 cache (include/quip_b200.h) in torch, for the CPU step: x (..., hd) -> (e4m3 (..., hd),
@@ -673,7 +914,8 @@ def _sampling_settings(n, temperature, top_k, top_p, seed):
 
 
 def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
-             temperature=1.0, top_k=0, top_p=1.0, seed=0):
+             temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
+             spec_stats=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -685,7 +927,14 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     (>= 0, finite; 0 is greedy), top_k (0: off; exactly k candidates, ties by lower id), top_p (in (0, 1]) and seed, each
     a scalar or one value per prompt.  An int seed gives prompt b the seed seed + b (mod 2^64); a list gives each prompt
     its own, and then a prompt's continuation is the same alone or in any batch.  A sampling setting other than the
-    default without do_sample=True raises ValueError."""
+    default without do_sample=True raises ValueError.
+
+    prompt_lookup_num_tokens=k (1 .. 7; default None: off) generates speculatively (SpecDecoder): each step verifies the
+    current token and k drafts copied from the latest longest match (up to max_matching_ngram_size tokens) of the row's
+    own prompt and output, and keeps the drafts the model itself would have chosen plus one more token.  The tokens are
+    the ones plain generation selects from the same logits (greedy or sampled, with the same seeds); only the step's
+    arithmetic differs (other token counts take other kernel routes).  The default max_len grows by k.  spec_stats: a
+    dict that receives 'accepted' (drafts taken per row) and 'steps'."""
     prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
     max_new_tokens = int(max_new_tokens)
     if not prompts:
@@ -695,9 +944,18 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     lens = [p.numel() for p in prompts]
     if min(lens) == 0:
         raise ValueError('empty prompt')
-    max_len = max(lens) + max_new_tokens if max_len is None else int(max_len)
-    if max(lens) + max_new_tokens > max_len:
-        raise ValueError(f'a prompt of {max(lens)} tokens plus {max_new_tokens} new ones exceeds max_len {max_len}')
+    spec = prompt_lookup_num_tokens is not None
+    k = 0
+    if spec:
+        k, n_max = int(prompt_lookup_num_tokens), int(max_matching_ngram_size)
+        if k != prompt_lookup_num_tokens or not 1 <= k <= 7:
+            raise ValueError(f'prompt_lookup_num_tokens must be an integer in [1, 7], got {prompt_lookup_num_tokens}')
+        if n_max != max_matching_ngram_size or n_max < 1:
+            raise ValueError(f'max_matching_ngram_size must be an integer >= 1, got {max_matching_ngram_size}')
+    max_len = max(lens) + max_new_tokens + k if max_len is None else int(max_len)
+    if max(lens) + max_new_tokens + k > max_len:
+        raise ValueError(f'a prompt of {max(lens)} tokens plus {max_new_tokens} new ones' +
+                         (f' and {k} drafts' if k else '') + f' exceeds max_len {max_len}')
     cfg = model.config
     if cfg.model_type == 'opt' and max_len > cfg.max_position_embeddings:
         raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the model')
@@ -709,14 +967,20 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                 raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
     else:
         settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
-    dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype,
-                        sampling=bool(do_sample))
+    if spec:
+        dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
+                          max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample))
+    else:
+        dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype,
+                            sampling=bool(do_sample))
     if do_sample:
         dec.set_sampling(*settings)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()
     dec.prefill(prompts)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
+    if spec:
+        return _generate_spec(dec, max_new_tokens, eos_t, spec_stats)
     n = 1
     while n < max_new_tokens:
         if eos and n % EOS_CHECK_EVERY == 0 and bool(torch.isin(dec.generated[:, :n], eos_t).any(1).all()):
@@ -725,6 +989,31 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         n += 1
     out = []
     for row in dec.generated[:, :n].cpu():
+        hit = torch.isin(row, eos_t.cpu()).nonzero()
+        out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+    return out
+
+
+def _generate_spec(dec, max_new, eos_t, stats):
+    """generate()'s host loop over SpecDecoder steps: it syncs only every EOS_CHECK_EVERY steps, to stop once every row
+    has max_new tokens or an EOS among its tokens."""
+    steps = 0
+    cols = torch.arange(dec.generated.shape[1], device=dec.dev)
+    while steps < max_new - 1:
+        if steps and steps % EOS_CHECK_EVERY == 0:
+            done = dec.n_gen >= max_new
+            if eos_t.numel():
+                done = done | (torch.isin(dec.generated, eos_t) & (cols[None] < dec.n_gen[:, None])).any(1)
+            if bool(done.all()):
+                break
+        dec.step()
+        steps += 1
+    if stats is not None:
+        stats['accepted'] = dec.accepted.tolist()
+        stats['steps'] = steps
+    out = []
+    for row, n in zip(dec.generated.cpu(), dec.n_gen.tolist()):
+        row = row[:n]
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
     return out

@@ -219,6 +219,110 @@ def sample(logits, temperature, top_k, top_p, seed, step, out):
     return out
 
 
+def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None):
+    """quip_extend_attention(_fp8) on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot
+    positions[b] + i of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots
+    0 .. positions[b] + i.  fp16 q / k / v; fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale
+    (B, nkv, max_len).  CUDA, one device, contiguous; positions (B,) int64.  Returns (B, T, nh, hd) fp16."""
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise ValueError('extend_attention: k_scale / v_scale go with float8_e4m3fn caches only')
+    if fp8 and (k_scale is None or v_scale is None):
+        raise ValueError('extend_attention: float8_e4m3fn caches need k_scale and v_scale')
+    cdt = torch.float8_e4m3fn if fp8 else torch.float16
+    if (any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or k_cache.dtype != cdt or v_cache.dtype != cdt or
+            positions.dtype != torch.int64 or (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
+        raise ValueError('extend_attention takes fp16 q / k / v, fp16 or float8_e4m3fn caches (fp32 scales) and int64 '
+                         'positions')
+    if q.dim() != 4 or k_cache.dim() != 4:
+        raise ValueError(f'extend_attention: q must be (B, T, nh, hd) and the caches (B, nkv, max_len, hd), got '
+                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
+    B, T, nh, hd = q.shape
+    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
+    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+            tuple(k_new.shape) != (B, T, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
+            (fp8 and (tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape))):
+        raise ValueError(f'extend_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
+                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
+                         f'{tuple(positions.shape)} do not agree')
+    ts = (q, k_new, v_new, k_cache, v_cache, positions) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('extend_attention', ts, q.device)
+    lib = _lib.load()
+    need = C.c_size_t(0)
+    _lib.check(lib.quip_extend_attention_workspace_bytes(B, T, nh, hd, max_len, C.byref(need)))
+    ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
+    out = torch.empty_like(q)
+    st = torch.cuda.current_stream(q.device).cuda_stream
+    with torch.cuda.device(q.device):
+        if fp8:
+            _lib.check(lib.quip_extend_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                     v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+                                                     positions.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,
+                                                     C.c_float(scale), ws.data_ptr(), ws.numel(), st))
+        else:
+            _lib.check(lib.quip_extend_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                 v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, T, nh, nkv,
+                                                 hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
+    return out
+
+
+def sample_at(logits, temperature, top_k, top_p, seed, steps, out):
+    """quip_sample_at: logits (B, T, V) fp16 -> out (B, T) int64, token i of row b by the rule of quip_sample with row b's
+    settings and seed at step steps[b] + i (steps (B,) int64).  CUDA, one device, contiguous; on the current stream."""
+    if logits.dim() != 3 or logits.dtype != torch.float16:
+        raise ValueError(f'sample_at: logits must be (B, T, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    B, T, V = logits.shape
+    for name, t, dts, shape in (('temperature', temperature, (torch.float32,), (B,)),
+                                ('top_k', top_k, (torch.int32,), (B,)), ('top_p', top_p, (torch.float32,), (B,)),
+                                ('seed', seed, (torch.int64, torch.uint64), (B,)), ('steps', steps, (torch.int64,), (B,)),
+                                ('out', out, (torch.int64,), (B, T))):
+        if t.dtype not in dts or tuple(t.shape) != shape:
+            raise ValueError(f'sample_at: {name} must be {shape} {" or ".join(str(d) for d in dts)}, got '
+                             f'{tuple(t.shape)} {t.dtype}')
+    _check_cuda('sample_at', (logits, temperature, top_k, top_p, seed, steps, out), logits.device)
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_sample_at(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(),
+                                              top_p.data_ptr(), seed.data_ptr(), steps.data_ptr(), out.data_ptr(), B, T, V,
+                                              torch.cuda.current_stream(logits.device).cuda_stream))
+    return out
+
+
+def _check_i64(fn, **ts):
+    for name, (t, shape) in ts.items():
+        if t.dtype != torch.int64 or tuple(t.shape) != tuple(shape):
+            raise ValueError(f'{fn}: {name} must be {tuple(shape)} int64, got {tuple(t.shape)} {t.dtype}')
+
+
+def ngram_draft(hist, positions, tokens, n_min, n_max):
+    """quip_ngram_draft: tokens (B, 1 + k) = the current token hist[b, positions[b]] and k prompt-lookup drafts from
+    hist (B, max_len) (the rule is in include/quip_b200.h).  int64, CUDA, contiguous.  Returns tokens."""
+    B, max_len = hist.shape
+    _check_i64('ngram_draft', hist=(hist, (B, max_len)), positions=(positions, (B,)),
+               tokens=(tokens, (B, tokens.shape[-1] if tokens.dim() == 2 else -1)))
+    _check_cuda('ngram_draft', (hist, positions, tokens), hist.device)
+    with torch.cuda.device(hist.device):
+        _lib.check(_lib.load().quip_ngram_draft(hist.data_ptr(), positions.data_ptr(), tokens.data_ptr(), B, max_len,
+                                                tokens.shape[1] - 1, n_min, n_max,
+                                                torch.cuda.current_stream(hist.device).cuda_stream))
+    return tokens
+
+
+def spec_accept(tokens, targets, generated, hist, positions, n_gen, accepted, max_new):
+    """quip_spec_accept: accept the longest matching prefix of drafts plus one token per unfinished row (the rule is in
+    include/quip_b200.h), writing generated (B, >= max_new) and hist (B, max_len) and advancing positions, n_gen and
+    accepted (B,).  int64, CUDA, contiguous."""
+    B, T = tokens.shape
+    _check_i64('spec_accept', tokens=(tokens, (B, T)), targets=(targets, (B, T)),
+               generated=(generated, (B, generated.shape[-1])), hist=(hist, (B, hist.shape[-1])),
+               positions=(positions, (B,)), n_gen=(n_gen, (B,)), accepted=(accepted, (B,)))
+    _check_cuda('spec_accept', (tokens, targets, generated, hist, positions, n_gen, accepted), tokens.device)
+    with torch.cuda.device(tokens.device):
+        _lib.check(_lib.load().quip_spec_accept(tokens.data_ptr(), targets.data_ptr(), generated.data_ptr(),
+                                                hist.data_ptr(), positions.data_ptr(), n_gen.data_ptr(),
+                                                accepted.data_ptr(), B, T, max_new, generated.shape[1], hist.shape[1],
+                                                torch.cuda.current_stream(tokens.device).cuda_stream))
+
+
 def mlp_layout_plan(mlp):
     """The combined index of the three permutations around SiLU(gate) * up of a packed Llama MLP -- the output gathers of
     gate_proj / up_proj (y[j] = layout[u_idx[j]]) and the input gather of down_proj (layout[l] = x[v_idx[l]]) -- so that one

@@ -5,7 +5,8 @@ HBM bandwidth of the H100 SXM data sheet (3.35 TB/s).  Needs a CUDA device.
 
     python tools/generate_bench.py --out DIR [--models llama7b,llama70b] [--layers70b 80] [--steps 16]
                                    [--sections kernel,prefill,decode,fp8]      (fp8kernel: the fp8 kernel rows only;
-                                                                                sample: the sampling rows)
+                                                                                sample: the sampling rows;
+                                                                                spec: speculative generation)
 
 Section fp8 measures the e4m3 KV cache (PromptDecoder(kv_dtype=torch.float8_e4m3fn)): the fp8 kernel alone next to the
 fp16 one (bytes: hd per cached K / V vector plus its 4-byte scale), PromptDecoder steps fp16 against fp8 at B = 32 and
@@ -17,6 +18,13 @@ Section sample times quip_sample (csrc/sample.cu) alone for B in {1, 32, 128} x 
 T = 0.7, k = 50, p = 0.9 and at k = 0, p = 0.9, next to torch.argmax and the torch warper chain (temperature, top-k, sort,
 softmax, cumsum, top-p mask, multinomial) on the same rows, and a 7B PromptDecoder step at B = 32, context 2048, greedy
 against sampling, alternated over three trials.
+
+Section spec measures speculative generation: quip_extend_attention(_fp8) alone next to quip_decode_attention(_fp8)
+(B in {1, 8}, T in {1, 4, 8}, contexts 2048 / 4096, every row's new slots ending at the context); the captured
+SpecDecoder step at T in {2, 4, 5, 6, 8} against the PromptDecoder step on the 7B shape at B in {1, 4}, context 2048
+(t_T / t_1 is the break-even number of tokens a step must yield); and generate() end to end, plain against
+prompt_lookup_num_tokens=4, on a prompt that repeats itself, with the measured acceptance (synthetic weights: the
+acceptance says nothing about real text).
 
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
@@ -255,6 +263,112 @@ def decode_steps_fp8(model, B, ctx, steps, trials=2, kinds=('fp16', 'fp8')):
     return out
 
 
+def extend_alone(nh, nkv, hd, B, T, ctx, fp8, reps):
+    """quip_extend_attention(_fp8) with every row's T new slots ending at slot ctx - 1, and quip_decode_attention(_fp8)
+    at position ctx - 1 on the same cache."""
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(0)
+    k16 = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    v16 = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    q = torch.randn(B, T, nh, hd, generator=g, device='cuda').half()
+    kn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    vn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    sc = {}
+    if fp8:
+        kc = torch.empty(B, nkv, ctx, hd, dtype=torch.float8_e4m3fn, device='cuda')
+        vc = torch.empty_like(kc)
+        sc = dict(k_scale=torch.empty(B, nkv, ctx, device='cuda'), v_scale=torch.empty(B, nkv, ctx, device='cuda'))
+        fused.kv_quantize(k16, kc, sc['k_scale'])
+        fused.kv_quantize(v16, vc, sc['v_scale'])
+        del k16, v16
+    else:
+        kc, vc = k16, v16
+    pos = torch.full((B,), ctx - T, dtype=torch.long, device='cuda')
+    scale = hd ** -0.5
+    ms = events_ms(lambda: fused.extend_attention(q, kn, vn, kc, vc, pos, scale, **sc), reps)
+    pos1 = torch.full((B,), ctx - 1, dtype=torch.long, device='cuda')
+    q1, kn1, vn1 = q[:, 0].contiguous(), kn[:, 0].contiguous(), vn[:, 0].contiguous()
+    ms_dec = events_ms(lambda: fused.decode_attention(q1, kn1, vn1, kc, vc, pos1, scale, **sc), reps)
+    nbytes = attn_bytes([ctx - 1] * B, nkv, hd, fp8=fp8)
+    del kc, vc
+    torch.cuda.empty_cache()
+    return dict(kv='fp8' if fp8 else 'fp16', nh=nh, nkv=nkv, hd=hd, B=B, T=T, context=ctx, extend_ms=ms,
+                decode_ms=ms_dec, bytes=nbytes, extend_bytes_per_s=nbytes / ms * 1e3, decode_bytes_per_s=nbytes / ms_dec * 1e3)
+
+
+def spec_steps(model, B, ctx, Ts, steps, trials=3):
+    """Per-step ms of a captured PromptDecoder (T = 1) and SpecDecoders of T tokens per row, every row starting at
+    position ctx of a cache filled with random values, alternating trial by trial."""
+    from quip_b200.decode import PromptDecoder, SpecDecoder
+    res = {T: [] for T in (1,) + tuple(Ts)}
+    for t in range(trials + 1):
+        for T in res:
+            max_new = steps * T + 2
+            max_len = ctx + max_new + T
+            if T == 1:
+                dec = PromptDecoder(model, max_len=max_len, batch=B, max_new=max_new)
+            else:
+                dec = SpecDecoder(model, max_len=max_len, batch=B, max_new=max_new, draft_tokens=T - 1)
+                dec.hist.random_(0, model.config.vocab_size)
+            dec.k_cache.normal_(0.0, 0.5)
+            dec.v_cache.normal_(0.0, 0.5)
+            dec.capture()
+            with torch.no_grad():
+                for r in range(2):
+                    dec.positions.fill_(ctx)
+                    dec._pos_host = [ctx] * B
+                    dec._t.fill_(1)
+                    dec._t_host = 1
+                    if T > 1:
+                        dec.n_gen.fill_(1)
+                        dec._steps_host = 0
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(steps):
+                        dec.step()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    if r and t:
+                        res[T].append(e0.elapsed_time(e1) / steps)
+            del dec
+            torch.cuda.empty_cache()
+    med = {T: sorted(v)[len(v) // 2] for T, v in res.items()}
+    return dict(B=B, context=ctx, trials_ms={str(k): v for k, v in res.items()}, step_ms={str(k): v for k, v in med.items()},
+                break_even_tokens_per_step={str(T): med[T] / med[1] for T in Ts})
+
+
+def spec_generate(model, B, n_new, k, seg=64, reps=2):
+    """generate() wall time (prefill, capture and the host loop included), plain and with prompt_lookup_num_tokens=k,
+    on prompts made of a random segment repeated 8 times."""
+    import time
+
+    from quip_b200.decode import generate
+    g = torch.Generator().manual_seed(3)
+    prompts = [torch.randint(0, model.config.vocab_size, (seg,), generator=g).repeat(8) for _ in range(B)]
+    out = dict(B=B, prompt=8 * seg, new_tokens=n_new, k=k)
+    for name, kw in (('plain', {}), ('spec', dict(prompt_lookup_num_tokens=k))):
+        times = []
+        for _ in range(reps + 1):
+            stats = {}
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            toks = generate(model, prompts, n_new, spec_stats=stats, **kw) if kw else generate(model, prompts, n_new)
+            torch.cuda.synchronize()
+            times.append(time.perf_counter() - t0)
+        s = sorted(times[1:])[len(times[1:]) // 2]
+        out[f'{name}_s'] = s
+        out[f'{name}_tok_s'] = sum(int(t.numel()) for t in toks) / s
+        if kw:
+            out['accepted'] = stats['accepted']
+            out['steps'] = stats['steps']
+            out['tokens_per_step'] = n_new / (stats['steps'] + 1)
+        else:
+            plain = toks
+    out['same_tokens'] = all(torch.equal(a, b) for a, b in zip(plain, toks))
+    return out
+
+
 def torch_warpers(x, T, k, p):
     """HF-style sampling chain in torch ops: temperature, top-k, top-p over a descending sort, multinomial."""
     z = x.float() / T
@@ -369,7 +483,18 @@ def main():
                         print(f'sample B={B} V={V} k={k} p={p}: kernel {1e3 * r["kernel_ms"]:.1f} us, torch argmax '
                               f'{1e3 * r["torch_argmax_ms"]:.1f} us, torch warpers {1e3 * r["torch_warpers_ms"]:.1f} us',
                               flush=True)
-        if not sections & {'prefill', 'decode', 'fp8', 'sample'}:
+        if 'spec' in sections:
+            rec['extend_kernel'] = []
+            for B in (1, 8):
+                for T in (1, 4, 8):
+                    for ctx in (2048, 4096):
+                        for fp8 in (False, True):
+                            r = extend_alone(nh, nkv, hd, B, T, ctx, fp8, a.kernel_reps)
+                            rec['extend_kernel'].append(r)
+                            print(f'{name} extend kernel {r["kv"]} B={B} T={T} ctx={ctx}: {1e3 * r["extend_ms"]:.1f} us '
+                                  f'({r["extend_bytes_per_s"] / 1e12:.2f} TB/s), decode kernel {1e3 * r["decode_ms"]:.1f} us '
+                                  f'({r["decode_bytes_per_s"] / 1e12:.2f} TB/s)', flush=True)
+        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'}:
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
@@ -394,6 +519,19 @@ def main():
             rec['sample_decode'] = r
             print(f'{name} PromptDecoder B=32 ctx=2048: greedy {r["greedy_ms"]:.3f} ms/step, sampling '
                   f'{r["sampling_ms"]:.3f} ms/step', flush=True)
+        if 'spec' in sections and name == 'llama7b':
+            rec['spec_steps'] = []
+            for B in (1, 4):
+                r = spec_steps(model, B, 2048, (2, 4, 5, 6, 8), a.steps)
+                rec['spec_steps'].append(r)
+                print(f'{name} step cost B={B} ctx=2048: ' + ', '.join(f'T={T} {ms:.3f} ms' for T, ms in r['step_ms'].items()),
+                      flush=True)
+            rec['spec_generate'] = []
+            for B in (1, 4):
+                r = spec_generate(model, B, 128, 4)
+                rec['spec_generate'].append(r)
+                print(f'{name} generate B={B} 128 tokens: plain {r["plain_tok_s"]:.0f} tok/s, k=4 {r["spec_tok_s"]:.0f} '
+                      f'tok/s, {r["tokens_per_step"]:.2f} tokens per step, same tokens {r["same_tokens"]}', flush=True)
         # fp16 against fp8 at B = 32, then the configurations only an e4m3 cache fits (7B 48 x 4096, 70B 64 x 4096)
         runs = [(32, 2048, ('fp16', 'fp8')), (32, 4096, ('fp16', 'fp8'))] if 'fp8' in sections else []
         if 'fp8' in sections:
