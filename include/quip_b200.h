@@ -210,6 +210,42 @@ int quip_spec_accept(const int64_t* tokens, const int64_t* targets, int64_t* gen
 int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,
                          int32_t max_len, int32_t hd, void* stream);
 
+/* Chunked prefill, part 1: append a chunk of new keys and values to one layer of the static KV cache.  k_new / v_new
+ * (B, T, nkv, hd) fp16 token-major; caches (B, nkv, max_len, hd) fp16; positions, counts (B) int64 on the device.  Token
+ * i of row b goes to slot positions[b] + i for i < counts[b]; no other slot, and nothing of a row with counts[b] == 0, is
+ * touched.  A row with positions[b] < 0, counts[b] outside [0, T] or positions[b] + counts[b] > max_len writes nothing.
+ * 1 <= T <= max_len, hd in {64, 128}; pointers 16-byte aligned. */
+int quip_kv_append(const void* k_new, const void* v_new, void* k_cache, void* v_cache, const int64_t* positions,
+                   const int64_t* counts, int32_t B, int32_t T, int32_t nkv, int32_t hd, int32_t max_len, void* stream);
+/* The same into an e4m3 cache: each new head vector is quantized by the rule of quip_decode_attention_fp8 (amax / 448,
+ * round to nearest even, subnormals kept) and stored with its fp32 scale in k_scale / v_scale (B, nkv, max_len). */
+int quip_kv_append_fp8(const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
+                       float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T,
+                       int32_t nkv, int32_t hd, int32_t max_len, void* stream);
+/* Chunked prefill, part 2: causal attention of a chunk of T query tokens per row over the cache that already holds the
+ * chunk (quip_kv_append first).  q (B, T, nh, hd) fp16 token-major, rotary applied; out (B, T, nh, hd) fp16.  For
+ * i < counts[b]
+ *   out[b][i][h] = softmax_j(scale * q[b][i][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b] + i,
+ * and out[b][i] = 0 for counts[b] <= i < T.  No slot past positions[b] + counts[b] - 1 is read.  Flash-attention style:
+ * Q.K^T and P.V on tensor cores (fp16 operands, fp32 accumulation), online softmax in fp32, p rounded once to fp16 per
+ * 64-slot block, one fp16 rounding of the output; no workspace.  1 <= T <= max_len, hd in {64, 128}, nh % nkv == 0,
+ * nh / nkv <= 8; pointers 16-byte aligned.  A row with positions[b] < 0, counts[b] outside [0, T] or positions[b] +
+ * counts[b] > max_len gets NaN outputs.  Deterministic, and a row's result does not depend on the other rows.  At T <= 8
+ * it computes what quip_extend_attention does, to within the rounding of p. */
+int quip_prefill_attention(const void* q, const void* k_cache, const void* v_cache, const int64_t* positions,
+                           const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
+                           int32_t max_len, float scale, void* stream);
+/* The same over an e4m3 cache with per-slot scales (scale pointers 4-byte aligned).  A chunk attends over the quantized
+ * values the cache holds, its own keys and values included (quip_kv_append_fp8 wrote them): the values every later
+ * decode step reads back, the rule of quip_decode_attention_fp8 and quip_extend_attention_fp8.  (Filling the cache by
+ * quip_kv_quantize_fp8 after an fp16 forward instead attends in fp16 and rounds afterwards.)  Per 64-slot block, a
+ * slot's k scale multiplies its score column; its v scale multiplies p before p is rounded to fp16, normalised by the
+ * largest v scale among the query row's visible slots of the block, which multiplies the block's P.V. */
+int quip_prefill_attention_fp8(const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
+                               const float* v_scale, const int64_t* positions, const int64_t* counts, void* out,
+                               int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale,
+                               void* stream);
+
 /* Token selection of one generation step: for each row b of logits (B, V) fp16 contiguous (rows need no alignment),
  * with T = temperature[b], k = top_k[b], p = top_p[b] and s = seed[b] (each (B), device) and t = *step (device; the
  * index of the token being chosen, 0 for the one after the prompt), tokens[b] (int64) is:

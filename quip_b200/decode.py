@@ -57,6 +57,7 @@ class GraphDecoder:
         dt = model.get_input_embeddings().weight.dtype     # fp16 on the GPU path; fp32 in the CPU tests
         self.first, self.last = bool(first), bool(last)
         self.T = 1                                         # tokens per row in a step (SpecDecoder: 1 + drafts)
+        self._tarange = torch.arange(self.T, device=self.dev)
         if self.family == 'llama':
             self.layers = list(model.model.layers)
             self.nkv = getattr(cfg, 'num_key_value_heads', None) or self.nh
@@ -135,8 +136,8 @@ class GraphDecoder:
         learned position table."""
         return self.position
 
-    def _attn_mask(self, pos):
-        """Boolean mask over the cache slots for _attend, broadcast over rows and heads."""
+    def _attn_mask(self, pos, T=1):
+        """Boolean mask over the cache slots for _attend of T tokens per row, broadcast over rows and heads."""
         return (self._arange <= pos)[None, None, None, :]                                  # (1, 1, 1, max_len)
 
     def _attend(self, li, q, k, v, mask, scale):
@@ -153,30 +154,42 @@ class GraphDecoder:
         o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
         return o.transpose(1, 2).reshape(B, 1, nh * hd)
 
-    def _rope_rows(self, pos):
-        """Rotary cos / sin rows of the step's tokens: (1 or B, hd) at T = 1; (B * T, hd), token i of row b at position
+    def _tar(self, T):
+        """arange(T): the offsets of a row's T tokens from its position (a step's own buffer at the step's T)."""
+        return self._tarange if T == self.T else self._arange[:T]
+
+    def _rope_rows(self, pos, T):
+        """Rotary cos / sin rows of T tokens per row: (1 or B, hd) at T = 1; (B * T, hd), token i of row b at position
         pos[b] + i, otherwise."""
-        if self.T > 1:
-            pos = (pos[:, None] + self._tarange).reshape(-1)
+        if T > 1:
+            pos = (pos[:, None] + self._tar(T)).reshape(-1)
         return self.cos.index_select(0, pos), self.sin.index_select(0, pos)
 
     def _advance(self):
         self.position.add_(1)
 
-    # ---- the layers of the stage, three kinds of glue.  Each takes the hidden state entering the stage and returns
-    # (h, pend): the residual stream and a branch output still to be added to it (None when already added).
+    # ---- the layers of the stage, three kinds of glue.  Each takes the hidden state entering the stage, (B, T, hidden)
+    # with T tokens per row (a step's, or a prefill chunk's), and returns (h, pend): the residual stream and a branch
+    # output still to be added to it (None when already added).
+
+    def _layers(self, h):
+        if self.family == 'opt':
+            return self._layers_opt(h)
+        if self.ops is not None:
+            return self._layers_fused(h)
+        return self._layers_llama(h)
 
     # csrc/glue.cu: 4 launches per layer instead of ~30 (at one token every torch elementwise op is a launch-latency-bound
     # graph node); the residual add of a branch rides on the next RMSNorm
     def _layers_fused(self, h):
         ops = self.ops
-        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
+        (B, T), nh, nkv, hd = h.shape[:2], self.nh, self.nkv, self.hd
         pos = self._step_positions()
         h = h.contiguous()
-        cos, sin = self._rope_rows(pos)
+        cos, sin = self._rope_rows(pos, T)
         cos = cos.expand(B * T, hd).contiguous()                                          # one row per token
         sin = sin.expand(B * T, hd).contiguous()
-        mask = self._attn_mask(pos)
+        mask = self._attn_mask(pos, T)
         pend = None
         for li, layer in enumerate(self.layers):
             a, mlp = layer.self_attn, layer.mlp
@@ -195,14 +208,14 @@ class GraphDecoder:
         return h, pend
 
     def _layers_llama(self, h):
-        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
+        (B, T), nh, nkv, hd = h.shape[:2], self.nh, self.nkv, self.hd
         pos = self._step_positions()
-        cos, sin = self._rope_rows(pos)
+        cos, sin = self._rope_rows(pos, T)
         if T == 1:
             cos, sin = cos[:, None, None], sin[:, None, None]                              # (1 or B, 1, 1, hd)
         else:
             cos, sin = cos.view(B, 1, T, hd), sin.view(B, 1, T, hd)
-        mask = self._attn_mask(pos)
+        mask = self._attn_mask(pos, T)
         for li, layer in enumerate(self.layers):
             a = layer.self_attn
             x = layer.input_layernorm(h)
@@ -223,8 +236,8 @@ class GraphDecoder:
     # OPT (modeling_opt.OPTDecoderLayer): pre- or post-LayerNorm, q scaled before the dot product, ReLU between fc1 and fc2;
     # biases live inside the (Quant)Linear modules
     def _layers_opt(self, h):
-        B, T, nh, hd = self.batch, self.T, self.nh, self.hd
-        mask = self._attn_mask(self._step_positions())
+        (B, T), nh, hd = h.shape[:2], self.nh, self.hd
+        mask = self._attn_mask(self._step_positions(), T)
         for li, layer in enumerate(self.layers):
             a, before = layer.self_attn, layer.do_layer_norm_before
             x = layer.self_attn_layer_norm(h) if before else h
@@ -240,24 +253,26 @@ class GraphDecoder:
                 h = layer.final_layer_norm(h)
         return h, None
 
-    def _embed(self):
-        """Token (and, for OPT, learned position: index position + 2) embeddings of the step: (B, T, hidden); tokens is
-        (B,) at T = 1 and (B, T) otherwise."""
-        multi = self.T > 1
+    def _embed(self, tokens=None):
+        """Token (and, for OPT, learned position: index position + 2) embeddings of tokens (default: the step's):
+        (B, T, hidden); tokens is (B,) for one token per row and (B, T) otherwise."""
+        tokens = self.tokens if tokens is None else tokens
+        multi = tokens.dim() == 2
         if self.family == 'llama':
-            return self.model.model.embed_tokens(self.tokens) if multi else self.model.model.embed_tokens(self.tokens)[:, None, :]
+            return self.model.model.embed_tokens(tokens) if multi else self.model.model.embed_tokens(tokens)[:, None, :]
         d = self.model.model.decoder
-        h = d.embed_tokens(self.tokens) if multi else d.embed_tokens(self.tokens)[:, None, :]
+        h = d.embed_tokens(tokens) if multi else d.embed_tokens(tokens)[:, None, :]
         if d.project_in is not None:
             h = d.project_in(h)
         pos = self._step_positions()
         if multi:
-            return h + F.embedding(pos[:, None] + self._tarange + d.embed_positions.offset, d.embed_positions.weight)
+            return h + F.embedding(pos[:, None] + self._tar(tokens.shape[1]) + d.embed_positions.offset,
+                                   d.embed_positions.weight)
         return h + F.embedding(pos + d.embed_positions.offset, d.embed_positions.weight)[:, None]
 
     def _head(self, h, pend):
-        """Final norm (fused with the pending residual add on the glue-kernel path) -> lm_head: logits (B, vocab), or
-        (B, T, vocab) for a step of T > 1 tokens per row."""
+        """Final norm (fused with the pending residual add on the glue-kernel path) -> lm_head: logits (B, vocab) for
+        h (B, 1, hidden), or (B, T, vocab) for T > 1 tokens per row."""
         if self.family == 'llama':
             fn = self.model.model.norm
             if self.ops is not None:
@@ -271,17 +286,12 @@ class GraphDecoder:
             if d.project_out is not None:
                 h = d.project_out(h)
         logits = self.model.lm_head(h)
-        return logits if self.T > 1 else logits[:, 0, :]
+        return logits if h.shape[1] > 1 else logits[:, 0, :]
 
     # one decode step of the stage on the static buffers (what the graph records)
     def _step(self):
         h = self._embed() if self.first else self.h_in
-        if self.family == 'opt':
-            h, pend = self._layers_opt(h)
-        elif self.ops is not None:
-            h, pend = self._layers_fused(h)
-        else:
-            h, pend = self._layers_llama(h)
+        h, pend = self._layers(h)
         if self.last:
             self.logits = self._head(h, pend)
         else:
@@ -387,7 +397,8 @@ class PromptDecoder(GraphDecoder):
       * attention on CUDA is quip_decode_attention (csrc/attn_decode.cu): k / v appended at positions[b] inside the
         kernel, slots 0 .. positions[b] read and no others, GQA without copies.  On the CPU the same step in torch:
         per-row scatter into the cache, SDPA under the mask arange(max_len) <= positions[:, None];
-      * `prefill` fills the cache from a batch of prompts with the model's own many-token forward;
+      * `prefill` fills the cache from a batch of prompts with the model's own many-token forward, or with chunk=C in
+        chunks of C tokens through the step's own layer loops, appended and attended by csrc/attn_prefill.cu;
       * max_new > 0: selection inside the step -- tokens = argmax(logits), stored in generated[:, t] -- so a host loop
         only replays the graph;
       * sampling=True: the selection is quip_sample (csrc/sample.cu) over the device buffers temperature, top_k, top_p
@@ -411,6 +422,7 @@ class PromptDecoder(GraphDecoder):
         self._pos_host = [0] * B
         self._t_host = 0
         self._kernel = self.dev.type == 'cuda'
+        self._chunk = None                       # counts (B,) of the prefill chunk running the layer loops, if any
         self.sampling = bool(sampling)
         if self.sampling:
             self.temperature = torch.ones(B, dtype=torch.float32, device=self.dev)
@@ -475,16 +487,18 @@ class PromptDecoder(GraphDecoder):
     def _step_positions(self):
         return self.positions
 
-    def _attn_mask(self, pos):
-        if self._kernel:
+    def _attn_mask(self, pos, T=1):
+        if self._kernel or self._chunk is not None:                                    # a chunk masks in _attend_chunk
             return None
-        if self.T > 1:                                                                 # (B, 1, T, max_len), causal
-            return (self._arange[None, None] <= (pos[:, None] + self._tarange)[:, :, None])[:, None]
+        if T > 1:                                                                      # (B, 1, T, max_len), causal
+            return (self._arange[None, None] <= (pos[:, None] + self._tar(T))[:, :, None])[:, None]
         return (self._arange[None] <= pos[:, None])[:, None, None, :]                  # (B, 1, 1, max_len)
 
     def _attend(self, li, q, k, v, mask, scale):
         B, nh, nkv, hd = self.batch, self.nh, self.nkv, self.hd
-        if self.T > 1:
+        if self._chunk is not None:
+            return self._attend_chunk(li, q, k, v, scale)
+        if q.shape[2] > 1:
             return self._attend_multi(li, q, k, v, mask, scale)
         if self._kernel:
             from . import fused
@@ -541,6 +555,47 @@ class PromptDecoder(GraphDecoder):
         o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
         return o.transpose(1, 2).reshape(B, T, nh * hd)
 
+    def _attend_chunk(self, li, q, k, v, scale):
+        """_attend for a prefill chunk (q (B, nh, T, hd), k / v (B, nkv, T, hd)) with counts = self._chunk (B,): token
+        i < counts[b] appended at slot positions[b] + i and attending over slots 0 .. positions[b] + i; the outputs of
+        tokens i >= counts[b] are zero and nothing of theirs is written.  CUDA: quip_kv_append(_fp8), then
+        quip_prefill_attention(_fp8).  CPU: per-row scatter of the counted slots, SDPA under the causal mask over the
+        slots below positions[b] + counts[b].  Returns (B, T, nh * hd)."""
+        (B, nh, T, hd), nkv, counts = q.shape, self.nkv, self._chunk
+        sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
+        if self._kernel:
+            from . import fused
+            fused.kv_append(k.transpose(1, 2).contiguous(), v.transpose(1, 2).contiguous(), self.k_cache[li],
+                            self.v_cache[li], self.positions, counts, **sc)
+            o = fused.prefill_attention(q.transpose(1, 2).contiguous(), self.k_cache[li], self.v_cache[li],
+                                        self.positions, counts, scale, **sc)
+            return o.view(B, T, nh * hd)
+        tar = self._tar(T)
+        live = tar[None] < counts[:, None]                                             # (B, T)
+        rows = self._rows[:, None].expand(B, T)[live]
+        slots = (self.positions[:, None] + tar)[live]
+        if self._fp8:
+            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
+                xq, xs = _e4m3_quantize(x.transpose(1, 2)[live])                       # (n, nkv, hd), (n, nkv)
+                cache[rows, :, slots] = xq
+                scales[rows, :, slots] = xs
+            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
+            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
+        else:
+            self.k_cache[li][rows, :, slots] = k.transpose(1, 2)[live]
+            self.v_cache[li][rows, :, slots] = v.transpose(1, 2)[live]
+            kk, vv = self.k_cache[li], self.v_cache[li]
+        seen = (self._arange[None] < (self.positions + counts)[:, None])[:, None, :, None]   # whatever lies past: not read
+        kk, vv = torch.where(seen, kk, 0), torch.where(seen, vv, 0)
+        if nkv != nh:
+            kk = kk.repeat_interleave(nh // nkv, dim=1)
+            vv = vv.repeat_interleave(nh // nkv, dim=1)
+        last = self.positions[:, None] + torch.minimum(tar[None], (counts[:, None] - 1).clamp(min=0))   # (B, T)
+        mask = (self._arange[None, None] <= last[:, :, None])[:, None]                 # (B, 1, T, max_len)
+        o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=mask, scale=scale)
+        o = torch.where(live[:, None, :, None], o, 0)
+        return o.transpose(1, 2).reshape(B, T, nh * hd)
+
     def _advance(self):
         self.positions.add_(1)
         if self.max_new:
@@ -569,16 +624,25 @@ class PromptDecoder(GraphDecoder):
         self._pos_host = [0] * self.batch
         self._t_host = 0
 
-    def prefill(self, prompts):
-        """Fill the cache from `prompts` (B 1-D id tensors): right-padded to the longest, run through the model's own
-        forward (`model.model(ids, attention_mask=..., use_cache=True)`, the packed linears at M = B * P), its keys and
-        values copied to the cache slots 0 .. P-1.  Slots past a row's length hold padding; the step overwrites them in
-        turn and never reads past positions[b].  Returns the logits after each prompt's last token (B, vocab); with
-        max_new > 0 the token selected from them (argmax, or sampled at t = 0) is the first generated token and the next
-        step's input."""
+    def prefill(self, prompts, chunk=None):
+        """Fill the cache from `prompts` (B 1-D id tensors).  Returns the logits after each prompt's last token
+        (B, vocab); with max_new > 0 the token selected from them (argmax, or sampled at t = 0) is the first generated
+        token and the next step's input.
+
+        chunk=None: right-padded to the longest (P), run through the model's own forward (`model.model(ids,
+        attention_mask=..., use_cache=True)`, the packed linears at M = B * P), its keys and values copied (e4m3:
+        quantized) to the cache slots 0 .. P-1.  Slots past a row's length hold padding; the step overwrites them in
+        turn and never reads past positions[b].
+
+        chunk=C (an int >= 1): the prompts in chunks of C tokens through the decoder's own layers, straight into the
+        cache (_prefill_chunks): peak memory follows C, not P, and no fp16 copy of the cache is made.  Only slots
+        0 .. len_b - 1 of row b are written.  With an e4m3 cache every token attends over the quantized keys and values
+        the cache holds, its own included -- what teacher-forced decode steps compute, not the fp16 attention of
+        chunk=None."""
         B = self.batch
         if len(prompts) != B:
             raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
+        chunk = _chunk_size(chunk)
         lens = [int(p.numel()) for p in prompts]
         if min(lens) < 1:
             raise ValueError('empty prompt')
@@ -589,22 +653,56 @@ class PromptDecoder(GraphDecoder):
         for b, p in enumerate(prompts):
             ids[b, :lens[b]] = p.reshape(-1).to(self.dev)
         lens_t = torch.tensor(lens, dtype=torch.long, device=self.dev)
-        attn = (torch.arange(P, device=self.dev)[None] < lens_t[:, None]).long()
         with torch.no_grad():
-            out = self.model.model(input_ids=ids, attention_mask=attn, use_cache=True)
-            cache = out.past_key_values
-            for li in range(len(self.layers)):
-                if self._fp8:
-                    self._store_fp8(li, cache.layers[li].keys, cache.layers[li].values)
-                else:
-                    self.k_cache[li, :, :, :P].copy_(cache.layers[li].keys)
-                    self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
-            logits = self.model.lm_head(out.last_hidden_state[self._rows, lens_t - 1])     # last real token per row
+            if chunk is None:
+                attn = (torch.arange(P, device=self.dev)[None] < lens_t[:, None]).long()
+                out =self.model.model(input_ids=ids, attention_mask=attn, use_cache=True)
+                cache = out.past_key_values
+                for li in range(len(self.layers)):
+                    if self._fp8:
+                        self._store_fp8(li, cache.layers[li].keys, cache.layers[li].values)
+                    else:
+                        self.k_cache[li, :, :, :P].copy_(cache.layers[li].keys)
+                        self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
+                logits = self.model.lm_head(out.last_hidden_state[self._rows, lens_t - 1])     # last real token per row
+            else:
+                logits = self._prefill_chunks(ids, lens, chunk)
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
             if self.max_new:
                 self._first_token(logits)
         return logits
+
+    def _prefill_chunks(self, ids, lens, C):
+        """Chunked prefill of ids (B, P): chunk c0 feeds ids[:, c0:c0 + T], T = min(C, P - c0), with every row at
+        position c0 and counts[b] = clamp(len_b - c0, 0, T) tokens of its own, through the embedding and layer loops
+        of a step (packed linears at M = B * T; attention by _attend_chunk).  Rows whose prompt has ended ride along as
+        padding and write nothing.  The final norm and lm_head run once, on each row's last prompt token, gathered from
+        the chunk it falls in.  Leaves positions at c0 of the last chunk (prefill sets them)."""
+        B, P = ids.shape
+        counts = torch.empty(B, dtype=torch.long, device=self.dev)
+        h_last = p_last = None
+        for c0 in range(0, P, C):
+            T = min(C, P - c0)
+            self.positions.fill_(c0)
+            counts.copy_(torch.tensor([min(max(n - c0, 0), T) for n in lens], dtype=torch.long))
+            self._chunk = counts
+            try:
+                h, pend = self._layers(self._embed(ids[:, c0:c0 + T]))
+            finally:
+                self._chunk = None
+            ends = [b for b in range(B) if c0 < lens[b] <= c0 + T]                     # rows whose last token is here
+            if not ends:
+                continue
+            if h_last is None:
+                h_last = h.new_empty(B, 1, h.shape[-1])
+                p_last = None if pend is None else pend.new_empty(B, 1, pend.shape[-1])
+            r = torch.tensor(ends, dtype=torch.long, device=self.dev)
+            i = torch.tensor([lens[b] - 1 - c0 for b in ends], dtype=torch.long, device=self.dev)
+            h_last[r, 0] = h[r, i]
+            if pend is not None:
+                p_last[r, 0] = pend[r, i]
+        return self._head(h_last, p_last)
 
     def _first_token(self, logits):
         """Select the first generated token from the prefill's logits (B, vocab), at t = 0."""
@@ -731,13 +829,14 @@ class SpecDecoder(PromptDecoder):
             t.zero_()
         self._steps_host = 0
 
-    def prefill(self, prompts):
-        """PromptDecoder.prefill, plus the history: each prompt and its first generated token in hist, n_gen = 1."""
+    def prefill(self, prompts, chunk=None):
+        """PromptDecoder.prefill (chunk as there), plus the history: each prompt and its first generated token in hist,
+        n_gen = 1."""
         lens = [int(torch.as_tensor(p).numel()) for p in prompts]
         if lens and max(lens) + self.max_new + self.k > self.max_len:
             raise ValueError(f'a prompt of {max(lens)} tokens, {self.max_new} new ones and {self.k} drafts exceed the '
                              f'cache of {self.max_len} positions')
-        logits = super().prefill(prompts)
+        logits = super().prefill(prompts, chunk=chunk)
         with torch.no_grad():
             for b, p in enumerate(prompts):
                 self.hist[b, :lens[b]] = torch.as_tensor(p).reshape(-1).to(self.dev)
@@ -881,6 +980,15 @@ def _sample_torch(logits, temperature, top_k, top_p, seed, t):
 EOS_CHECK_EVERY = 16
 
 
+def _chunk_size(chunk):
+    """A prefill chunk size: None (one many-token forward of the whole prompts) or an int >= 1."""
+    if chunk is None:
+        return None
+    if isinstance(chunk, bool) or not isinstance(chunk, int) or chunk < 1:
+        raise ValueError(f'the prefill chunk size must be None or an integer >= 1, got {chunk!r}')
+    return chunk
+
+
 def _per_prompt(name, v, n):
     """A generate() setting as one value per prompt: a scalar for all, or a list / 1-D tensor of n."""
     if torch.is_tensor(v):
@@ -915,7 +1023,7 @@ def _sampling_settings(n, temperature, top_k, top_p, seed):
 
 def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
-             spec_stats=None):
+             spec_stats=None, prefill_chunk_size=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -934,7 +1042,13 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     own prompt and output, and keeps the drafts the model itself would have chosen plus one more token.  The tokens are
     the ones plain generation selects from the same logits (greedy or sampled, with the same seeds); only the step's
     arithmetic differs (other token counts take other kernel routes).  The default max_len grows by k.  spec_stats: a
-    dict that receives 'accepted' (drafts taken per row) and 'steps'."""
+    dict that receives 'accepted' (drafts taken per row) and 'steps'.
+
+    prefill_chunk_size=C (an int >= 1; default None: one many-token forward of the padded prompts) prefills in chunks
+    of C tokens straight into the KV cache (PromptDecoder.prefill(chunk=C)): the prefill's peak memory is bounded by C
+    instead of the prompt length, with no fp16 copy of the cache.  With an e4m3 cache the prompt then attends over its
+    own quantized keys and values, as the decode steps do."""
+    prefill_chunk_size = _chunk_size(prefill_chunk_size)
     prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
     max_new_tokens = int(max_new_tokens)
     if not prompts:
@@ -977,7 +1091,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         dec.set_sampling(*settings)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()
-    dec.prefill(prompts)
+    dec.prefill(prompts, chunk=prefill_chunk_size)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
     if spec:
         return _generate_spec(dec, max_new_tokens, eos_t, spec_stats)

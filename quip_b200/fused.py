@@ -266,6 +266,83 @@ def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
     return out
 
 
+def _check_chunk(fn, k_cache, v_cache, positions, counts, k_scale, v_scale):
+    """The checks kv_append and prefill_attention share: cache and scale dtypes, positions / counts (B,) int64.
+    Returns whether the caches are e4m3."""
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn caches only')
+    if fp8 and (k_scale is None or v_scale is None):
+        raise ValueError(f'{fn}: float8_e4m3fn caches need k_scale and v_scale')
+    cdt = torch.float8_e4m3fn if fp8 else torch.float16
+    if (k_cache.dtype != cdt or v_cache.dtype != cdt or positions.dtype != torch.int64 or counts.dtype != torch.int64 or
+            (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
+        raise ValueError(f'{fn} takes fp16 or float8_e4m3fn caches (fp32 scales) and int64 positions and counts')
+    if k_cache.dim() != 4:
+        raise ValueError(f'{fn}: the caches must be (B, nkv, max_len, hd), got {tuple(k_cache.shape)}')
+    B, nkv, max_len, _ = k_cache.shape
+    if (v_cache.shape != k_cache.shape or tuple(positions.shape) != (B,) or tuple(counts.shape) != (B,) or
+            (fp8 and (tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape))):
+        raise ValueError(f'{fn}: shapes caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
+                         f'{tuple(positions.shape)}, counts {tuple(counts.shape)} do not agree')
+    return fp8
+
+
+def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v_scale=None):
+    """quip_kv_append(_fp8) on torch tensors: token i of k_new / v_new (B, T, nkv, hd) fp16 to slot positions[b] + i of
+    one layer's caches (B, nkv, max_len, hd) for i < counts[b]; nothing else is written.  fp16 caches, or
+    float8_e4m3fn caches with fp32 k_scale / v_scale (B, nkv, max_len), quantized on the way.  CUDA, one device,
+    contiguous; positions / counts (B,) int64.  On the current stream."""
+    fp8 = _check_chunk('kv_append', k_cache, v_cache, positions, counts, k_scale, v_scale)
+    if k_new.dtype != torch.float16 or v_new.dtype != torch.float16:
+        raise ValueError('kv_append takes fp16 k_new / v_new')
+    B, nkv, max_len, hd = k_cache.shape
+    if k_new.dim() != 4 or k_new.shape[0] != B or tuple(k_new.shape[2:]) != (nkv, hd) or v_new.shape != k_new.shape:
+        raise ValueError(f'kv_append: k_new {tuple(k_new.shape)} / v_new {tuple(v_new.shape)} must be (B, T, nkv, hd) '
+                         f'for caches {tuple(k_cache.shape)}')
+    T = k_new.shape[1]
+    ts = (k_new, v_new, k_cache, v_cache, positions, counts) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('kv_append', ts, k_new.device)
+    lib, st = _lib.load(), torch.cuda.current_stream(k_new.device).cuda_stream
+    with torch.cuda.device(k_new.device):
+        if fp8:
+            _lib.check(lib.quip_kv_append_fp8(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                              k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
+                                              counts.data_ptr(), B, T, nkv, hd, max_len, st))
+        else:
+            _lib.check(lib.quip_kv_append(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                          positions.data_ptr(), counts.data_ptr(), B, T, nkv, hd, max_len, st))
+
+
+def prefill_attention(q, k_cache, v_cache, positions, counts, scale, k_scale=None, v_scale=None):
+    """quip_prefill_attention(_fp8) on torch tensors: q (B, T, nh, hd) fp16 attends causally over one layer's caches
+    (B, nkv, max_len, hd), which already hold the chunk (kv_append): token i of row b over slots 0 .. positions[b] + i
+    for i < counts[b]; rows i >= counts[b] are zero.  fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale.
+    CUDA, one device, contiguous; positions / counts (B,) int64.  Returns (B, T, nh, hd) fp16, on the current stream."""
+    fp8 = _check_chunk('prefill_attention', k_cache, v_cache, positions, counts, k_scale, v_scale)
+    if q.dtype != torch.float16 or q.dim() != 4:
+        raise ValueError(f'prefill_attention: q must be (B, T, nh, hd) fp16, got {tuple(q.shape)} {q.dtype}')
+    B, T, nh, hd = q.shape
+    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
+    if tuple(k_cache.shape) != (B, nkv, max_len, hd):
+        raise ValueError(f'prefill_attention: q {tuple(q.shape)} and caches {tuple(k_cache.shape)} do not agree')
+    ts = (q, k_cache, v_cache, positions, counts) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('prefill_attention', ts, q.device)
+    out = torch.empty_like(q)
+    lib, st = _lib.load(), torch.cuda.current_stream(q.device).cuda_stream
+    with torch.cuda.device(q.device):
+        if fp8:
+            _lib.check(lib.quip_prefill_attention_fp8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                      k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
+                                                      counts.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,
+                                                      C.c_float(scale), st))
+        else:
+            _lib.check(lib.quip_prefill_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                  positions.data_ptr(), counts.data_ptr(), out.data_ptr(), B, T, nh, nkv,
+                                                  hd, max_len, C.c_float(scale), st))
+    return out
+
+
 def sample_at(logits, temperature, top_k, top_p, seed, steps, out):
     """quip_sample_at: logits (B, T, V) fp16 -> out (B, T) int64, token i of row b by the rule of quip_sample with row b's
     settings and seed at step steps[b] + i (steps (B,) int64).  CUDA, one device, contiguous; on the current stream."""

@@ -26,6 +26,13 @@ SpecDecoder step at T in {2, 4, 5, 6, 8} against the PromptDecoder step on the 7
 prompt_lookup_num_tokens=4, on a prompt that repeats itself, with the measured acceptance (synthetic weights: the
 acceptance says nothing about real text).
 
+Section chunked measures chunked prefill (PromptDecoder.prefill(chunk=C), csrc/attn_prefill.cu): the prefill-attention
+kernel alone in causal TFLOP/s against F.scaled_dot_product_attention(is_causal=True) on the same fp16 q / k / v (B in
+{1, 8}, T in {512, 2048} at position 0, fp16 and e4m3 caches), the extend kernel against append + prefill at T = 8; on the
+7B shape, tokens/s and peak allocation of the HF-path prefill against chunks of 256 .. 2048 tokens, and an e4m3 cache of
+48 x 4096 filled from 4000-token prompts in chunks of 512 followed by decode steps, with the fp16 cache bytes the HF path
+would have added.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -436,6 +443,132 @@ def sample_steps(model, B, ctx, steps, trials=3):
     return out
 
 
+def causal_flops(nh, hd, B, pos, T):
+    """Q.K^T and P.V flops of causal attention: sum_i 4 * (pos + i + 1) * hd per query head."""
+    return B * nh * 4 * hd * (T * (pos + 1) + T * (T - 1) // 2)
+
+
+def prefill_kernel_alone(nh, nkv, hd, B, T, fp8, reps):
+    """quip_prefill_attention(_fp8) of T tokens per row at position 0 (the cache already appended), in causal TFLOP/s,
+    next to F.scaled_dot_product_attention(is_causal=True) on the same fp16 q / k / v (GQA expanded outside the
+    timing)."""
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(0)
+    q = torch.randn(B, T, nh, hd, generator=g, device='cuda').half()
+    kn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    vn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    pos = torch.zeros(B, dtype=torch.long, device='cuda')
+    cnt = torch.full((B,), T, dtype=torch.long, device='cuda')
+    if fp8:
+        kc = torch.zeros(B, nkv, T, hd, dtype=torch.float8_e4m3fn, device='cuda')
+        sc = dict(k_scale=torch.zeros(B, nkv, T, device='cuda'), v_scale=torch.zeros(B, nkv, T, device='cuda'))
+    else:
+        kc, sc = torch.zeros(B, nkv, T, hd, dtype=torch.float16, device='cuda'), {}
+    vc = torch.zeros_like(kc)
+    fused.kv_append(kn, vn, kc, vc, pos, cnt, **sc)
+    scale = hd ** -0.5
+    ms = events_ms(lambda: fused.prefill_attention(q, kc, vc, pos, cnt, scale, **sc), reps)
+    got = fused.prefill_attention(q, kc, vc, pos, cnt, scale, **sc)
+    qt = q.transpose(1, 2).contiguous()
+    kt = kn.transpose(1, 2).repeat_interleave(nh // nkv, dim=1).contiguous()
+    vt = vn.transpose(1, 2).repeat_interleave(nh // nkv, dim=1).contiguous()
+    sdpa = torch.nn.functional.scaled_dot_product_attention
+    ms_sdpa = events_ms(lambda: sdpa(qt, kt, vt, is_causal=True, scale=scale), reps)
+    ref = sdpa(qt, kt, vt, is_causal=True, scale=scale).transpose(1, 2)
+    fl = causal_flops(nh, hd, B, 0, T)
+    del kc, vc, kt, vt
+    torch.cuda.empty_cache()
+    return dict(kv='fp8' if fp8 else 'fp16', nh=nh, nkv=nkv, hd=hd, B=B, T=T, pos=0, kernel_ms=ms,
+                kernel_tflops=fl / ms / 1e9, sdpa_ms=ms_sdpa, sdpa_tflops=fl / ms_sdpa / 1e9, rel_err_vs_sdpa=rel(got, ref))
+
+
+def extend_vs_prefill(nh, nkv, hd, B, ctx, reps, T=8):
+    """A step of T new tokens per row ending at slot ctx - 1: quip_extend_attention (append included) against
+    quip_kv_append + quip_prefill_attention on the same fp16 cache."""
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(0)
+    kc = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    vc = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    q = torch.randn(B, T, nh, hd, generator=g, device='cuda').half()
+    kn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    vn = torch.randn(B, T, nkv, hd, generator=g, device='cuda').half()
+    pos = torch.full((B,), ctx - T, dtype=torch.long, device='cuda')
+    cnt = torch.full((B,), T, dtype=torch.long, device='cuda')
+    scale = hd ** -0.5
+    ms_ext = events_ms(lambda: fused.extend_attention(q, kn, vn, kc, vc, pos, scale), reps)
+
+    def pair():
+        fused.kv_append(kn, vn, kc, vc, pos, cnt)
+        return fused.prefill_attention(q, kc, vc, pos, cnt, scale)
+    ms_pf = events_ms(pair, reps)
+    err = rel(pair(), fused.extend_attention(q, kn, vn, kc, vc, pos, scale))
+    del kc, vc
+    torch.cuda.empty_cache()
+    return dict(nh=nh, nkv=nkv, hd=hd, B=B, T=T, context=ctx, extend_ms=ms_ext, append_prefill_ms=ms_pf,
+                rel_err=err)
+
+
+def _peak(fn):
+    """(ms, peak bytes allocated above the start) of one call of fn."""
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    base = torch.cuda.memory_allocated()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1), torch.cuda.max_memory_allocated() - base
+
+
+def chunked_prefill_rates(model, B, P, chunks, reps=2):
+    """Tokens/s and peak allocation above the static cache of the HF-path prefill and of chunked prefills (fp16 cache);
+    each timed call follows one warm-up call of the same kind."""
+    from quip_b200.decode import PromptDecoder
+    g = torch.Generator().manual_seed(3)
+    prompts = [torch.randint(0, model.config.vocab_size, (P,), generator=g) for _ in range(B)]
+    dec = PromptDecoder(model, max_len=P, batch=B)
+    rows = []
+    with torch.no_grad():
+        for C in (None,) + tuple(c for c in chunks if c <= P):
+            dec.prefill(prompts, chunk=C)
+            res = [_peak(lambda: dec.prefill(prompts, chunk=C)) for _ in range(reps)]
+            ms = sorted(r[0] for r in res)[len(res) // 2]
+            rows.append(dict(B=B, P=P, chunk=C, ms=ms, tokens_per_s=B * P * 1e3 / ms, peak_bytes=max(r[1] for r in res)))
+    del dec
+    torch.cuda.empty_cache()
+    return rows
+
+
+def chunked_capacity(model, cfg, B, P, max_len, C, steps):
+    """The configuration the HF path cannot run: an e4m3 cache of B x max_len, prompts of P tokens prefilled in chunks
+    of C, then `steps` captured decode steps; with the bytes the HF path would have needed on top of the static cache."""
+    from quip_b200.decode import PromptDecoder
+    g = torch.Generator().manual_seed(4)
+    prompts = [torch.randint(0, cfg.vocab_size, (P,), generator=g) for _ in range(B)]
+    L = cfg.num_hidden_layers
+    hf_cache = cache_bytes(cfg, L, B, P)                              # the HF DynamicCache of the padded prompts (fp16)
+    free = torch.cuda.mem_get_info()[0]
+    dec = PromptDecoder(model, max_len=max_len, batch=B, max_new=steps + 1, kv_dtype=torch.float8_e4m3fn).capture()
+    static = cache_bytes(cfg, L, B, max_len, fp8=True)
+    with torch.no_grad():
+        ms_prefill, peak = _peak(lambda: dec.prefill(prompts, chunk=C))
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            dec.step()
+        e1.record()
+        torch.cuda.synchronize()
+    out = dict(kv='fp8', B=B, P=P, max_len=max_len, chunk=C, prefill_ms=ms_prefill, prefill_tokens_per_s=B * P * 1e3 / ms_prefill,
+               prefill_peak_bytes_above_cache=peak, decode_steps=steps, decode_ms_per_step=e0.elapsed_time(e1) / steps,
+               static_cache_bytes=static, hf_path_fp16_cache_bytes=hf_cache, free_bytes_before=free,
+               positions=sorted(set(dec.positions.tolist())), tokens_finite=bool(torch.isfinite(dec.logits.float()).all()))
+    del dec
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -494,9 +627,38 @@ def main():
                             print(f'{name} extend kernel {r["kv"]} B={B} T={T} ctx={ctx}: {1e3 * r["extend_ms"]:.1f} us '
                                   f'({r["extend_bytes_per_s"] / 1e12:.2f} TB/s), decode kernel {1e3 * r["decode_ms"]:.1f} us '
                                   f'({r["decode_bytes_per_s"] / 1e12:.2f} TB/s)', flush=True)
-        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'}:
+        if 'chunked' in sections:
+            rec['prefill_kernel'], rec['extend_vs_prefill'] = [], []
+            for fp8 in (False, True):
+                for B in (1, 8):
+                    for T in (512, 2048):
+                        r = prefill_kernel_alone(nh, nkv, hd, B, T, fp8, max(a.kernel_reps // 10, 10))
+                        rec['prefill_kernel'].append(r)
+                        print(f'{name} prefill kernel {r["kv"]} B={B} T={T}: {r["kernel_ms"]:.3f} ms '
+                              f'({r["kernel_tflops"]:.0f} TFLOP/s), SDPA causal {r["sdpa_ms"]:.3f} ms '
+                              f'({r["sdpa_tflops"]:.0f} TFLOP/s), rel err {r["rel_err_vs_sdpa"]:.1e}', flush=True)
+            for B in (1, 8):
+                r = extend_vs_prefill(nh, nkv, hd, B, 2048, a.kernel_reps)
+                rec['extend_vs_prefill'].append(r)
+                print(f'{name} T=8 B={B} ctx=2048: extend {1e3 * r["extend_ms"]:.1f} us, append + prefill '
+                      f'{1e3 * r["append_prefill_ms"]:.1f} us, rel err {r["rel_err"]:.1e}', flush=True)
+        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not ('chunked' in sections and
+                                                                                  name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
+        if 'chunked' in sections and name == 'llama7b':
+            rec['chunked_prefill'] = []
+            for B, P in ((1, 2048), (8, 512), (8, 2048)):
+                for r in chunked_prefill_rates(model, B, P, (256, 512, 1024, 2048)):
+                    rec['chunked_prefill'].append(r)
+                    print(f'{name} prefill {B}x{P} chunk={r["chunk"]}: {r["ms"]:.1f} ms, {r["tokens_per_s"]:.0f} '
+                          f'tokens/s, peak {r["peak_bytes"] / 2**30:.2f} GiB above the cache', flush=True)
+            r = chunked_capacity(model, cfg, 48, 4000, 4096, 512, a.steps)
+            rec['chunked_capacity'] = r
+            print(f'{name} e4m3 B=48 P=4000 chunk=512: prefill {r["prefill_ms"] / 1e3:.1f} s '
+                  f'({r["prefill_tokens_per_s"]:.0f} tokens/s, peak {r["prefill_peak_bytes_above_cache"] / 2**30:.2f} GiB '
+                  f'above the {r["static_cache_bytes"] / 2**30:.1f} GiB cache), {r["decode_ms_per_step"]:.2f} ms/step; the '
+                  f'HF path would add {r["hf_path_fp16_cache_bytes"] / 2**30:.1f} GiB of fp16 cache', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
