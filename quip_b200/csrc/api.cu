@@ -34,7 +34,7 @@ int qgemm_tc(const QuipLinearDesc* d, const __half* x, const float* xsum, const 
              cudaStream_t s);
 
 extern int g_gather_rows, g_pass_min_tiles, g_fewtok;   // rot.cu
-extern int g_fewtok_max_m;                               // rot_fewtok.cu: token count up to which the few-token kernels run (8)
+extern int g_fewtok_max_m;                               // rot_fewtok.cu: token count up to which the few-token kernels run (32)
 bool side_fused_ok(const QuipSide* sd, int n);               // rot_side.cu
 int side_fused(const QuipSide* sd, const __half* in, __half* out, int64_t M, const int32_t* in_idx, const float* in_scale,
                const int32_t* out_idx, const __half* out_bias, float* xsum, cudaStream_t s);
