@@ -129,6 +129,10 @@ def load():
         if lib.quip_abi_version() != ABI_VERSION:
             raise QuipError('libquip_b200.so ABI version mismatch')
         _lib = lib
+        # weight rows per 2-bit GEMM tile above 64 tokens: 128 or 256 forces one kernel, 0 (default) picks by shape
+        rows = os.environ.get('QUIP_TC_ROWS')
+        if rows:
+            check(lib.quip_config(b'tc_rows', int(rows)))
     return _lib
 
 

@@ -11,6 +11,12 @@ constexpr int TC_BM = 128;            // output rows per tile: two consumer warp
 constexpr int TC_BK = 64;             // k per stage = one 128-byte swizzle atom of fp16
 constexpr int TC_CONSUMER_WARPS = 8;  // warps 0-7: two consumer warpgroups (wgmma + epilogue)
 constexpr int TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;   // + one TMA warp
+// 256-row packed tiles: 128 accumulators per consumer thread.  ptxas sizes a wgmma kernel's registers by whole
+// warpgroups (at most 168 for 288 or 384 threads), so those tiles run a full producer warpgroup that gives its registers
+// to the consumers with setmaxnreg: 128 x 40 + 256 x 232 <= 64K.
+constexpr int TC_THREADS_TALL = 32 * TC_CONSUMER_WARPS + 128;
+constexpr int TC_TALL_PRODUCER_REGS = 40;
+constexpr int TC_TALL_CONSUMER_REGS = 232;
 constexpr uint32_t TC_WATCHDOG = 1u << 28;
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
