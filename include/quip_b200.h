@@ -246,6 +246,53 @@ int quip_prefill_attention_fp8(const void* q, const void* k_cache, const void* v
                                int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale,
                                void* stream);
 
+/* Paged KV cache.  Per layer, k_pool / v_pool (n_pages, nkv, 64, hd) hold fp16 or e4m3fn values (e4m3: with k_scale /
+ * v_scale (n_pages, nkv, 64) fp32, the format of quip_decode_attention_fp8); a page holds 64 slots of every kv head.
+ * page_table (B, max_pages) int32 on the device, shared by all layers: slot j of row b lives at slot j % 64 of page
+ * page_table[b][j / 64].  Rows may map the same page (a shared prompt prefix).  A page id outside [0, n_pages) -- the
+ * -1 of an unmapped entry, say -- follows the rule of a position outside the cache: it is never dereferenced, nothing
+ * is written through it, and every output of a token that would read or write a slot on that page is NaN.  Pages past
+ * the slots a launch reads or writes are not looked up.
+ *
+ * Each entry point below takes the arguments of its contiguous twin with the caches replaced by the pools and max_len by
+ * (page_table, max_pages, n_pages); max_len = max_pages * 64 everywhere it mattered (decode chunking, grids, the
+ * workspace sizes of quip_decode_attention_workspace_bytes / quip_extend_attention_workspace_bytes), so a paged launch
+ * runs the contiguous launch's blocks and arithmetic: its results are bit-identical to the contiguous launch over the
+ * same cached bytes.  page_table 4-byte aligned, 0 < max_pages <= 2^31 / 64, n_pages > 0. */
+int quip_decode_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
+                                float scale, void* workspace, size_t workspace_bytes, const int32_t* page_table,
+                                int32_t max_pages, int32_t n_pages, void* stream);
+int quip_decode_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                    float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
+                                    int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
+                                    size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
+                                    int32_t n_pages, void* stream);
+int quip_extend_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
+                                int32_t hd, float scale, void* workspace, size_t workspace_bytes,
+                                const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
+int quip_extend_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                    float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
+                                    int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
+                                    size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
+                                    int32_t n_pages, void* stream);
+int quip_kv_append_paged(const void* k_new, const void* v_new, void* k_pool, void* v_pool, const int64_t* positions,
+                         const int64_t* counts, int32_t B, int32_t T, int32_t nkv, int32_t hd,
+                         const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
+int quip_kv_append_paged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool, float* k_scale,
+                             float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T,
+                             int32_t nkv, int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                             void* stream);
+int quip_prefill_attention_paged(const void* q, const void* k_pool, const void* v_pool, const int64_t* positions,
+                                 const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
+                                 int32_t hd, float scale, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                 void* stream);
+int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale,
+                                     const float* v_scale, const int64_t* positions, const int64_t* counts, void* out,
+                                     int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale,
+                                     const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
+
 /* Token selection of one generation step: for each row b of logits (B, V) fp16 contiguous (rows need no alignment),
  * with T = temperature[b], k = top_k[b], p = top_p[b] and s = seed[b] (each (B), device) and t = *step (device; the
  * index of the token being chosen, 0 for the one after the prompt), tokens[b] (int64) is:

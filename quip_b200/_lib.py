@@ -90,6 +90,25 @@ EXPORTS = {
     'quip_prefill_attention_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                              C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
+    'quip_decode_attention_paged': (C.c_int, [C.c_void_p] * 7 + [C.c_int32] * 4 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                  C.c_void_p, C.c_int32, C.c_int32,
+                                                                                  C.c_void_p]),
+    'quip_decode_attention_paged_fp8': (C.c_int, [C.c_void_p] * 9 + [C.c_int32] * 4 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                      C.c_void_p, C.c_int32, C.c_int32,
+                                                                                      C.c_void_p]),
+    'quip_extend_attention_paged': (C.c_int, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                  C.c_void_p, C.c_int32, C.c_int32,
+                                                                                  C.c_void_p]),
+    'quip_extend_attention_paged_fp8': (C.c_int, [C.c_void_p] * 9 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                      C.c_void_p, C.c_int32, C.c_int32,
+                                                                                      C.c_void_p]),
+    'quip_kv_append_paged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    'quip_kv_append_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_int32,
+                                                                               C.c_void_p]),
+    'quip_prefill_attention_paged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
+                                                                                   C.c_int32, C.c_void_p]),
+    'quip_prefill_attention_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
+                                                                                       C.c_int32, C.c_void_p]),
     'quip_ngram_draft':(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p]),
     'quip_spec_accept': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -34,7 +34,7 @@ def build(force=False, verbose=False):
     flags = ' '.join([NVCC] + FLAGS)
     if not os.path.exists(stamp) or open(stamp).read() != flags:
         force = True
-    headers = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'), os.path.join(CSRC, 'kv_fp8.cuh'),
+    headers = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'), os.path.join(CSRC, 'kv_fp8.cuh'), os.path.join(CSRC, 'kv_page.cuh'),
                os.path.join(os.path.dirname(HERE), 'include', 'quip_b200.h')]
     jobs = []
     for src in SOURCES:

@@ -43,6 +43,7 @@
 
 #include "common.cuh"
 #include "kv_fp8.cuh"
+#include "kv_page.cuh"
 
 namespace quip {
 
@@ -91,12 +92,13 @@ struct AttnFp8Smem<false, HD> {};
 
 // Partials: o  [B][nh][nsplit][HD] fp32, then ml [B][nh][nsplit][2] fp32 (running max, sum of exp).
 // FP8: kc / vc hold e4m3 bytes with one fp32 scale per slot in ksc / vsc (same (row, slot) index); fp16: ksc / vsc unused.
-template <bool FP8, int HD, int G>
+// PAGED: kc / vc (and ksc / vsc) are the page pools and pg the page table (kv_page.cuh); a chunk spans at most two pages.
+template <bool FP8, bool PAGED, int HD, int G>
 __global__ void __launch_bounds__(AD_THREADS)
 attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict__ k_new, const __half* __restrict__ v_new,
                          void* __restrict__ kc, void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
                          const int64_t* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml,
-                         int nh, int nkv, int max_len, int nsplit, int chunk, float scale) {
+                         KvPages pg, int nh, int nkv, int max_len, int nsplit, int chunk, float scale) {
   using CT = std::conditional_t<FP8, uint8_t, __half>;   // cache element
   using LT = std::conditional_t<FP8, uint2, uint4>;      // a lane's 8 elements of a slot
   constexpr int U = FP8 ? AD_U8 : AD_U;
@@ -116,25 +118,42 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sg = tid / LPS, sl = tid % LPS;
 
+  // head-vector index of chunk slot j (kv_page.cuh): the chunk's pages are looked up once, here.  A page outside the
+  // pool is not dereferenced: the chunk's partials are NaN, so the combine gives the row NaN, and nothing is written.
+  const int64_t v0 = kv_vec<PAGED>(pg, b, kvh, nkv, max_len, start);
+  const int64_t v1 = PAGED && n > KV_PAGE ? kv_vec<PAGED>(pg, b, kvh, nkv, max_len, start + KV_PAGE) : v0 + KV_PAGE;
+  if (PAGED && (v0 < 0 || v1 < 0)) {
+    if (tid < G) {
+      float* ml = part_ml + (((int64_t)b * nh + (int64_t)kvh * G + tid) * nsplit + split) * 2;
+      ml[0] = NAN;
+      ml[1] = NAN;
+    }
+    return;
+  }
+  auto slot = [&](int j) -> int64_t {
+    if constexpr (PAGED) return (j < KV_PAGE ? v0 : v1 - KV_PAGE) + j;
+    else return v0 + j;
+  };
+
   const int64_t row = (int64_t)b * nkv + kvh;
   const __half* kn = k_new + row * HD;
   const __half* vn = v_new + row * HD;
-  CT* kr = reinterpret_cast<CT*>(kc) + row * (int64_t)max_len * HD;
-  CT* vr = reinterpret_cast<CT*>(vc) + row * (int64_t)max_len * HD;
+  CT* kr = reinterpret_cast<CT*>(kc);
+  CT* vr = reinterpret_cast<CT*>(vc);
   float ks = 0.f, vs = 0.f;                   // FP8: the scales of slot start + tid, in flight during the scores
   if constexpr (FP8) {
     if (tid < n && tid != rel) {
-      ks = ksc[row * max_len + start + tid];
-      vs = vsc[row * max_len + start + tid];
+      ks = ksc[slot(tid)];
+      vs = vsc[slot(tid)];
     }
     if (rel < chunk) {                        // append: this CTA owns slot pos; warp 0 quantizes k_new, warp 1 v_new
       if (warp < 2) {
         float s;
         const uint32_t w = e4m3_quantize_warp<HD>(warp ? vn : kn, lane, s);
-        e4m3_store_warp<HD>((warp ? vr : kr) + pos * HD, lane, w);
+        e4m3_store_warp<HD>((warp ? vr : kr) + slot(rel) * HD, lane, w);
         e4m3_store_warp<HD>(f8.q[warp], lane, w);
         if (lane == 0) {
-          (warp ? vsc : ksc)[row * max_len + pos] = s;
+          (warp ? vsc : ksc)[slot(rel)] = s;
           f8.qs[warp] = s;
         }
       }
@@ -142,8 +161,8 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
     }
   } else if (rel < chunk && tid < 2 * LPS) {  // append: this CTA owns slot pos
     const int c = tid % LPS;
-    if (tid < LPS) reinterpret_cast<uint4*>(kr + pos * HD)[c] = reinterpret_cast<const uint4*>(kn)[c];
-    else reinterpret_cast<uint4*>(vr + pos * HD)[c] = reinterpret_cast<const uint4*>(vn)[c];
+    if (tid < LPS) reinterpret_cast<uint4*>(kr + slot(rel) * HD)[c] = reinterpret_cast<const uint4*>(kn)[c];
+    else reinterpret_cast<uint4*>(vr + slot(rel) * HD)[c] = reinterpret_cast<const uint4*>(vn)[c];
   }
 
   // q of the G heads sharing this kv head: the lane's 8 dims of each, in registers
@@ -161,10 +180,10 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
     for (int u = 0; u < U; ++u) {
       const int j = min(jb + u * SG + sg, n - 1);
       if constexpr (FP8) {
-        const void* src = j == rel ? (const void*)kn : (const void*)(kr + (int64_t)(start + j) * HD);
+        const void* src = j == rel ? (const void*)kn : (const void*)(kr + slot(j) * HD);
         raw[u] = ldg_nc_v2(reinterpret_cast<const uint2*>(src) + sl);
       } else {
-        const __half* src = j == rel ? kn : kr + (int64_t)(start + j) * HD;
+        const __half* src = j == rel ? kn : kr + slot(j) * HD;
         raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
       }
     }
@@ -240,10 +259,10 @@ attn_decode_split_kernel(const __half* __restrict__ q, const __half* __restrict_
     for (int u = 0; u < U; ++u) {
       const int j = min(jb + u * SG + sg, n - 1);
       if constexpr (FP8) {
-        const void* src = j == rel ? (const void*)vn : (const void*)(vr + (int64_t)(start + j) * HD);
+        const void* src = j == rel ? (const void*)vn : (const void*)(vr + slot(j) * HD);
         raw[u] = ldg_nc_v2(reinterpret_cast<const uint2*>(src) + sl);
       } else {
-        const __half* src = j == rel ? vn : vr + (int64_t)(start + j) * HD;
+        const __half* src = j == rel ? vn : vr + slot(j) * HD;
         raw[u] = ldg_nc_v4(reinterpret_cast<const uint4*>(src) + sl);
       }
     }
@@ -351,12 +370,13 @@ __device__ __forceinline__ uint32_t h2_pack(__half lo, __half hi) {
 }
 
 // Partials: o [B][T][nh][nsplit][HD], ml [B][T][nh][nsplit][2], the layout of the decode kernel with B * T rows.
-template <bool FP8, int HD, int G>
+// PAGED: kc / vc (and ksc / vsc) are the page pools and pg the page table; a chunk is one page.
+template <bool FP8, bool PAGED, int HD, int G>
 __global__ void __launch_bounds__(AX_THREADS)
 attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict__ k_new, const __half* __restrict__ v_new,
                          void* __restrict__ kc, void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
                          const int64_t* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml,
-                         int nh, int nkv, int max_len, int nsplit, int T, float scale) {
+                         KvPages pg, int nh, int nkv, int max_len, int nsplit, int T, float scale) {
   using L = AxLayout<HD>;
   using CT = std::conditional_t<FP8, uint8_t, __half>;
   constexpr int QS = L::QS, PS = L::PS, SS = L::SS;
@@ -381,9 +401,21 @@ attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   const int R = G * T, MT = (R + 15) / 16;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
 
-  const int64_t row = (int64_t)b * nkv + kvh;
-  CT* kr = reinterpret_cast<CT*>(kc) + row * (int64_t)max_len * HD;
-  CT* vr = reinterpret_cast<CT*>(vc) + row * (int64_t)max_len * HD;
+  // head-vector index of chunk slot 0 (kv_page.cuh).  A page outside the pool is not dereferenced: every query row's
+  // partial of this chunk is NaN (the combine reads it only for the tokens that see the chunk), nothing is written.
+  const int64_t v0 = kv_vec<PAGED>(pg, b, kvh, nkv, max_len, start);
+  if (PAGED && v0 < 0) {
+    for (int r = tid; r < R; r += AX_THREADS) {
+      float* ml = part_ml + ((((int64_t)b * T + r / G) * nh + (int64_t)kvh * G + r % G) * nsplit + split) * 2;
+      ml[0] = NAN;
+      ml[1] = NAN;
+    }
+    return;
+  }
+  CT* kr = reinterpret_cast<CT*>(kc) + v0 * HD;
+  CT* vr = reinterpret_cast<CT*>(vc) + v0 * HD;
+  float* ksr = ksc + v0;
+  float* vsr = vsc + v0;
   auto new_vec = [&](const __half* x, int j) {  // the new key / value of chunk slot j
     return x + (((int64_t)b * T + (start + j - pos)) * nkv + kvh) * HD;
   };
@@ -400,17 +432,17 @@ attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict_
     uint4 kv = make_uint4(0, 0, 0, 0), vv = kv;
     if (j < nold) {
       if constexpr (FP8) {
-        kv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(kr + (int64_t)(start + j) * HD) + c));
-        vv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(vr + (int64_t)(start + j) * HD) + c));
+        kv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(kr + (int64_t)j * HD) + c));
+        vv = e4m3x8_to_h8(ldg_nc_v2(reinterpret_cast<const uint2*>(vr + (int64_t)j * HD) + c));
       } else {
-        kv = ldg_nc_v4(reinterpret_cast<const uint4*>(kr + (int64_t)(start + j) * HD) + c);
-        vv = ldg_nc_v4(reinterpret_cast<const uint4*>(vr + (int64_t)(start + j) * HD) + c);
+        kv = ldg_nc_v4(reinterpret_cast<const uint4*>(kr + (int64_t)j * HD) + c);
+        vv = ldg_nc_v4(reinterpret_cast<const uint4*>(vr + (int64_t)j * HD) + c);
       }
     } else if (j < n && !FP8) {               // append: this CTA owns slot start + j
       kv = reinterpret_cast<const uint4*>(new_vec(k_new, j))[c];
       vv = reinterpret_cast<const uint4*>(new_vec(v_new, j))[c];
-      reinterpret_cast<uint4*>(kr + (int64_t)(start + j) * HD)[c] = kv;
-      reinterpret_cast<uint4*>(vr + (int64_t)(start + j) * HD)[c] = vv;
+      reinterpret_cast<uint4*>(kr + (int64_t)j * HD)[c] = kv;
+      reinterpret_cast<uint4*>(vr + (int64_t)j * HD)[c] = vv;
     } else if (j < n) {
       continue;                               // e4m3 append below
     }
@@ -419,8 +451,8 @@ attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict_
   }
   if constexpr (FP8) {
     for (int j = tid; j < nold; j += AX_THREADS) {
-      sks[j] = ksc[row * max_len + start + j];
-      svs[j] = vsc[row * max_len + start + j];
+      sks[j] = ksr[j];
+      svs[j] = vsr[j];
     }
     // append: one warp per new vector (k of slot j, then v), quantized, stored, and staged as fp16
     constexpr int E = HD / 32;
@@ -428,14 +460,14 @@ attn_extend_split_kernel(const __half* __restrict__ q, const __half* __restrict_
       const int isv = v & 1, j = nold + v / 2;
       float s;
       const uint32_t w = e4m3_quantize_warp<HD>(new_vec(isv ? v_new : k_new, j), lane, s);
-      e4m3_store_warp<HD>((isv ? vr : kr) + (int64_t)(start + j) * HD, lane, w);
+      e4m3_store_warp<HD>((isv ? vr : kr) + (int64_t)j * HD, lane, w);
       __half* t = (isv ? sv : sk) + j * QS + lane * E;
 #pragma unroll
       for (int e = 0; e < E / 2; ++e)
         reinterpret_cast<__half2*>(t)[e] =
             __half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)((w >> (16 * e)) & 0xFFFFu), __NV_E4M3));
       if (lane == 0) {
-        (isv ? vsc : ksc)[row * max_len + start + j] = s;
+        (isv ? vsr : ksr)[j] = s;
         (isv ? svs : sks)[j] = s;
       }
     }
@@ -596,21 +628,22 @@ kv_quantize_fp8_kernel(const __half* __restrict__ src, uint8_t* __restrict__ cac
   if (lane == 0) scales[slot] = s;
 }
 
-template <bool FP8, int HD, int G>
+template <bool FP8, bool PAGED, int HD, int G>
 void launch_split(dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
-                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
-                  int nsplit, int chunk, float scale) {
-  attn_decode_split_kernel<FP8, HD, G><<<grid, AD_THREADS, 0, st>>>((const __half*)q, (const __half*)kn,
-                                                                    (const __half*)vn, kc, vc, ksc, vsc, pos, po, pml,
-                                                                    nh, nkv, max_len, nsplit, chunk, scale);
+                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, KvPages pg, int nh, int nkv,
+                  int max_len, int nsplit, int chunk, float scale) {
+  attn_decode_split_kernel<FP8, PAGED, HD, G><<<grid, AD_THREADS, 0, st>>>((const __half*)q, (const __half*)kn,
+                                                                           (const __half*)vn, kc, vc, ksc, vsc, pos, po,
+                                                                           pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
 }
 
-template <bool FP8, int HD>
+template <bool FP8, bool PAGED, int HD>
 void launch_split_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
-                    float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
-                    int nsplit, int chunk, float scale) {
+                    float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, KvPages pg, int nh, int nkv,
+                    int max_len, int nsplit, int chunk, float scale) {
 #define AD_LAUNCH(g) \
-  launch_split<FP8, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, nh, nkv, max_len, nsplit, chunk, scale)
+  launch_split<FP8, PAGED, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, pg, nh, nkv, max_len, nsplit, \
+                                  chunk, scale)
   switch (G) {
     case 1: AD_LAUNCH(1); break;
     case 2: AD_LAUNCH(2); break;
@@ -632,16 +665,20 @@ size_t ws_bytes(int64_t B, int64_t nh, int64_t hd, int64_t nsplit) {
   return ((o + 255) & ~(size_t)255) + (size_t)(B * nh * nsplit * 2) * sizeof(float);
 }
 
-// Argument checks and launches of quip_decode_attention (FP8 false) and quip_decode_attention_fp8 (FP8 true); fn names
+// Argument checks and launches of quip_decode_attention (FP8 false) and quip_decode_attention_fp8 (FP8 true), and of
+// their paged twins (PAGED true: k_cache / v_cache and the scales are page pools, max_len = max_pages * 64); fn names
 // the entry point in the messages.
-template <bool FP8>
+template <bool FP8, bool PAGED = false>
 int decode_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
                      float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t nh,
                      int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
-                     void* stream) {
+                     void* stream, KvPages pg = {}) {
   QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
+                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
+                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
   QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
@@ -660,33 +697,34 @@ int decode_attention(const char* fn, const void* q, const void* k_new, const voi
   const cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(nsplit, nkv, B);
   const int G = nh / nkv;
-  if (hd == 64) launch_split_g<FP8, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
-  else launch_split_g<FP8, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, chunk, scale);
+  if (hd == 64) launch_split_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
+  else launch_split_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
   QUIP_LAUNCHED("attn_decode_split_kernel");
   attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk, 1);
   QUIP_LAUNCHED("attn_decode_combine_kernel");
   return QUIP_OK;
 }
 
-template <bool FP8, int HD, int G>
+template <bool FP8, bool PAGED, int HD, int G>
 int launch_extend(dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc, void* vc,
-                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv, int max_len,
-                  int nsplit, int T, float scale) {
+                  float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, KvPages pg, int nh, int nkv,
+                  int max_len, int nsplit, int T, float scale) {
   constexpr size_t smem = AxLayout<HD>::BYTES;
-  auto kern = attn_extend_split_kernel<FP8, HD, G>;
+  auto kern = attn_extend_split_kernel<FP8, PAGED, HD, G>;
   if (smem > 48 * 1024) QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, AX_THREADS, smem, st>>>((const __half*)q, (const __half*)kn, (const __half*)vn, kc, vc, ksc, vsc, pos, po,
-                                       pml, nh, nkv, max_len, nsplit, T, scale);
+                                       pml, pg, nh, nkv, max_len, nsplit, T, scale);
   QUIP_LAUNCHED("attn_extend_split_kernel");
   return QUIP_OK;
 }
 
-template <bool FP8, int HD>
+template <bool FP8, bool PAGED, int HD>
 int launch_extend_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kn, const void* vn, void* kc,
-                    void* vc, float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, int nh, int nkv,
-                    int max_len, int nsplit, int T, float scale) {
+                    void* vc, float* ksc, float* vsc, const int64_t* pos, float* po, float* pml, KvPages pg, int nh,
+                    int nkv, int max_len, int nsplit, int T, float scale) {
 #define AX_LAUNCH(g) \
-  return launch_extend<FP8, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, nh, nkv, max_len, nsplit, T, scale)
+  return launch_extend<FP8, PAGED, HD, g>(grid, st, q, kn, vn, kc, vc, ksc, vsc, pos, po, pml, pg, nh, nkv, max_len, \
+                                          nsplit, T, scale)
   switch (G) {
     case 1: AX_LAUNCH(1);
     case 2: AX_LAUNCH(2);
@@ -700,15 +738,19 @@ int launch_extend_g(int G, dim3 grid, cudaStream_t st, const void* q, const void
 #undef AX_LAUNCH
 }
 
-// Argument checks and launches of quip_extend_attention (FP8 false) and quip_extend_attention_fp8 (FP8 true).
-template <bool FP8>
+// Argument checks and launches of quip_extend_attention (FP8 false) and quip_extend_attention_fp8 (FP8 true), and of
+// their paged twins.
+template <bool FP8, bool PAGED = false>
 int extend_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
                      float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t T,
                      int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
-                     size_t workspace_bytes, void* stream) {
+                     size_t workspace_bytes, void* stream, KvPages pg = {}) {
   QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
+                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
+                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
   QUIP_CHECK_ARG(T >= 1 && T <= AX_MAXT, "%s: %d tokens per row: need 1 <= T <= %d", fn, T, AX_MAXT);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
@@ -728,8 +770,8 @@ int extend_attention(const char* fn, const void* q, const void* k_new, const voi
   const dim3 grid(nsplit, nkv, B);
   const int G = nh / nkv;
   const int e = hd == 64
-      ? launch_extend_g<FP8, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, T, scale)
-      : launch_extend_g<FP8, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, nh, nkv, max_len, nsplit, T, scale);
+      ? launch_extend_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale)
+      : launch_extend_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale);
   if (e != QUIP_OK) return e;
   attn_decode_combine_kernel<<<(unsigned)((int64_t)B * T * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd,
                                                                              max_len, nsplit, AX_CHUNK, T);
@@ -793,6 +835,48 @@ extern "C" int quip_extend_attention_fp8(const void* q, const void* k_new, const
                                          void* stream) {
   return extend_attention<true>("quip_extend_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
                                 positions, out, B, T, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+}
+
+// Paged twins: max_len = max_pages * 64 everywhere (chunking, grid, workspace), so a paged launch runs the contiguous
+// launch's chunking on the same shape.
+extern "C" int quip_decode_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool,
+                                           void* v_pool, const int64_t* positions, void* out, int32_t B, int32_t nh,
+                                           int32_t nkv, int32_t hd, float scale, void* workspace, size_t workspace_bytes,
+                                           const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream) {
+  return decode_attention<false, true>("quip_decode_attention_paged", q, k_new, v_new, k_pool, v_pool, nullptr, nullptr,
+                                       positions, out, B, nh, nkv, hd, paged_len(max_pages), scale, workspace,
+                                       workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_decode_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool,
+                                               void* v_pool, float* k_scale, float* v_scale, const int64_t* positions,
+                                               void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd, float scale,
+                                               void* workspace, size_t workspace_bytes, const int32_t* page_table,
+                                               int32_t max_pages, int32_t n_pages, void* stream) {
+  return decode_attention<true, true>("quip_decode_attention_paged_fp8", q, k_new, v_new, k_pool, v_pool, k_scale,
+                                      v_scale, positions, out, B, nh, nkv, hd, paged_len(max_pages), scale, workspace,
+                                      workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_extend_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool,
+                                           void* v_pool, const int64_t* positions, void* out, int32_t B, int32_t T,
+                                           int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
+                                           size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
+                                           int32_t n_pages, void* stream) {
+  return extend_attention<false, true>("quip_extend_attention_paged", q, k_new, v_new, k_pool, v_pool, nullptr, nullptr,
+                                       positions, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, workspace,
+                                       workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_extend_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool,
+                                               void* v_pool, float* k_scale, float* v_scale, const int64_t* positions,
+                                               void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
+                                               float scale, void* workspace, size_t workspace_bytes,
+                                               const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                               void* stream) {
+  return extend_attention<true, true>("quip_extend_attention_paged_fp8", q, k_new, v_new, k_pool, v_pool, k_scale,
+                                      v_scale, positions, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, workspace,
+                                      workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
 }
 
 extern "C" int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,

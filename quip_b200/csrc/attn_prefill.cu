@@ -25,12 +25,14 @@
 // block rescales O' by alpha * c / max s_v once instead of keeping a second accumulator.
 //
 // Fixed orders everywhere: bit-identical from run to run; a row's result depends on its own q, cache and counts only.
+#include <limits.h>
 #include <math.h>
 
 #include <type_traits>
 
 #include "common.cuh"
 #include "kv_fp8.cuh"
+#include "kv_page.cuh"
 
 namespace quip {
 
@@ -89,13 +91,13 @@ __device__ __forceinline__ bool row_ok(int64_t pos, int64_t cnt, int T, int max_
 }
 
 // One warp per new head vector v = (b, i, h) of k_new / v_new (B, T, nkv, HD): slot positions[b] + i of both caches
-// when i < counts[b].
-template <bool FP8, int HD>
+// when i < counts[b] (PAGED: of the page pools, when the slot's page lies in the pool).
+template <bool FP8, bool PAGED, int HD>
 __global__ void __launch_bounds__(KA_WARPS * 32)
 kv_append_kernel(const __half* __restrict__ k_new, const __half* __restrict__ v_new, void* __restrict__ kc,
                  void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
-                 const int64_t* __restrict__ positions, const int64_t* __restrict__ counts, int64_t nvec, int T, int nkv,
-                 int max_len) {
+                 const int64_t* __restrict__ positions, const int64_t* __restrict__ counts, KvPages pg, int64_t nvec,
+                 int T, int nkv, int max_len) {
   const int64_t v = (int64_t)blockIdx.x * KA_WARPS + threadIdx.x / 32;
   if (v >= nvec) return;                      // warp-uniform
   const int lane = threadIdx.x & 31;
@@ -103,7 +105,8 @@ kv_append_kernel(const __half* __restrict__ k_new, const __half* __restrict__ v_
   const int i = (int)(v / nkv % T), h = (int)(v % nkv);
   const int64_t pos = positions[b], cnt = counts[b];
   if (!row_ok(pos, cnt, T, max_len) || i >= cnt) return;
-  const int64_t slot = (b * nkv + h) * max_len + pos + i;
+  const int64_t slot = kv_vec<PAGED>(pg, b, h, nkv, max_len, pos + i);
+  if (PAGED && slot < 0) return;              // a page outside the pool: not written
   if constexpr (FP8) {
 #pragma unroll
     for (int t = 0; t < 2; ++t) {
@@ -123,12 +126,15 @@ kv_append_kernel(const __half* __restrict__ k_new, const __half* __restrict__ v_
   }
 }
 
-template <bool FP8, int HD, int G>
+// PAGED: kc / vc (and ksc / vsc) are the page pools and pg the page table; a 64-slot block is one page, looked up by
+// the load that stages it.  A block whose page lies outside the pool is zero-filled, never read, and every row that
+// sees one of its slots gets a NaN output.
+template <bool FP8, bool PAGED, int HD, int G>
 __global__ void __launch_bounds__(PF_THREADS)
 attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, const void* __restrict__ vc,
                     const float* __restrict__ ksc, const float* __restrict__ vsc, const int64_t* __restrict__ positions,
-                    const int64_t* __restrict__ counts, __half* __restrict__ out, int T, int nh, int nkv, int max_len,
-                    float scale) {
+                    const int64_t* __restrict__ counts, __half* __restrict__ out, KvPages pg, int T, int nh, int nkv,
+                    int max_len, float scale) {
   using L = PfLayout<FP8, HD>;
   using CT = std::conditional_t<FP8, uint8_t, __half>;
   constexpr int KS = L::KS, BS = L::BS;
@@ -158,9 +164,9 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
   const int64_t diag0 = pos + i_lo;           // blocks reaching past this slot need the mask
   const int nblk = (int)(last / PF_BN) + 1;
 
-  const int64_t row = (int64_t)b * nkv + kvh;
-  const CT* kr = reinterpret_cast<const CT*>(kc) + row * max_len * HD;
-  const CT* vr = reinterpret_cast<const CT*>(vc) + row * max_len * HD;
+  const CT* kr = reinterpret_cast<const CT*>(kc);
+  const CT* vr = reinterpret_cast<const CT*>(vc);
+  int bad = INT_MAX;                          // PAGED: the first block whose page is not in the pool
 
   // the thread's two query rows (gid, gid + 8 of the warp's 16) and the last slot each sees
   int rr[2];
@@ -187,24 +193,27 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
   auto load_block = [&](int kb, int st) {
     unsigned char* base = pf_smem + st * L::STAGE;
     const int64_t start = (int64_t)kb * PF_BN;
+    const int64_t v0 = kv_vec<PAGED>(pg, b, kvh, nkv, max_len, start);   // head-vector index of the block's slot 0
+    const bool page = !PAGED || v0 >= 0;
+    if (!page) bad = min(bad, kb);
     if constexpr (FP8) {
       constexpr int S8 = HD / 16;             // 16-byte segments of an e4m3 head vector
       for (int x = tid; x < PF_BN * S8; x += PF_THREADS) {
         const int j = x / S8, c = x % S8;
-        const bool in = start + j <= last;
-        const int64_t off = (in ? start + j : 0) * HD + c * 16;
+        const bool in = page && start + j <= last;
+        const int64_t off = (in ? v0 + j : 0) * HD + c * 16;
         cp_async16(base + j * BS + c * 16, kr + off, in ? 16 : 0);
         cp_async16(base + L::TILE8 + j * BS + c * 16, vr + off, in ? 16 : 0);
       }
       float* sc = reinterpret_cast<float*>(base + 2 * L::TILE8);
       const int j = tid % PF_BN;
-      const bool in = start + j <= last;
-      cp_async4(sc + tid, (tid < PF_BN ? ksc : vsc) + row * max_len + (in ? start + j : 0), in ? 4 : 0);
+      const bool in = page && start + j <= last;
+      cp_async4(sc + tid, (tid < PF_BN ? ksc : vsc) + (in ? v0 + j : 0), in ? 4 : 0);
     } else {
       for (int x = tid; x < PF_BN * SEG; x += PF_THREADS) {
         const int j = x / SEG, c = x % SEG;
-        const bool in = start + j <= last;
-        const int64_t off = (in ? start + j : 0) * HD + c * 8;
+        const bool in = page && start + j <= last;
+        const int64_t off = (in ? v0 + j : 0) * HD + c * 8;
         cp_async16(base + (j * KS + c * 8) * 2, kr + off, in ? 16 : 0);
         cp_async16(base + L::TILE16 + (j * KS + c * 8) * 2, vr + off, in ? 16 : 0);
       }
@@ -369,6 +378,7 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
     const int r = rr[h];
     if (r < R) {
       const bool live = r / G < cnt;
+      const bool lost = PAGED && lim[h] >= (int64_t)bad * PF_BN;   // the row saw a block whose page is not in the pool
       __half* dst = out_row(r) + 2 * tig;
 #pragma unroll
       for (int n = 0; n < 2 * KT; ++n) {
@@ -377,7 +387,7 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
           x0 *= c[h];
           x1 *= c[h];
         }
-        *reinterpret_cast<uint32_t*>(dst + 8 * n) = live ? f2_to_h2(x0 / sum, x1 / sum) : 0u;
+        *reinterpret_cast<uint32_t*>(dst + 8 * n) = !live ? 0u : lost ? 0x7E007E00u : f2_to_h2(x0 / sum, x1 / sum);
       }
     }
   }
@@ -386,24 +396,25 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
 bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
-template <bool FP8, int HD, int G>
+template <bool FP8, bool PAGED, int HD, int G>
 int launch_prefill(dim3 grid, cudaStream_t st, const void* q, const void* kc, const void* vc, const float* ksc,
-                   const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, int T, int nh, int nkv,
-                   int max_len, float scale) {
+                   const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, KvPages pg, int T, int nh,
+                   int nkv, int max_len, float scale) {
   constexpr size_t smem = PfLayout<FP8, HD>::BYTES;
-  auto kern = attn_prefill_kernel<FP8, HD, G>;
+  auto kern = attn_prefill_kernel<FP8, PAGED, HD, G>;
   if (smem > 48 * 1024) QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, PF_THREADS, smem, st>>>((const __half*)q, kc, vc, ksc, vsc, pos, cnt, (__half*)out, T, nh, nkv, max_len,
-                                       scale);
+  kern<<<grid, PF_THREADS, smem, st>>>((const __half*)q, kc, vc, ksc, vsc, pos, cnt, (__half*)out, pg, T, nh, nkv,
+                                       max_len, scale);
   QUIP_LAUNCHED("attn_prefill_kernel");
   return QUIP_OK;
 }
 
-template <bool FP8, int HD>
+template <bool FP8, bool PAGED, int HD>
 int launch_prefill_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kc, const void* vc, const float* ksc,
-                     const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, int T, int nh, int nkv,
-                     int max_len, float scale) {
-#define PF_LAUNCH(g) return launch_prefill<FP8, HD, g>(grid, st, q, kc, vc, ksc, vsc, pos, cnt, out, T, nh, nkv, max_len, scale)
+                     const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, KvPages pg, int T, int nh,
+                     int nkv, int max_len, float scale) {
+#define PF_LAUNCH(g) \
+  return launch_prefill<FP8, PAGED, HD, g>(grid, st, q, kc, vc, ksc, vsc, pos, cnt, out, pg, T, nh, nkv, max_len, scale)
   switch (G) {
     case 1: PF_LAUNCH(1);
     case 2: PF_LAUNCH(2);
@@ -417,14 +428,19 @@ int launch_prefill_g(int G, dim3 grid, cudaStream_t st, const void* q, const voi
 #undef PF_LAUNCH
 }
 
-// Argument checks and launches of quip_prefill_attention (FP8 false) and quip_prefill_attention_fp8 (FP8 true).
-template <bool FP8>
+// Argument checks and launches of quip_prefill_attention (FP8 false) and quip_prefill_attention_fp8 (FP8 true), and of
+// their paged twins (PAGED true: the caches and scales are page pools, max_len = max_pages * 64).
+template <bool FP8, bool PAGED = false>
 int prefill_attention(const char* fn, const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
                       const float* v_scale, const int64_t* positions, const int64_t* counts, void* out, int32_t B,
-                      int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* stream) {
+                      int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* stream,
+                      KvPages pg = {}) {
   QUIP_CHECK_ARG(q && k_cache && v_cache && positions && counts && out && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
+                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
+                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
@@ -437,20 +453,24 @@ int prefill_attention(const char* fn, const void* q, const void* k_cache, const 
   const int G = nh / nkv;
   const dim3 grid(ceil_div((int64_t)G * T, PF_BM), nkv, B);
   const cudaStream_t st = (cudaStream_t)stream;
-  return hd == 64 ? launch_prefill_g<FP8, 64>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions, counts, out,
-                                              T, nh, nkv, max_len, scale)
-                  : launch_prefill_g<FP8, 128>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions, counts,
-                                               out, T, nh, nkv, max_len, scale);
+  return hd == 64 ? launch_prefill_g<FP8, PAGED, 64>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions,
+                                                     counts, out, pg, T, nh, nkv, max_len, scale)
+                  : launch_prefill_g<FP8, PAGED, 128>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions,
+                                                      counts, out, pg, T, nh, nkv, max_len, scale);
 }
 
-// Argument checks and launches of quip_kv_append (FP8 false) and quip_kv_append_fp8 (FP8 true).
-template <bool FP8>
+// Argument checks and launches of quip_kv_append (FP8 false) and quip_kv_append_fp8 (FP8 true), and of their paged
+// twins.
+template <bool FP8, bool PAGED = false>
 int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
               float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
-              int32_t hd, int32_t max_len, void* stream) {
+              int32_t hd, int32_t max_len, void* stream, KvPages pg = {}) {
   QUIP_CHECK_ARG(k_new && v_new && k_cache && v_cache && positions && counts && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
+  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
+                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
+                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
   QUIP_CHECK_ARG(B >= 0 && max_len > 0 && nkv > 0, "%s: bad sizes (B %d, nkv %d, max_len %d)", fn, B, nkv, max_len);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
   QUIP_CHECK_ARG(al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache), "%s: pointers must be 16-byte aligned",
@@ -463,11 +483,11 @@ int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cach
   const __half* kn = (const __half*)k_new;
   const __half* vn = (const __half*)v_new;
   if (hd == 64)
-    kv_append_kernel<FP8, 64><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale, positions,
-                                                                counts, nvec, T, nkv, max_len);
+    kv_append_kernel<FP8, PAGED, 64><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale,
+                                                                       positions, counts, pg, nvec, T, nkv, max_len);
   else
-    kv_append_kernel<FP8, 128><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale, positions,
-                                                                 counts, nvec, T, nkv, max_len);
+    kv_append_kernel<FP8, PAGED, 128><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale,
+                                                                        positions, counts, pg, nvec, T, nkv, max_len);
   QUIP_LAUNCHED("kv_append_kernel");
   return QUIP_OK;
 }
@@ -505,4 +525,43 @@ extern "C" int quip_prefill_attention_fp8(const void* q, const void* k_cache, co
                                           int32_t max_len, float scale, void* stream) {
   return prefill_attention<true>("quip_prefill_attention_fp8", q, k_cache, v_cache, k_scale, v_scale, positions,
                                  counts, out, B, T, nh, nkv, hd, max_len, scale, stream);
+}
+
+// Paged twins: max_len = max_pages * 64.
+extern "C" int quip_kv_append_paged(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                    const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
+                                    int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                    void* stream) {
+  return kv_append<false, true>("quip_kv_append_paged", k_new, v_new, k_pool, v_pool, nullptr, nullptr, positions,
+                                counts, B, T, nkv, hd, paged_len(max_pages), stream,
+                                KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_kv_append_paged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                        float* k_scale, float* v_scale, const int64_t* positions, const int64_t* counts,
+                                        int32_t B, int32_t T, int32_t nkv, int32_t hd, const int32_t* page_table,
+                                        int32_t max_pages, int32_t n_pages, void* stream) {
+  return kv_append<true, true>("quip_kv_append_paged_fp8", k_new, v_new, k_pool, v_pool, k_scale, v_scale, positions,
+                               counts, B, T, nkv, hd, paged_len(max_pages), stream,
+                               KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_prefill_attention_paged(const void* q, const void* k_pool, const void* v_pool,
+                                            const int64_t* positions, const int64_t* counts, void* out, int32_t B,
+                                            int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale,
+                                            const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                            void* stream) {
+  return prefill_attention<false, true>("quip_prefill_attention_paged", q, k_pool, v_pool, nullptr, nullptr, positions,
+                                        counts, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, stream,
+                                        KvPages{page_table, max_pages, n_pages});
+}
+
+extern "C" int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const void* v_pool,
+                                                const float* k_scale, const float* v_scale, const int64_t* positions,
+                                                const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh,
+                                                int32_t nkv, int32_t hd, float scale, const int32_t* page_table,
+                                                int32_t max_pages, int32_t n_pages, void* stream) {
+  return prefill_attention<true, true>("quip_prefill_attention_paged_fp8", q, k_pool, v_pool, k_scale, v_scale,
+                                       positions, counts, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, stream,
+                                       KvPages{page_table, max_pages, n_pages});
 }

@@ -30,6 +30,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+KV_PAGE = 64                                           # slots per page of a paged KV cache (include/quip_b200.h)
+
 
 def _rotate_half(x):
     h = x.shape[-1] // 2
@@ -163,7 +165,14 @@ class GraphDecoder:
         pos[b] + i, otherwise."""
         if T > 1:
             pos = (pos[:, None] + self._tar(T)).reshape(-1)
+            if self._pad_past_end():
+                pos = pos.clamp(max=self.cos.shape[0] - 1)
         return self.cos.index_select(0, pos), self.sin.index_select(0, pos)
+
+    def _pad_past_end(self):
+        """Whether the padding tokens of a step may sit past the last position (a prefill chunk of a row that starts
+        inside it): their rotary rows and learned positions are then clamped to the table.  Padding writes nothing."""
+        return False
 
     def _advance(self):
         self.position.add_(1)
@@ -266,8 +275,10 @@ class GraphDecoder:
             h = d.project_in(h)
         pos = self._step_positions()
         if multi:
-            return h + F.embedding(pos[:, None] + self._tar(tokens.shape[1]) + d.embed_positions.offset,
-                                   d.embed_positions.weight)
+            pos = pos[:, None] + self._tar(tokens.shape[1])
+            if self._pad_past_end():
+                pos = pos.clamp(max=self.max_len - 1)
+            return h + F.embedding(pos + d.embed_positions.offset, d.embed_positions.weight)
         return h + F.embedding(pos + d.embed_positions.offset, d.embed_positions.weight)[:, None]
 
     def _head(self, h, pend):
@@ -408,12 +419,37 @@ class PromptDecoder(GraphDecoder):
         per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
         (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
         quantized values of every slot, its own included.  On the CPU the same step in torch: quantize, per-row scatter,
-        dequantize the cache to the compute dtype, SDPA under the mask.
+        dequantize the cache to the compute dtype, SDPA under the mask;
+      * n_pages=N: a paged cache (include/quip_b200.h).  k_cache / v_cache are pools (L, N, nkv, 64, hd) (scales
+        (L, N, nkv, 64)) and `page_table` (B, ceil(max_len / 64)) int32 on the device, shared by all layers, maps slot j
+        of row b to slot j % 64 of page page_table[b, j // 64].  The table starts unmapped (-1: nothing is read or
+        written there, NaN outputs) and prefill maps it to the page_table given here (default: row b's own pages
+        b * max_pages ..), so rows may share pages (plan_prefix_pages).  Every attention launch takes the table; on the
+        CPU reads gather pool[page_table] into the contiguous view and writes go through the same translation, so a
+        paged decoder computes what a contiguous one does.  A paged cache is filled by chunked prefill only.
     The whole model, no layer pipeline."""
 
-    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False):
+    def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False,
+                 page_table=None, n_pages=None):
+        if n_pages is None and page_table is not None:
+            raise ValueError('a page_table needs n_pages, the size of the page pool')
+        self.n_pages = None if n_pages is None else int(n_pages)
+        if self.n_pages is not None and self.n_pages < 1:
+            raise ValueError(f'n_pages must be at least 1, got {n_pages}')
+        self.max_pages = -(-int(max_len) // KV_PAGE)
         super().__init__(model, max_len=max_len, batch=batch, ops=ops, kv_dtype=kv_dtype)
         B = self.batch
+        if self.paged:
+            if page_table is None:
+                page_table = torch.arange(B * self.max_pages, dtype=torch.int32).view(B, self.max_pages)
+            page_table = torch.as_tensor(page_table).to(torch.int32).cpu()
+            if tuple(page_table.shape) != (B, self.max_pages):
+                raise ValueError(f'page_table must be (batch {B}, ceil(max_len / {KV_PAGE}) = {self.max_pages}), got '
+                                 f'{tuple(page_table.shape)}')
+            if bool(((page_table < -1) | (page_table >= self.n_pages)).any()):
+                raise ValueError(f'page ids must lie in [0, n_pages = {self.n_pages}) or be -1 (unmapped)')
+            self._page_map = page_table
+            self.page_table = torch.full((B, self.max_pages), -1, dtype=torch.int32, device=self.dev)
         self.positions = torch.zeros(B, dtype=torch.long, device=self.dev)
         self.max_new = int(max_new)
         self.generated = torch.zeros(B, max(self.max_new, 1), dtype=torch.long, device=self.dev)
@@ -470,7 +506,9 @@ class PromptDecoder(GraphDecoder):
 
     def _alloc_cache(self, shape, dt, kv_dtype):
         """fp8: e4m3 caches and their fp32 scales, allocated as such (never an fp16 cache first: at the sizes fp8 is for,
-        that one would not fit)."""
+        that one would not fit).  Paged: the pools (L, n_pages, nkv, 64, hd) instead of (L, B, nkv, max_len, hd)."""
+        if self.paged:
+            shape = (shape[0], self.n_pages, shape[2], KV_PAGE, shape[4])
         self.k_scale = self.v_scale = None
         if kv_dtype != torch.float8_e4m3fn:
             return super()._alloc_cache(shape, dt, kv_dtype)
@@ -483,6 +521,49 @@ class PromptDecoder(GraphDecoder):
     @property
     def _fp8(self):
         return self.kv_dtype == torch.float8_e4m3fn
+
+    @property
+    def paged(self):
+        return self.n_pages is not None
+
+    def _kv_kw(self, li):
+        """The cache arguments of layer li's attention launches beyond the caches: e4m3 scales, the page table."""
+        kw = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
+        if self.paged:
+            kw['page_table'] = self.page_table
+        return kw
+
+    def _store(self, li, rows, slots, k, v):
+        """CPU: k / v (..., nkv, hd) to slots of rows (index tensors of shape ...) of layer li's cache, e4m3-quantized
+        with their scales on an e4m3 cache; paged, through the page table (nothing on an unmapped page)."""
+        nkv, hd = k.shape[-2:]
+        rows, slots, k, v = rows.reshape(-1), slots.reshape(-1), k.reshape(-1, nkv, hd), v.reshape(-1, nkv, hd)
+        if self.paged:
+            page = self.page_table[rows, slots // KV_PAGE].long()
+            ok = (page >= 0) & (page < self.n_pages)
+            rows, slots, k, v = page[ok], (slots % KV_PAGE)[ok], k[ok], v[ok]
+        for x, cache, scales in ((k, self.k_cache[li], self.k_scale), (v, self.v_cache[li], self.v_scale)):
+            if self._fp8:
+                xq, xs = _e4m3_quantize(x)
+                cache[rows, :, slots] = xq
+                scales[li][rows, :, slots] = xs
+            else:
+                cache[rows, :, slots] = x
+
+    def _cached(self, li, dtype):
+        """CPU: layer li's keys and values as (B, nkv, max_len, hd) in dtype (e4m3: dequantized); paged, gathered through
+        the page table (an unmapped page reads page 0: such slots lie past every row's position, under the mask)."""
+        out = []
+        for cache, scales in ((self.k_cache[li], self.k_scale), (self.v_cache[li], self.v_scale)):
+            s = None if scales is None else scales[li]
+            if self.paged:
+                tbl = self.page_table.long().clamp(min=0)                             # (B, max_pages)
+                B, nkv, hd = tbl.shape[0], cache.shape[1], cache.shape[3]
+                cache = cache[tbl].transpose(1, 2).reshape(B, nkv, -1, hd)[:, :, :self.max_len]
+                if s is not None:
+                    s = s[tbl].transpose(1, 2).reshape(B, nkv, -1)[:, :, :self.max_len]
+            out.append(cache if s is None else _e4m3_dequantize(cache, s, dtype))
+        return out
 
     def _step_positions(self):
         return self.positions
@@ -502,22 +583,12 @@ class PromptDecoder(GraphDecoder):
             return self._attend_multi(li, q, k, v, mask, scale)
         if self._kernel:
             from . import fused
-            sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
             o = fused.decode_attention(q.reshape(B, nh, hd).contiguous(), k.reshape(B, nkv, hd).contiguous(),
                                        v.reshape(B, nkv, hd).contiguous(), self.k_cache[li], self.v_cache[li],
-                                       self.positions, scale, **sc)
+                                       self.positions, scale, **self._kv_kw(li))
             return o.view(B, 1, nh * hd)
-        if self._fp8:
-            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
-                xq, xs = _e4m3_quantize(x[:, :, 0])
-                cache[self._rows, :, self.positions] = xq
-                scales[self._rows, :, self.positions] = xs
-            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
-            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
-        else:
-            self.k_cache[li][self._rows, :, self.positions] = k[:, :, 0]
-            self.v_cache[li][self._rows, :, self.positions] = v[:, :, 0]
-            kk, vv = self.k_cache[li], self.v_cache[li]
+        self._store(li, self._rows, self.positions, k[:, :, 0], v[:, :, 0])
+        kk, vv = self._cached(li, q.dtype)
         if nkv != nh:
             kk = kk.repeat_interleave(nh // nkv, dim=1)
             vv = vv.repeat_interleave(nh // nkv, dim=1)
@@ -531,24 +602,14 @@ class PromptDecoder(GraphDecoder):
         B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
         if self._kernel:
             from . import fused
-            sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
             o = fused.extend_attention(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous(),
                                        v.transpose(1, 2).contiguous(), self.k_cache[li], self.v_cache[li],
-                                       self.positions, scale, **sc)
+                                       self.positions, scale, **self._kv_kw(li))
             return o.view(B, T, nh * hd)
         rows = self._rows[:, None].expand(B, T)
         slots = self.positions[:, None] + self._tarange                                 # (B, T)
-        if self._fp8:
-            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
-                xq, xs = _e4m3_quantize(x.transpose(1, 2))                              # (B, T, nkv, hd), (B, T, nkv)
-                cache[rows, :, slots] = xq
-                scales[rows, :, slots] = xs
-            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
-            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
-        else:
-            self.k_cache[li][rows, :, slots] = k.transpose(1, 2)
-            self.v_cache[li][rows, :, slots] = v.transpose(1, 2)
-            kk, vv = self.k_cache[li], self.v_cache[li]
+        self._store(li, rows, slots, k.transpose(1, 2), v.transpose(1, 2))
+        kk, vv = self._cached(li, q.dtype)
         if nkv != nh:
             kk = kk.repeat_interleave(nh // nkv, dim=1)
             vv = vv.repeat_interleave(nh // nkv, dim=1)
@@ -562,29 +623,20 @@ class PromptDecoder(GraphDecoder):
         quip_prefill_attention(_fp8).  CPU: per-row scatter of the counted slots, SDPA under the causal mask over the
         slots below positions[b] + counts[b].  Returns (B, T, nh * hd)."""
         (B, nh, T, hd), nkv, counts = q.shape, self.nkv, self._chunk
-        sc = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
         if self._kernel:
             from . import fused
+            kw = self._kv_kw(li)
             fused.kv_append(k.transpose(1, 2).contiguous(), v.transpose(1, 2).contiguous(), self.k_cache[li],
-                            self.v_cache[li], self.positions, counts, **sc)
+                            self.v_cache[li], self.positions, counts, **kw)
             o = fused.prefill_attention(q.transpose(1, 2).contiguous(), self.k_cache[li], self.v_cache[li],
-                                        self.positions, counts, scale, **sc)
+                                        self.positions, counts, scale, **kw)
             return o.view(B, T, nh * hd)
         tar = self._tar(T)
         live = tar[None] < counts[:, None]                                             # (B, T)
         rows = self._rows[:, None].expand(B, T)[live]
         slots = (self.positions[:, None] + tar)[live]
-        if self._fp8:
-            for x, cache, scales in ((k, self.k_cache[li], self.k_scale[li]), (v, self.v_cache[li], self.v_scale[li])):
-                xq, xs = _e4m3_quantize(x.transpose(1, 2)[live])                       # (n, nkv, hd), (n, nkv)
-                cache[rows, :, slots] = xq
-                scales[rows, :, slots] = xs
-            kk = _e4m3_dequantize(self.k_cache[li], self.k_scale[li], q.dtype)
-            vv = _e4m3_dequantize(self.v_cache[li], self.v_scale[li], q.dtype)
-        else:
-            self.k_cache[li][rows, :, slots] = k.transpose(1, 2)[live]
-            self.v_cache[li][rows, :, slots] = v.transpose(1, 2)[live]
-            kk, vv = self.k_cache[li], self.v_cache[li]
+        self._store(li, rows, slots, k.transpose(1, 2)[live], v.transpose(1, 2)[live])
+        kk, vv = self._cached(li, q.dtype)
         seen = (self._arange[None] < (self.positions + counts)[:, None])[:, None, :, None]   # whatever lies past: not read
         kk, vv = torch.where(seen, kk, 0), torch.where(seen, vv, 0)
         if nkv != nh:
@@ -605,7 +657,10 @@ class PromptDecoder(GraphDecoder):
 
     def _capture_state(self):
         # Not the cache: a warm-up step writes slot positions[b] (clamped to max_len - 1), and a later step writes that
-        # slot before it reads it.  A row clamped from max_len takes no further step: its cache is full.
+        # slot before it reads it.  A row clamped from max_len takes no further step: its cache is full.  A paged
+        # decoder is captured before prefill maps its table (generate does so): the warm-up steps then run against an
+        # unmapped table and write nothing -- with a page shared by several rows, a warm-up write to slot 0 would
+        # corrupt another row's prefix.
         return [self.positions, self.tokens, self._t, self.generated]
 
     def _counters_in_range(self):
@@ -623,8 +678,13 @@ class PromptDecoder(GraphDecoder):
         self.generated.zero_()
         self._pos_host = [0] * self.batch
         self._t_host = 0
+        if self.paged:
+            self.page_table.fill_(-1)
 
-    def prefill(self, prompts, chunk=None):
+    def _pad_past_end(self):
+        return self.paged and self._chunk is not None
+
+    def prefill(self, prompts, chunk=None, starts=None):
         """Fill the cache from `prompts` (B 1-D id tensors).  Returns the logits after each prompt's last token
         (B, vocab); with max_new > 0 the token selected from them (argmax, or sampled at t = 0) is the first generated
         token and the next step's input.
@@ -638,17 +698,35 @@ class PromptDecoder(GraphDecoder):
         cache (_prefill_chunks): peak memory follows C, not P, and no fp16 copy of the cache is made.  Only slots
         0 .. len_b - 1 of row b are written.  With an e4m3 cache every token attends over the quantized keys and values
         the cache holds, its own included -- what teacher-forced decode steps compute, not the fp16 attention of
-        chunk=None."""
+        chunk=None.
+
+        A paged decoder maps its page table first, and takes chunk=C only (the many-token forward cannot start mid-
+        prompt).  starts (one multiple of 64 per row, below its length; default 0): row b prefills from slot starts[b]
+        on, its slots below read from pages other rows write (plan_prefix_pages: starts[b] = 64 * S_b over a leading run
+        of S_b shared pages).  Chunks stay aligned to c0 = 0, C, 2C, ...; in a chunk row b feeds its tokens
+        [max(c0, starts[b]), min(c0 + C, len_b)), the first at positions[b].  This is correct because (1) the owner of a
+        page row b shares starts at or below that page, so it writes slot j of the page in the chunk holding j, the
+        chunk of b's first token (starts[b] > j) or an earlier one; and (2) within a chunk, each layer's kv_append of
+        every row runs before that layer's prefill_attention, so b reads the slot after it is written."""
         B = self.batch
         if len(prompts) != B:
             raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
         chunk = _chunk_size(chunk)
+        if self.paged and chunk is None:
+            raise ValueError('a paged KV cache is filled by chunked prefill: pass chunk=C')
         lens = [int(p.numel()) for p in prompts]
         if min(lens) < 1:
             raise ValueError('empty prompt')
         P = max(lens)
         if P > self.max_len:
             raise ValueError(f'a prompt of {P} tokens does not fit a cache of {self.max_len} positions')
+        starts = [0] * B if starts is None else [int(x) for x in starts]
+        if len(starts) != B or any(x % KV_PAGE or not 0 <= x < n for x, n in zip(starts, lens)):
+            raise ValueError(f'starts must hold one multiple of {KV_PAGE} per row, below its prompt length; got {starts}')
+        if any(starts) and not self.paged:
+            raise ValueError('per-row prefill starts need a paged decoder (n_pages=...)')
+        if self.paged:
+            self.page_table.copy_(self._page_map)
         ids = torch.zeros(B, P, dtype=torch.long, device=self.dev)
         for b, p in enumerate(prompts):
             ids[b, :lens[b]] = p.reshape(-1).to(self.dev)
@@ -666,29 +744,40 @@ class PromptDecoder(GraphDecoder):
                         self.v_cache[li, :, :, :P].copy_(cache.layers[li].values)
                 logits = self.model.lm_head(out.last_hidden_state[self._rows, lens_t - 1])     # last real token per row
             else:
-                logits = self._prefill_chunks(ids, lens, chunk)
+                logits = self._prefill_chunks(ids, lens, chunk, starts)
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
             if self.max_new:
                 self._first_token(logits)
         return logits
 
-    def _prefill_chunks(self, ids, lens, C):
-        """Chunked prefill of ids (B, P): chunk c0 feeds ids[:, c0:c0 + T], T = min(C, P - c0), with every row at
-        position c0 and counts[b] = clamp(len_b - c0, 0, T) tokens of its own, through the embedding and layer loops
-        of a step (packed linears at M = B * T; attention by _attend_chunk).  Rows whose prompt has ended ride along as
-        padding and write nothing.  The final norm and lm_head run once, on each row's last prompt token, gathered from
-        the chunk it falls in.  Leaves positions at c0 of the last chunk (prefill sets them)."""
+    def _prefill_chunks(self, ids, lens, C, starts):
+        """Chunked prefill of ids (B, P): chunk c0 feeds T = min(C, P - c0) tokens per row, row b from position
+        lo_b = max(c0, starts[b]) with counts[b] = clamp(min(len_b, c0 + T) - lo_b, 0, T) tokens of its own (with every
+        start 0: ids[:, c0:c0 + T] at position c0), through the embedding and layer loops of a step (packed linears at
+        M = B * T; attention by _attend_chunk).  Rows with nothing to feed ride along as padding and write nothing.
+        The final norm and lm_head run once, on each row's last prompt token, gathered from the chunk it falls in.
+        Leaves positions at lo of the last chunk (prefill sets them)."""
         B, P = ids.shape
         counts = torch.empty(B, dtype=torch.long, device=self.dev)
         h_last = p_last = None
         for c0 in range(0, P, C):
             T = min(C, P - c0)
-            self.positions.fill_(c0)
-            counts.copy_(torch.tensor([min(max(n - c0, 0), T) for n in lens], dtype=torch.long))
+            lo = [max(c0, s) for s in starts]
+            cnt = [min(max(min(n, c0 + T) - l, 0), T) for n, l in zip(lens, lo)]
+            if not any(cnt):
+                continue
+            counts.copy_(torch.tensor(cnt, dtype=torch.long))
+            if any(starts):
+                lo_t = torch.tensor(lo, dtype=torch.long, device=self.dev)
+                self.positions.copy_(lo_t)
+                chunk_ids = ids.gather(1, (lo_t[:, None] + torch.arange(T, device=self.dev)).clamp(max=P - 1))
+            else:
+                self.positions.fill_(c0)
+                chunk_ids = ids[:, c0:c0 + T]
             self._chunk = counts
             try:
-                h, pend = self._layers(self._embed(ids[:, c0:c0 + T]))
+                h, pend = self._layers(self._embed(chunk_ids))
             finally:
                 self._chunk = None
             ends = [b for b in range(B) if c0 < lens[b] <= c0 + T]                     # rows whose last token is here
@@ -698,7 +787,7 @@ class PromptDecoder(GraphDecoder):
                 h_last = h.new_empty(B, 1, h.shape[-1])
                 p_last = None if pend is None else pend.new_empty(B, 1, pend.shape[-1])
             r = torch.tensor(ends, dtype=torch.long, device=self.dev)
-            i = torch.tensor([lens[b] - 1 - c0 for b in ends], dtype=torch.long, device=self.dev)
+            i = torch.tensor([lens[b] - 1 - lo[b] for b in ends], dtype=torch.long, device=self.dev)
             h_last[r, 0] = h[r, i]
             if pend is not None:
                 p_last[r, 0] = pend[r, i]
@@ -763,7 +852,7 @@ class SpecDecoder(PromptDecoder):
     prompt + max_new + draft_tokens (a finished row's step still writes its T slots)."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=1, draft_tokens=4, max_ngram=3, ops=None, kv_dtype=None,
-                 sampling=False):
+                 sampling=False, page_table=None, n_pages=None):
         k, n_max = int(draft_tokens), int(max_ngram)
         if not 1 <= k <= 7:
             raise ValueError(f'draft_tokens must lie in [1, 7], got {draft_tokens}')
@@ -774,7 +863,7 @@ class SpecDecoder(PromptDecoder):
         if int(max_len) < k + 2:
             raise ValueError(f'max_len {max_len} leaves no room for a step of {k + 1} tokens')
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
-                         sampling=sampling)
+                         sampling=sampling, page_table=page_table, n_pages=n_pages)
         B, dev = self.batch, self.dev
         self.k, self.n_min, self.n_max = k, 1, n_max
         self.T = k + 1
@@ -829,14 +918,14 @@ class SpecDecoder(PromptDecoder):
             t.zero_()
         self._steps_host = 0
 
-    def prefill(self, prompts, chunk=None):
-        """PromptDecoder.prefill (chunk as there), plus the history: each prompt and its first generated token in hist,
-        n_gen = 1."""
+    def prefill(self, prompts, chunk=None, starts=None):
+        """PromptDecoder.prefill (chunk and starts as there), plus the history: each whole prompt and its first
+        generated token in hist, n_gen = 1."""
         lens = [int(torch.as_tensor(p).numel()) for p in prompts]
         if lens and max(lens) + self.max_new + self.k > self.max_len:
             raise ValueError(f'a prompt of {max(lens)} tokens, {self.max_new} new ones and {self.k} drafts exceed the '
                              f'cache of {self.max_len} positions')
-        logits = super().prefill(prompts, chunk=chunk)
+        logits = super().prefill(prompts, chunk=chunk, starts=starts)
         with torch.no_grad():
             for b, p in enumerate(prompts):
                 self.hist[b, :lens[b]] = torch.as_tensor(p).reshape(-1).to(self.dev)
@@ -980,6 +1069,48 @@ def _sample_torch(logits, temperature, top_k, top_p, seed, t):
 EOS_CHECK_EVERY = 16
 
 
+def plan_prefix_pages(prompts, budgets, max_pages=None):
+    """Page table of a paged KV cache whose rows share their common prompt prefixes.
+
+    prompts: 1-D id sequences; budgets: the slots row r may fill (its prompt, new tokens and drafts), >= its length.
+    Page p of row r (slots 64p .. 64p + 63) is shareable when 64 (p + 1) <= len_r - 1: it is full, and the row's last
+    prompt token -- whose logits start generation -- is never on it, nor is any slot decode writes.  Row r maps a
+    shareable page p to the page of the first earlier row with the same tokens 0 .. 64 (p + 1) - 1 that also finds page
+    p shareable; those pages form a leading run of S_r pages.  Its other pages, up to ceil(budget_r / 64), are its own.
+
+    Returns (page_table (B, max_pages) int32 with -1 past each row's pages; max_pages defaults to the largest row's
+    count), n_pages (the distinct pages), starts (64 * S_r: where row r's prefill begins)."""
+    B = len(prompts)
+    if len(budgets) != B:
+        raise ValueError(f'{len(budgets)} budgets for {B} prompts')
+    toks = [torch.as_tensor(p).reshape(-1).tolist() for p in prompts]
+    if any(int(b) < len(t) or not t for b, t in zip(budgets, toks)):
+        raise ValueError('every prompt must be non-empty and fit its budget')
+    need = [-(-int(b) // KV_PAGE) for b in budgets]
+    max_pages = max(need) if max_pages is None else int(max_pages)
+    if max_pages < max(need):
+        raise ValueError(f'max_pages {max_pages} is below the {max(need)} pages a row needs')
+    table = torch.full((B, max_pages), -1, dtype=torch.int32)
+    owner = {}                                    # (prefix node, page tokens) -> (node of the longer prefix, page id)
+    n_pages, starts = 0, []
+    for r, t in enumerate(toks):
+        node, shared = 0, 0
+        for p in range(need[r]):
+            if KV_PAGE * (p + 1) <= len(t) - 1:      # shareable; once a page is the row's own, no later one is shared
+                key = (node, tuple(t[KV_PAGE * p:KV_PAGE * (p + 1)]))
+                if key in owner:
+                    node, page = owner[key]
+                    table[r, p] = page
+                    shared += 1
+                    continue
+                owner[key] = (len(owner) + 1, n_pages)
+                node = len(owner)
+            table[r, p] = n_pages
+            n_pages += 1
+        starts.append(KV_PAGE * shared)
+    return table, n_pages, starts
+
+
 def _chunk_size(chunk):
     """A prefill chunk size: None (one many-token forward of the whole prompts) or an int >= 1."""
     if chunk is None:
@@ -1023,7 +1154,7 @@ def _sampling_settings(n, temperature, top_k, top_p, seed):
 
 def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
-             spec_stats=None, prefill_chunk_size=None):
+             spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -1047,9 +1178,29 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     prefill_chunk_size=C (an int >= 1; default None: one many-token forward of the padded prompts) prefills in chunks
     of C tokens straight into the KV cache (PromptDecoder.prefill(chunk=C)): the prefill's peak memory is bounded by C
     instead of the prompt length, with no fp16 copy of the cache.  With an e4m3 cache the prompt then attends over its
-    own quantized keys and values, as the decode steps do."""
+    own quantized keys and values, as the decode steps do.
+
+    share_prompt_prefixes=True keeps the KV cache in 64-slot pages (PromptDecoder(n_pages=...)) and lets prompts share
+    the full pages of their common prefixes (plan_prefix_pages): a shared page is prefilled and stored once.  The pool
+    holds the plan's pages, not batch * max_len slots; prefill_chunk_size defaults to 512.  The tokens are the ones of
+    the unshared call up to the arithmetic of other GEMM token counts (fewer prefilled tokens per chunk).
+
+    num_return_sequences=n > 1 (with do_sample=True: n greedy copies would be one answer) returns n samples of each
+    prompt, len(prompts) * n tensors in (prompt, sample) order: by definition, what
+    generate([p for p in prompts for _ in range(n)], share_prompt_prefixes=True, ...) returns -- an int seed s gives
+    output row r the seed s + r, and a list setting takes one value per output row.  A prompt is prefilled once, but
+    for its last partial page and last token."""
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
-    prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
+    n_ret = num_return_sequences
+    if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
+        raise ValueError(f'num_return_sequences must be an integer >= 1, got {num_return_sequences!r}')
+    n_ret = int(n_ret)
+    if n_ret > 1 and not do_sample:
+        raise ValueError(f'num_return_sequences={n_ret} needs do_sample=True (greedy samples would all be the same)')
+    share = bool(share_prompt_prefixes) or n_ret > 1
+    if share and prefill_chunk_size is None:
+        prefill_chunk_size = 512
+    prompts = [torch.as_tensor(p).reshape(-1) for p in prompts for _ in range(n_ret)]
     max_new_tokens = int(max_new_tokens)
     if not prompts:
         raise ValueError('no prompts')
@@ -1081,17 +1232,22 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                 raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
     else:
         settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
+    pages, starts = {}, None
+    if share:
+        table, n_pages, starts = plan_prefix_pages(prompts, [n + max_new_tokens + k for n in lens],
+                                                   max_pages=-(-max_len // KV_PAGE))
+        pages = dict(page_table=table, n_pages=n_pages)
     if spec:
         dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
-                          max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample))
+                          max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
     else:
         dec = PromptDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, kv_dtype=kv_dtype,
-                            sampling=bool(do_sample))
+                            sampling=bool(do_sample), **pages)
     if do_sample:
         dec.set_sampling(*settings)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
-        dec.capture()
-    dec.prefill(prompts, chunk=prefill_chunk_size)
+        dec.capture()                                                # before prefill maps a paged table
+    dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
     if spec:
         return _generate_spec(dec, max_new_tokens, eos_t, spec_stats)

@@ -88,15 +88,48 @@ class CudaGlue:
         return out
 
 
-def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None):
+KV_PAGE = 64
+
+
+def _kv_layout(fn, k_cache, B, page_table):
+    """(rows, slots, max_len) of one layer's cache k_cache (rows, nkv, slots, hd): the contiguous cache (B, nkv, max_len,
+    hd) without a page table; with page_table (B, max_pages) int32, pools (n_pages, nkv, 64, hd) and max_len =
+    max_pages * 64 (include/quip_b200.h has the rule).  Checks the table's dtype, shape, device and alignment and the
+    pools' alignment; the callers check the rest of the shapes against these."""
+    if page_table is None:
+        return B, k_cache.shape[2], k_cache.shape[2]
+    if page_table.dtype != torch.int32 or page_table.dim() != 2 or page_table.shape[0] != B or page_table.shape[1] < 1:
+        raise ValueError(f'{fn}: page_table must be (B={B}, max_pages >= 1) int32, got {tuple(page_table.shape)} '
+                         f'{page_table.dtype}')
+    if k_cache.dim() != 4 or k_cache.shape[2] != KV_PAGE or k_cache.shape[0] < 1:
+        raise ValueError(f'{fn}: with a page table the caches are pools (n_pages, nkv, {KV_PAGE}, hd), got '
+                         f'{tuple(k_cache.shape)}')
+    if page_table.shape[1] > (2 ** 31 - 1) // KV_PAGE:
+        raise ValueError(f'{fn}: {page_table.shape[1]} pages per row: max_pages * {KV_PAGE} must fit int32')
+    if not page_table.is_cuda or page_table.device != k_cache.device or not page_table.is_contiguous():
+        raise ValueError(f'{fn}: page_table must be a contiguous CUDA tensor on the caches\' device')
+    if page_table.data_ptr() % 4 or k_cache.data_ptr() % 16:
+        raise ValueError(f'{fn}: page_table must be 4-byte aligned and the pools 16-byte aligned')
+    return k_cache.shape[0], KV_PAGE, page_table.shape[1] * KV_PAGE
+
+
+def _paged_args(page_table, n_pages):
+    return (page_table.data_ptr(), page_table.shape[1], n_pages)
+
+
+def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
     """quip_decode_attention on torch tensors: append k_new / v_new (B, nkv, hd) at slot positions[b] of one layer's
     k_cache / v_cache (B, nkv, max_len, hd) and attend q (B, nh, hd) over slots 0 .. positions[b].  fp16, CUDA,
     contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream.
 
     Caches of dtype torch.float8_e4m3fn take quip_decode_attention_fp8 and need their per-slot fp32 scales k_scale /
-    v_scale (B, nkv, max_len): k_new / v_new are quantized on append (include/quip_b200.h has the format)."""
+    v_scale (B, nkv, max_len): k_new / v_new are quantized on append (include/quip_b200.h has the format).
+
+    page_table (B, max_pages) int32: the caches are page pools (n_pages, nkv, 64, hd), scales (n_pages, nkv, 64), and
+    slot j of row b lives at slot j % 64 of page page_table[b, j // 64] (quip_decode_attention_paged(_fp8)); a row that
+    would touch a page id outside [0, n_pages) writes nothing there and gets NaN."""
     if k_cache.dtype == torch.float8_e4m3fn:
-        return _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale)
+        return _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale, page_table)
     if k_scale is not None or v_scale is not None:
         raise ValueError('decode_attention: k_scale / v_scale go with float8_e4m3fn caches only')
     ts = (q, k_new, v_new, k_cache, v_cache)
@@ -113,8 +146,9 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
         raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
                          f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
     B, nh, hd = q.shape
-    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
-    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+    nkv = k_cache.shape[1]
+    rows, slots, max_len = _kv_layout('decode_attention', k_cache, B, page_table)
+    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
             tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,)):
         raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
                          f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
@@ -124,11 +158,17 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
     _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
     ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
     out = torch.empty_like(q)
+    st = torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        _lib.check(lib.quip_decode_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                             v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh, nkv, hd,
-                                             max_len, C.c_float(scale), ws.data_ptr(), ws.numel(),
-                                             torch.cuda.current_stream(q.device).cuda_stream))
+        if page_table is not None:
+            _lib.check(lib.quip_decode_attention_paged(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                                       k_cache.data_ptr(), v_cache.data_ptr(), positions.data_ptr(),
+                                                       out.data_ptr(), B, nh, nkv, hd, C.c_float(scale), ws.data_ptr(),
+                                                       ws.numel(), *_paged_args(page_table, rows), st))
+        else:
+            _lib.check(lib.quip_decode_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                 v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh, nkv,
+                                                 hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
     return out
 
 
@@ -142,7 +182,7 @@ def _check_cuda(fn, ts, dev):
             raise ValueError(f'{fn} takes contiguous tensors')
 
 
-def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale):
+def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale, page_table):
     if k_scale is None or v_scale is None:
         raise ValueError('decode_attention: float8_e4m3fn caches need k_scale and v_scale')
     if (any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or v_cache.dtype != torch.float8_e4m3fn or
@@ -153,10 +193,11 @@ def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, p
         raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
                          f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
     B, nh, hd = q.shape
-    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
-    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+    nkv = k_cache.shape[1]
+    rows, slots, max_len = _kv_layout('decode_attention', k_cache, B, page_table)
+    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
             tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
-            tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape):
+            tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape):
         raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
                          f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, scales '
                          f'{tuple(k_scale.shape)} / {tuple(v_scale.shape)}, positions {tuple(positions.shape)} do not agree')
@@ -166,12 +207,19 @@ def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, p
     _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
     ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
     out = torch.empty_like(q)
+    st = torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        _lib.check(lib.quip_decode_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                 v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
-                                                 positions.data_ptr(), out.data_ptr(), B, nh, nkv, hd, max_len,
-                                                 C.c_float(scale), ws.data_ptr(), ws.numel(),
-                                                 torch.cuda.current_stream(q.device).cuda_stream))
+        if page_table is not None:
+            _lib.check(lib.quip_decode_attention_paged_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                                           k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
+                                                           v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B,
+                                                           nh, nkv, hd, C.c_float(scale), ws.data_ptr(), ws.numel(),
+                                                           *_paged_args(page_table, rows), st))
+        else:
+            _lib.check(lib.quip_decode_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                                     k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
+                                                     v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh,
+                                                     nkv, hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
     return out
 
 
@@ -219,11 +267,12 @@ def sample(logits, temperature, top_k, top_p, seed, step, out):
     return out
 
 
-def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None):
+def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
     """quip_extend_attention(_fp8) on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot
     positions[b] + i of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots
     0 .. positions[b] + i.  fp16 q / k / v; fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale
-    (B, nkv, max_len).  CUDA, one device, contiguous; positions (B,) int64.  Returns (B, T, nh, hd) fp16."""
+    (B, nkv, max_len).  CUDA, one device, contiguous; positions (B,) int64.  Returns (B, T, nh, hd) fp16.
+    page_table: page pools as in decode_attention (quip_extend_attention_paged(_fp8))."""
     fp8 = k_cache.dtype == torch.float8_e4m3fn
     if not fp8 and (k_scale is not None or v_scale is not None):
         raise ValueError('extend_attention: k_scale / v_scale go with float8_e4m3fn caches only')
@@ -238,10 +287,11 @@ def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
         raise ValueError(f'extend_attention: q must be (B, T, nh, hd) and the caches (B, nkv, max_len, hd), got '
                          f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
     B, T, nh, hd = q.shape
-    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
-    if (tuple(k_cache.shape) != (B, nkv, max_len, hd) or v_cache.shape != k_cache.shape or
+    nkv = k_cache.shape[1]
+    rows, slots, max_len = _kv_layout('extend_attention', k_cache, B, page_table)
+    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
             tuple(k_new.shape) != (B, T, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
-            (fp8 and (tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape))):
+            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
         raise ValueError(f'extend_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
                          f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
                          f'{tuple(positions.shape)} do not agree')
@@ -254,7 +304,18 @@ def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
     out = torch.empty_like(q)
     st = torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        if fp8:
+        if page_table is not None and fp8:
+            _lib.check(lib.quip_extend_attention_paged_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                                           k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
+                                                           v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B, T,
+                                                           nh, nkv, hd, C.c_float(scale), ws.data_ptr(), ws.numel(),
+                                                           *_paged_args(page_table, rows), st))
+        elif page_table is not None:
+            _lib.check(lib.quip_extend_attention_paged(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                                       k_cache.data_ptr(), v_cache.data_ptr(), positions.data_ptr(),
+                                                       out.data_ptr(), B, T, nh, nkv, hd, C.c_float(scale),
+                                                       ws.data_ptr(), ws.numel(), *_paged_args(page_table, rows), st))
+        elif fp8:
             _lib.check(lib.quip_extend_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
                                                      v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
                                                      positions.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,
@@ -266,9 +327,9 @@ def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scal
     return out
 
 
-def _check_chunk(fn, k_cache, v_cache, positions, counts, k_scale, v_scale):
-    """The checks kv_append and prefill_attention share: cache and scale dtypes, positions / counts (B,) int64.
-    Returns whether the caches are e4m3."""
+def _check_chunk(fn, k_cache, v_cache, positions, counts, k_scale, v_scale, page_table=None):
+    """The checks kv_append and prefill_attention share: cache and scale dtypes, positions / counts (B,) int64, and the
+    page table with its pools.  Returns (whether the caches are e4m3, B, rows, max_len) (_kv_layout)."""
     fp8 = k_cache.dtype == torch.float8_e4m3fn
     if not fp8 and (k_scale is not None or v_scale is not None):
         raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn caches only')
@@ -280,23 +341,26 @@ def _check_chunk(fn, k_cache, v_cache, positions, counts, k_scale, v_scale):
         raise ValueError(f'{fn} takes fp16 or float8_e4m3fn caches (fp32 scales) and int64 positions and counts')
     if k_cache.dim() != 4:
         raise ValueError(f'{fn}: the caches must be (B, nkv, max_len, hd), got {tuple(k_cache.shape)}')
-    B, nkv, max_len, _ = k_cache.shape
+    B = k_cache.shape[0] if page_table is None else (positions.shape[0] if positions.dim() == 1 else -1)
+    nkv = k_cache.shape[1]
+    rows, slots, max_len = _kv_layout(fn, k_cache, B, page_table)
     if (v_cache.shape != k_cache.shape or tuple(positions.shape) != (B,) or tuple(counts.shape) != (B,) or
-            (fp8 and (tuple(k_scale.shape) != (B, nkv, max_len) or v_scale.shape != k_scale.shape))):
+            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
         raise ValueError(f'{fn}: shapes caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
                          f'{tuple(positions.shape)}, counts {tuple(counts.shape)} do not agree')
-    return fp8
+    return fp8, B, rows, max_len
 
 
-def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v_scale=None):
+def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v_scale=None, page_table=None):
     """quip_kv_append(_fp8) on torch tensors: token i of k_new / v_new (B, T, nkv, hd) fp16 to slot positions[b] + i of
     one layer's caches (B, nkv, max_len, hd) for i < counts[b]; nothing else is written.  fp16 caches, or
     float8_e4m3fn caches with fp32 k_scale / v_scale (B, nkv, max_len), quantized on the way.  CUDA, one device,
-    contiguous; positions / counts (B,) int64.  On the current stream."""
-    fp8 = _check_chunk('kv_append', k_cache, v_cache, positions, counts, k_scale, v_scale)
+    contiguous; positions / counts (B,) int64.  On the current stream.  page_table: page pools as in decode_attention
+    (quip_kv_append_paged(_fp8)); a slot whose page id lies outside the pool is not written."""
+    fp8, B, rows, max_len = _check_chunk('kv_append', k_cache, v_cache, positions, counts, k_scale, v_scale, page_table)
     if k_new.dtype != torch.float16 or v_new.dtype != torch.float16:
         raise ValueError('kv_append takes fp16 k_new / v_new')
-    B, nkv, max_len, hd = k_cache.shape
+    nkv, hd = k_cache.shape[1], k_cache.shape[3]
     if k_new.dim() != 4 or k_new.shape[0] != B or tuple(k_new.shape[2:]) != (nkv, hd) or v_new.shape != k_new.shape:
         raise ValueError(f'kv_append: k_new {tuple(k_new.shape)} / v_new {tuple(v_new.shape)} must be (B, T, nkv, hd) '
                          f'for caches {tuple(k_cache.shape)}')
@@ -305,7 +369,16 @@ def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v
     _check_cuda('kv_append', ts, k_new.device)
     lib, st = _lib.load(), torch.cuda.current_stream(k_new.device).cuda_stream
     with torch.cuda.device(k_new.device):
-        if fp8:
+        if page_table is not None and fp8:
+            _lib.check(lib.quip_kv_append_paged_fp8(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                    v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+                                                    positions.data_ptr(), counts.data_ptr(), B, T, nkv, hd,
+                                                    *_paged_args(page_table, rows), st))
+        elif page_table is not None:
+            _lib.check(lib.quip_kv_append_paged(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
+                                                v_cache.data_ptr(), positions.data_ptr(), counts.data_ptr(), B, T, nkv,
+                                                hd, *_paged_args(page_table, rows), st))
+        elif fp8:
             _lib.check(lib.quip_kv_append_fp8(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                               k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
                                               counts.data_ptr(), B, T, nkv, hd, max_len, st))
@@ -314,24 +387,36 @@ def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v
                                           positions.data_ptr(), counts.data_ptr(), B, T, nkv, hd, max_len, st))
 
 
-def prefill_attention(q, k_cache, v_cache, positions, counts, scale, k_scale=None, v_scale=None):
+def prefill_attention(q, k_cache, v_cache, positions, counts, scale, k_scale=None, v_scale=None, page_table=None):
     """quip_prefill_attention(_fp8) on torch tensors: q (B, T, nh, hd) fp16 attends causally over one layer's caches
     (B, nkv, max_len, hd), which already hold the chunk (kv_append): token i of row b over slots 0 .. positions[b] + i
     for i < counts[b]; rows i >= counts[b] are zero.  fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale.
-    CUDA, one device, contiguous; positions / counts (B,) int64.  Returns (B, T, nh, hd) fp16, on the current stream."""
-    fp8 = _check_chunk('prefill_attention', k_cache, v_cache, positions, counts, k_scale, v_scale)
+    CUDA, one device, contiguous; positions / counts (B,) int64.  Returns (B, T, nh, hd) fp16, on the current stream.
+    page_table: page pools as in decode_attention (quip_prefill_attention_paged(_fp8))."""
+    fp8, B, rows, max_len = _check_chunk('prefill_attention', k_cache, v_cache, positions, counts, k_scale, v_scale,
+                                         page_table)
     if q.dtype != torch.float16 or q.dim() != 4:
         raise ValueError(f'prefill_attention: q must be (B, T, nh, hd) fp16, got {tuple(q.shape)} {q.dtype}')
-    B, T, nh, hd = q.shape
-    nkv, max_len = k_cache.shape[1], k_cache.shape[2]
-    if tuple(k_cache.shape) != (B, nkv, max_len, hd):
+    T, nh, hd = q.shape[1:]
+    nkv = k_cache.shape[1]
+    if q.shape[0] != B or k_cache.shape[3] != hd:
         raise ValueError(f'prefill_attention: q {tuple(q.shape)} and caches {tuple(k_cache.shape)} do not agree')
     ts = (q, k_cache, v_cache, positions, counts) + ((k_scale, v_scale) if fp8 else ())
     _check_cuda('prefill_attention', ts, q.device)
     out = torch.empty_like(q)
     lib, st = _lib.load(), torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        if fp8:
+        if page_table is not None and fp8:
+            _lib.check(lib.quip_prefill_attention_paged_fp8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                            k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
+                                                            counts.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd,
+                                                            C.c_float(scale), *_paged_args(page_table, rows), st))
+        elif page_table is not None:
+            _lib.check(lib.quip_prefill_attention_paged(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                        positions.data_ptr(), counts.data_ptr(), out.data_ptr(), B, T,
+                                                        nh, nkv, hd, C.c_float(scale), *_paged_args(page_table, rows),
+                                                        st))
+        elif fp8:
             _lib.check(lib.quip_prefill_attention_fp8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                       k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
                                                       counts.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,

@@ -33,6 +33,13 @@ kernel alone in causal TFLOP/s against F.scaled_dot_product_attention(is_causal=
 48 x 4096 filled from 4000-token prompts in chunks of 512 followed by decode steps, with the fp16 cache bytes the HF path
 would have added.
 
+Section paged measures the paged KV cache (include/quip_b200.h; PromptDecoder(n_pages=...)): the decode kernel, the
+extend kernel at T = 5 and the prefill kernel (a 512-token chunk ending at the context) paged against contiguous on the
+same bytes, the pool scattered into shuffled pages (B in {1, 8, 32}, contexts 2048 / 4096, 7B and 70B shapes; the two
+launches alternate and each is timed three times), and on the 7B shape the generation of 128 tokens from a 2048-token
+prompt with 8 samples (num_return_sequences) and from 32 prompts sharing a 1536-token preamble, shared against unshared:
+prefill time, cache bytes, decode step time and tokens/s.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -569,6 +576,93 @@ def chunked_capacity(model, cfg, B, P, max_len, C, steps):
     return out
 
 
+def _scatter_pages(x, table):
+    """Pool (n_pages, nkv, 64, ...) holding slot j of row b of x (B, nkv, ctx, ...) at slot j % 64 of page
+    table[b, j // 64]."""
+    B, nkv, ctx = x.shape[:3]
+    pool = torch.empty((int(table.max()) + 1, nkv, 64) + tuple(x.shape[3:]), dtype=x.dtype, device=x.device)
+    pool[table.long().reshape(-1)] = x.view(B, nkv, ctx // 64, 64, *x.shape[3:]).transpose(1, 2).reshape(
+        B * (ctx // 64), nkv, 64, *x.shape[3:])
+    return pool
+
+
+def paged_kernels(nh, nkv, hd, B, ctx, reps):
+    """Decode, extend (T = 5) and prefill (T = 512) kernels at every row's context ctx: contiguous against paged over the
+    same bytes on shuffled pages.  Returns the median of three alternating timings of each and whether the outputs are
+    bit-identical."""
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(0)
+    kc = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    vc = torch.randn(B, nkv, ctx, hd, generator=g, device='cuda').half()
+    table = torch.randperm(B * (ctx // 64), generator=torch.Generator().manual_seed(1)).to(torch.int32)
+    table = table.view(B, ctx // 64).cuda()
+    kp, vp = _scatter_pages(kc, table), _scatter_pages(vc, table)
+    scale = hd ** -0.5
+    out = dict(nh=nh, nkv=nkv, hd=hd, B=B, context=ctx)
+    T5, T512 = 5, 512
+    q1 = torch.randn(B, nh, hd, generator=g, device='cuda').half()
+    kn1, vn1 = kc[:, :, -1].clone(), vc[:, :, -1].clone()
+    q5 = torch.randn(B, T5, nh, hd, generator=g, device='cuda').half()
+    kn5, vn5 = kc[:, :, -T5:].transpose(1, 2).contiguous(), vc[:, :, -T5:].transpose(1, 2).contiguous()
+    qp = torch.randn(B, T512, nh, hd, generator=g, device='cuda').half()
+    pos1 = torch.full((B,), ctx - 1, dtype=torch.long, device='cuda')
+    pos5 = torch.full((B,), ctx - T5, dtype=torch.long, device='cuda')
+    posp = torch.full((B,), ctx - T512, dtype=torch.long, device='cuda')
+    cnt = torch.full((B,), T512, dtype=torch.long, device='cuda')
+    kinds = dict(
+        decode=(lambda k, v, **kw: fused.decode_attention(q1, kn1, vn1, k, v, pos1, scale, **kw), reps),
+        extend=(lambda k, v, **kw: fused.extend_attention(q5, kn5, vn5, k, v, pos5, scale, **kw), reps),
+        prefill=(lambda k, v, **kw: fused.prefill_attention(qp, k, v, posp, cnt, scale, **kw), max(reps // 10, 10)))
+    for name, (fn, n) in kinds.items():
+        ms = {'contiguous': [], 'paged': []}
+        for _ in range(3):
+            ms['contiguous'].append(events_ms(lambda: fn(kc, vc), n))
+            ms['paged'].append(events_ms(lambda: fn(kp, vp, page_table=table), n))
+        a, b = (sorted(v)[1] for v in ms.values())
+        same = torch.equal(fn(kc, vc).view(torch.int16), fn(kp, vp, page_table=table).view(torch.int16))
+        out[name] = dict(contiguous_ms=a, paged_ms=b, paged_over_contiguous=b / a, bit_identical=same)
+    del kc, vc, kp, vp
+    torch.cuda.empty_cache()
+    return out
+
+
+def paged_generate(model, prompts, n_new, share, chunk=512, sample=False):
+    """What generate() does (capture, chunked prefill, captured steps), timed: prefill ms, decode ms per step, cache
+    bytes and tokens/s, unshared (contiguous cache) or with shared prefix pages (plan_prefix_pages).  Returns the
+    stats and the generated tokens."""
+    from quip_b200.decode import KV_PAGE, PromptDecoder, plan_prefix_pages
+    B = len(prompts)
+    max_len = max(len(p) for p in prompts) + n_new
+    pages, starts = {}, None
+    if share:
+        table, n_pages, starts = plan_prefix_pages(prompts, [len(p) + n_new for p in prompts],
+                                                   max_pages=-(-max_len // KV_PAGE))
+        pages = dict(page_table=table, n_pages=n_pages)
+    torch.cuda.synchronize()
+    dec = PromptDecoder(model, max_len=max_len, batch=B, max_new=n_new, sampling=sample, **pages)
+    if sample:
+        dec.set_sampling(temperature=0.8, seed=list(range(B)))
+    dec.capture()
+    cache = dec.k_cache.numel() * dec.k_cache.element_size() * 2
+    with torch.no_grad():
+        prefill_ms, _ = _peak(lambda: dec.prefill(prompts, chunk=chunk, starts=starts))
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(n_new - 1):
+            dec.step()
+        e1.record()
+        torch.cuda.synchronize()
+    step_ms = e0.elapsed_time(e1) / (n_new - 1)
+    fed = sum(len(p) - s for p, s in zip(prompts, starts or [0] * B))
+    r = dict(B=B, shared=share, prefill_ms=prefill_ms, prefilled_tokens=fed, cache_bytes=cache, decode_ms_per_step=step_ms,
+             tokens_per_s=B * n_new * 1e3 / (prefill_ms + step_ms * (n_new - 1)),
+             n_pages=pages.get('n_pages'), max_pages=-(-max_len // KV_PAGE))
+    gen = dec.generated.cpu()
+    del dec
+    torch.cuda.empty_cache()
+    return r, gen
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -576,7 +670,7 @@ def main():
     ap.add_argument('--layers70b', type=int, default=80, help='decoder layers of the 70B shape to build (of 80)')
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
-    ap.add_argument('--sections', default='kernel,prefill,decode,fp8')
+    ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged
     a = ap.parse_args()
     sections = set(a.sections.split(','))
     if not torch.cuda.is_available():
@@ -642,7 +736,17 @@ def main():
                 rec['extend_vs_prefill'].append(r)
                 print(f'{name} T=8 B={B} ctx=2048: extend {1e3 * r["extend_ms"]:.1f} us, append + prefill '
                       f'{1e3 * r["append_prefill_ms"]:.1f} us, rel err {r["rel_err"]:.1e}', flush=True)
-        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not ('chunked' in sections and
+        if 'paged' in sections:
+            rec['paged_kernel'] = []
+            for B in (1, 8, 32):
+                for ctx in (2048, 4096):
+                    r = paged_kernels(nh, nkv, hd, B, ctx, a.kernel_reps)
+                    rec['paged_kernel'].append(r)
+                    print(f'{name} paged kernels B={B} ctx={ctx}: ' + ', '.join(
+                        f'{k} {1e3 * r[k]["contiguous_ms"]:.1f} -> {1e3 * r[k]["paged_ms"]:.1f} us '
+                        f'({r[k]["paged_over_contiguous"]:.3f}x, same bits {r[k]["bit_identical"]})'
+                        for k in ('decode', 'extend', 'prefill')), flush=True)
+        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (sections & {'chunked', 'paged'} and
                                                                                   name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
@@ -659,6 +763,28 @@ def main():
                   f'({r["prefill_tokens_per_s"]:.0f} tokens/s, peak {r["prefill_peak_bytes_above_cache"] / 2**30:.2f} GiB '
                   f'above the {r["static_cache_bytes"] / 2**30:.1f} GiB cache), {r["decode_ms_per_step"]:.2f} ms/step; the '
                   f'HF path would add {r["hf_path_fp16_cache_bytes"] / 2**30:.1f} GiB of fp16 cache', flush=True)
+        if 'paged' in sections and name == 'llama7b':
+            g = torch.Generator().manual_seed(5)
+            V = cfg.vocab_size
+            one = torch.randint(0, V, (2048,), generator=g)
+            pre = torch.randint(0, V, (1536,), generator=g)
+            cases = dict(n8=([one] * 8, True),
+                         preamble32=([torch.cat((pre, torch.randint(0, V, (256,), generator=g))) for _ in range(32)],
+                                     False))
+            rec['paged_generate'] = {}
+            for case, (prompts, sample) in cases.items():
+                runs = {}
+                for share in (False, True):
+                    runs[share] = paged_generate(model, prompts, 128, share, sample=sample)
+                same = float((runs[False][1] == runs[True][1]).float().mean())
+                rec['paged_generate'][case] = dict(unshared=runs[False][0], shared=runs[True][0],
+                                                   same_token_share=same)
+                u, s_ = runs[False][0], runs[True][0]
+                print(f'{name} generate {case}: prefill {u["prefill_ms"]:.0f} -> {s_["prefill_ms"]:.0f} ms '
+                      f'({u["prefilled_tokens"]} -> {s_["prefilled_tokens"]} tokens), cache {u["cache_bytes"] / 2**30:.2f} '
+                      f'-> {s_["cache_bytes"] / 2**30:.2f} GiB, step {u["decode_ms_per_step"]:.2f} -> '
+                      f'{s_["decode_ms_per_step"]:.2f} ms, {u["tokens_per_s"]:.0f} -> {s_["tokens_per_s"]:.0f} tok/s, '
+                      f'same tokens {same:.3f}', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
