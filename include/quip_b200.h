@@ -320,6 +320,17 @@ int quip_sample_at(const void* logits, const float* temperature, const int32_t* 
                    const uint64_t* seed, const int64_t* steps, int64_t* tokens, int32_t B, int32_t T, int32_t V,
                    void* stream);
 
+/* Continuation scoring: for each row r of fp16 logits (R, V) with row stride ld (elements; rows need only 2-byte
+ * alignment) and t = targets[r] (int64):
+ *   logprob[r]   = (x_t - m) - log(sum_j exp(x_j - m)),  m = max_j x_j,  in fp32 (fp32 expf / logf);
+ *   is_greedy[r] = 1 if t is the lowest index holding the row's largest value (torch.argmax's tie rule), else 0 (uint8).
+ * A NaN anywhere in the row gives logprob NaN and is_greedy 0.  A target outside [0, V) is never dereferenced and gives
+ * NaN and 0 (the guard rule of the paged kernels).  One pass over the row; no workspace.  The per-thread partial sums
+ * are combined in a fixed order, so repeated launches are bit-identical, and a row's result does not depend on the
+ * other rows.  R >= 0 (0: nothing to do), V >= 1, ld >= V; targets 8-byte and logprob 4-byte aligned. */
+int quip_token_logprobs(const void* logits, int64_t ld, const int64_t* targets, float* logprob, uint8_t* is_greedy,
+                        int32_t R, int32_t V, void* stream);
+
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout
  * (bits 3: int32 (K*3/32, N) as Quant3Linear.pack writes it; bits 4: (K/8, N); bits 2: (K/16, N)):

@@ -109,6 +109,8 @@ EXPORTS = {
                                                                                    C.c_int32, C.c_void_p]),
     'quip_prefill_attention_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
                                                                                        C.c_int32, C.c_void_p]),
+    'quip_token_logprobs': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                      C.c_void_p]),
     'quip_ngram_draft':(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p]),
     'quip_spec_accept': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -442,13 +442,7 @@ class PromptDecoder(GraphDecoder):
         if self.paged:
             if page_table is None:
                 page_table = torch.arange(B * self.max_pages, dtype=torch.int32).view(B, self.max_pages)
-            page_table = torch.as_tensor(page_table).to(torch.int32).cpu()
-            if tuple(page_table.shape) != (B, self.max_pages):
-                raise ValueError(f'page_table must be (batch {B}, ceil(max_len / {KV_PAGE}) = {self.max_pages}), got '
-                                 f'{tuple(page_table.shape)}')
-            if bool(((page_table < -1) | (page_table >= self.n_pages)).any()):
-                raise ValueError(f'page ids must lie in [0, n_pages = {self.n_pages}) or be -1 (unmapped)')
-            self._page_map = page_table
+            self._page_map = self._checked_page_map(page_table)
             self.page_table = torch.full((B, self.max_pages), -1, dtype=torch.int32, device=self.dev)
         self.positions = torch.zeros(B, dtype=torch.long, device=self.dev)
         self.max_new = int(max_new)
@@ -465,6 +459,17 @@ class PromptDecoder(GraphDecoder):
             self.top_k = torch.zeros(B, dtype=torch.int32, device=self.dev)
             self.top_p = torch.ones(B, dtype=torch.float32, device=self.dev)
             self.seed = torch.zeros(B, dtype=torch.int64, device=self.dev)
+
+    def _checked_page_map(self, page_table):
+        """page_table as the host int32 (batch, max_pages) map prefill installs, after checking its shape and ids."""
+        B = self.batch
+        page_table = torch.as_tensor(page_table).to(torch.int32).cpu()
+        if tuple(page_table.shape) != (B, self.max_pages):
+            raise ValueError(f'page_table must be (batch {B}, ceil(max_len / {KV_PAGE}) = {self.max_pages}), got '
+                             f'{tuple(page_table.shape)}')
+        if bool(((page_table < -1) | (page_table >= self.n_pages)).any()):
+            raise ValueError(f'page ids must lie in [0, n_pages = {self.n_pages}) or be -1 (unmapped)')
+        return page_table
 
     def set_sampling(self, temperature=1.0, top_k=0, top_p=1.0, seed=0):
         """Write the sampling settings into the device buffers a captured step reads: each a scalar for every row or one
@@ -684,7 +689,31 @@ class PromptDecoder(GraphDecoder):
     def _pad_past_end(self):
         return self.paged and self._chunk is not None
 
-    def prefill(self, prompts, chunk=None, starts=None):
+    def _prefill_args(self, prompts, chunk, starts, page_table):
+        """The checked arguments of a prefill: (chunk, lens, starts, host page map or None); raises before any work."""
+        B = self.batch
+        if len(prompts) != B:
+            raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
+        chunk = _chunk_size(chunk)
+        if self.paged and chunk is None:
+            raise ValueError('a paged KV cache is filled by chunked prefill: pass chunk=C')
+        lens = [int(p.numel()) for p in prompts]
+        if min(lens) < 1:
+            raise ValueError('empty prompt')
+        P = max(lens)
+        if P > self.max_len:
+            raise ValueError(f'a prompt of {P} tokens does not fit a cache of {self.max_len} positions')
+        starts = [0] * B if starts is None else [int(x) for x in starts]
+        if len(starts) != B or any(x % KV_PAGE or not 0 <= x < n for x, n in zip(starts, lens)):
+            raise ValueError(f'starts must hold one multiple of {KV_PAGE} per row, below its prompt length; got {starts}')
+        if any(starts) and not self.paged:
+            raise ValueError('per-row prefill starts need a paged decoder (n_pages=...)')
+        if page_table is not None and not self.paged:
+            raise ValueError('a page_table needs a paged decoder (n_pages=...)')
+        page_map = None if page_table is None else self._checked_page_map(page_table)
+        return chunk, lens, starts, page_map
+
+    def prefill(self, prompts, chunk=None, starts=None, page_table=None):
         """Fill the cache from `prompts` (B 1-D id tensors).  Returns the logits after each prompt's last token
         (B, vocab); with max_new > 0 the token selected from them (argmax, or sampled at t = 0) is the first generated
         token and the next step's input.
@@ -707,24 +736,14 @@ class PromptDecoder(GraphDecoder):
         [max(c0, starts[b]), min(c0 + C, len_b)), the first at positions[b].  This is correct because (1) the owner of a
         page row b shares starts at or below that page, so it writes slot j of the page in the chunk holding j, the
         chunk of b's first token (starts[b] > j) or an earlier one; and (2) within a chunk, each layer's kv_append of
-        every row runs before that layer's prefill_attention, so b reads the slot after it is written."""
-        B = self.batch
-        if len(prompts) != B:
-            raise ValueError(f'{len(prompts)} prompts for a decoder of batch {B}')
-        chunk = _chunk_size(chunk)
-        if self.paged and chunk is None:
-            raise ValueError('a paged KV cache is filled by chunked prefill: pass chunk=C')
-        lens = [int(p.numel()) for p in prompts]
-        if min(lens) < 1:
-            raise ValueError('empty prompt')
-        P = max(lens)
-        if P > self.max_len:
-            raise ValueError(f'a prompt of {P} tokens does not fit a cache of {self.max_len} positions')
-        starts = [0] * B if starts is None else [int(x) for x in starts]
-        if len(starts) != B or any(x % KV_PAGE or not 0 <= x < n for x, n in zip(starts, lens)):
-            raise ValueError(f'starts must hold one multiple of {KV_PAGE} per row, below its prompt length; got {starts}')
-        if any(starts) and not self.paged:
-            raise ValueError('per-row prefill starts need a paged decoder (n_pages=...)')
+        every row runs before that layer's prefill_attention, so b reads the slot after it is written.
+
+        page_table: a new page map for this prefill (checked as the constructor checks it), so one paged decoder serves
+        batch after batch; default: the one given before."""
+        chunk, lens, starts, page_map = self._prefill_args(prompts, chunk, starts, page_table)
+        B, P = self.batch, max(lens)
+        if page_map is not None:
+            self._page_map = page_map
         if self.paged:
             self.page_table.copy_(self._page_map)
         ids = torch.zeros(B, P, dtype=torch.long, device=self.dev)
@@ -758,9 +777,28 @@ class PromptDecoder(GraphDecoder):
         M = B * T; attention by _attend_chunk).  Rows with nothing to feed ride along as padding and write nothing.
         The final norm and lm_head run once, on each row's last prompt token, gathered from the chunk it falls in.
         Leaves positions at lo of the last chunk (prefill sets them)."""
+        B = ids.shape[0]
+        h_last = p_last = None
+        for c0, T, lo, h, pend in self._chunks(ids, lens, C, starts):
+            ends = [b for b in range(B) if c0 < lens[b] <= c0 + T]                     # rows whose last token is here
+            if not ends:
+                continue
+            if h_last is None:
+                h_last = h.new_empty(B, 1, h.shape[-1])
+                p_last = None if pend is None else pend.new_empty(B, 1, pend.shape[-1])
+            r = torch.tensor(ends, dtype=torch.long, device=self.dev)
+            i = torch.tensor([lens[b] - 1 - lo[b] for b in ends], dtype=torch.long, device=self.dev)
+            h_last[r, 0] = h[r, i]
+            if pend is not None:
+                p_last[r, 0] = pend[r, i]
+        return self._head(h_last, p_last)
+
+    def _chunks(self, ids, lens, C, starts):
+        """The chunk loop of _prefill_chunks: for each chunk that feeds a token, runs the embedding and layer loops and
+        yields (c0, T, lo, h, pend) -- the chunk's first position, width, each row's first fed position and the layer
+        loops' output (B, T, hidden): token i of row b is position lo[b] + i (real for i < counts[b])."""
         B, P = ids.shape
         counts = torch.empty(B, dtype=torch.long, device=self.dev)
-        h_last = p_last = None
         for c0 in range(0, P, C):
             T = min(C, P - c0)
             lo = [max(c0, s) for s in starts]
@@ -780,18 +818,72 @@ class PromptDecoder(GraphDecoder):
                 h, pend = self._layers(self._embed(chunk_ids))
             finally:
                 self._chunk = None
-            ends = [b for b in range(B) if c0 < lens[b] <= c0 + T]                     # rows whose last token is here
-            if not ends:
-                continue
-            if h_last is None:
-                h_last = h.new_empty(B, 1, h.shape[-1])
-                p_last = None if pend is None else pend.new_empty(B, 1, pend.shape[-1])
-            r = torch.tensor(ends, dtype=torch.long, device=self.dev)
-            i = torch.tensor([lens[b] - 1 - lo[b] for b in ends], dtype=torch.long, device=self.dev)
-            h_last[r, 0] = h[r, i]
-            if pend is not None:
-                p_last[r, 0] = pend[r, i]
-        return self._head(h_last, p_last)
+            yield c0, T, lo, h, pend
+
+    def prefill_scores(self, prompts, targets, chunk, starts=None, page_table=None):
+        """Chunked prefill that scores the last n_b = len(targets[b]) positions of each prompt: position len_b - n_b + i
+        of row b against targets[b][i].  Returns (logprob (N,) fp32, is_greedy (N,) bool) over the N = sum n_b scored
+        tokens, row by row in order: log_softmax(logits)[target] and whether the target is the lowest index of the
+        largest logit (quip_token_logprobs, csrc/logprob.cu; on the CPU its torch restatement _token_logprobs_torch).
+
+        Arguments as prefill(chunk=C, starts, page_table); n_b may be 0 (a row that only rides along), and no scored
+        position may lie below starts[b] (a row has hidden states only for the positions it feeds).  In each chunk the
+        hidden states (and the pending residual) of the scored positions it holds are gathered, and the final norm and
+        lm_head run on those rows only: M = the chunk's scored tokens, not B * C; no (B, P, vocab) tensor and no
+        full-vocab fp32 tensor is made.  Positions are left at each row's length, as after prefill."""
+        chunk, lens, starts, page_map = self._prefill_args(prompts, chunk, starts, page_table)
+        if chunk is None:
+            raise ValueError('prefill_scores runs chunked prefill: pass chunk=C')
+        B = self.batch
+        if len(targets) != B:
+            raise ValueError(f'{len(targets)} target lists for a decoder of batch {B}')
+        targets = [torch.as_tensor(t, dtype=torch.long).reshape(-1).cpu() for t in targets]
+        n = [int(t.numel()) for t in targets]
+        if any(not starts[b] <= lens[b] - n[b] for b in range(B)) or any(k < 0 for k in n):
+            raise ValueError('each row scores at most its prompt length and nothing below its prefill start')
+        V = self.model.lm_head.out_features
+        if any(t.numel() and not (0 <= int(t.min()) and int(t.max()) < V) for t in targets):
+            raise ValueError(f'targets must lie in [0, {V})')
+        if page_map is not None:
+            self._page_map = page_map
+        if self.paged:
+            self.page_table.copy_(self._page_map)
+        P, N = max(lens), sum(n)
+        ids = torch.zeros(B, P, dtype=torch.long, device=self.dev)
+        for b, p in enumerate(prompts):
+            ids[b, :lens[b]] = p.reshape(-1).to(self.dev)
+        flat_t = torch.cat(targets).to(self.dev) if N else torch.zeros(0, dtype=torch.long, device=self.dev)
+        logprob = torch.empty(N, dtype=torch.float32, device=self.dev)
+        greedy = torch.empty(N, dtype=torch.uint8, device=self.dev)
+        first = [lens[b] - n[b] for b in range(B)]
+        off = [sum(n[:b]) for b in range(B)]
+        with torch.no_grad():
+            for c0, T, lo, h, pend in self._chunks(ids, lens, chunk, starts):
+                rows, cols, dst = [], [], []
+                for b in range(B):
+                    j0, j1 = max(first[b], lo[b]), min(lens[b], c0 + T)          # scored positions fed in this chunk
+                    for j in range(j0, j1):
+                        rows.append(b)
+                        cols.append(j - lo[b])
+                        dst.append(off[b] + j - first[b])
+                if not rows:
+                    continue
+                r = torch.tensor(rows, dtype=torch.long, device=self.dev)
+                i = torch.tensor(cols, dtype=torch.long, device=self.dev)
+                d = torch.tensor(dst, dtype=torch.long, device=self.dev)
+                logits = self._head(h[r, i][:, None], None if pend is None else pend[r, i][:, None])   # (M, vocab)
+                tg = flat_t[d]
+                if self._kernel:
+                    from . import fused
+                    lp, gr = fused.token_logprobs(logits, tg, torch.empty_like(tg, dtype=torch.float32),
+                                                  torch.empty_like(tg, dtype=torch.uint8))
+                else:
+                    lp, gr = _token_logprobs_torch(logits, tg)
+                logprob[d] = lp
+                greedy[d] = gr
+            self.positions.copy_(torch.tensor(lens, dtype=torch.long))
+            self._pos_host = list(lens)
+        return logprob, greedy.bool()
 
     def _first_token(self, logits):
         """Select the first generated token from the prefill's logits (B, vocab), at t = 0."""
@@ -1009,6 +1101,18 @@ def _sample_torch_at(logits, temperature, top_k, top_p, seed, steps):
             out[b, i] = _sample_torch(logits[b, i][None], temperature[b:b + 1], top_k[b:b + 1], top_p[b:b + 1],
                                       seed[b:b + 1], int(steps[b]) + i)[0]
     return out.to(logits.device)
+
+def _token_logprobs_torch(logits, targets):
+    """The rule of quip_token_logprobs (include/quip_b200.h) in torch, for the CPU path: (fp32 log_softmax gathered at
+    the targets, uint8 argmax == target), NaN and 0 for rows holding a NaN and for targets outside [0, V)."""
+    x = logits.float()
+    V = x.shape[-1]
+    ok = (targets >= 0) & (targets < V) & ~torch.isnan(x).any(-1)
+    t = targets.clamp(0, V - 1)
+    lp = torch.log_softmax(x, -1).gather(-1, t[:, None])[:, 0]
+    lp = torch.where(ok, lp, torch.full_like(lp, float('nan')))
+    return lp, ((x.argmax(-1) == t) & ok).to(torch.uint8)
+
 
 def _e4m3_quantize(x):
     """The e4m3 format of the fp8 cache (include/quip_b200.h) in torch, for the CPU step: x (..., hd) -> (e4m3 (..., hd),
@@ -1287,3 +1391,113 @@ def _generate_spec(dec, max_new, eos_t, stats):
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
     return out
+
+
+def _token_ids(name, seqs, vocab):
+    """seqs as lists of Python ints, checked on the host: each non-empty, every id in [0, vocab)."""
+    out = []
+    for s in seqs:
+        s = torch.as_tensor(s).reshape(-1).tolist() if torch.is_tensor(s) else [int(x) for x in s]
+        if not s:
+            raise ValueError(f'empty {name} sequence (the harness maps an empty context to [eot])')
+        if min(s) < 0 or max(s) >= vocab:
+            raise ValueError(f'{name}: token ids must lie in [0, vocab_size = {vocab})')
+        out.append(s)
+    return out
+
+
+def score_windows(contexts, continuations, max_length):
+    """The reference harness's request arithmetic (zeroShot/models/models_utils.py, BaseLM._loglikelihood_tokens):
+    identical token sequences ctx + cont are one request (its first occurrence's split is used), ordered by descending
+    length and then by the tokens; each is scored on inp = (ctx + cont)[-(max_length + 1):][:-1], whose last len(cont)
+    positions predict cont.  Returns [(inp, cont, caller indices)] in that order."""
+    groups = {}
+    for i, (c, x) in enumerate(zip(contexts, continuations)):
+        toks = tuple(c + x)
+        if toks in groups:
+            groups[toks][2].append(i)
+        else:
+            groups[toks] = (c, x, [i])
+    out = []
+    for toks in sorted(groups, key=lambda t: (-len(t), t)):
+        c, x, idx = groups[toks]
+        out.append(((c + x)[-(max_length + 1):][:-1], x, idx))
+    return out
+
+
+def score(model, contexts, continuations, batch_size=32, max_length=None, kv_dtype=None, prefill_chunk_size=512,
+          share_prompt_prefixes=True):
+    """Log-likelihoods of continuations: for each request (contexts[i], continuations[i]) (token-id sequences), the sum
+    over the continuation's tokens of log p(token | the tokens before it) and whether every continuation token is the
+    argmax of its logits -- the (logprob, is_greedy) of the reference harness's LM.loglikelihood, with its exact request
+    arithmetic (score_windows; max_length defaults to the model's max_position_embeddings).  One (float, bool) per
+    request, in the caller's order.  len(cont) >= 1 and len(ctx) >= 1 (the harness maps an empty context to [eot]).
+
+    The requests run batch_size at a time (the last batch padded with one-token rows whose results are dropped) through
+    one PromptDecoder by chunked prefill (prefill_chunk_size tokens per chunk) and PromptDecoder.prefill_scores: lm_head
+    runs only at the scored positions and csrc/logprob.cu turns their fp16 logits into log-probabilities and greedy
+    flags, so no (batch, length, vocab) tensor is made.  kv_dtype=torch.float8_e4m3fn keeps the cache in e4m3 as for
+    generation (the context then attends over its own quantized keys and values).
+
+    share_prompt_prefixes=True keeps the cache in 64-slot pages and plans each batch with plan_prefix_pages over
+    inp[:first scored position + 1] (budget len(inp)): a full page of a common prefix that ends at or before the first
+    scored position is prefilled and stored once -- a multiple-choice document's context is prefilled once for all its
+    choices.  One decoder serves every batch: its page pool holds the largest batch's plan and each batch installs its
+    own page table.  Results equal the unshared call's up to the rounding of other GEMM token counts.
+
+    Every argument (token ids against the vocabulary included) is checked on the host before any work."""
+    cfg = model.config
+    vocab = int(cfg.vocab_size)
+    if len(contexts) != len(continuations):
+        raise ValueError(f'{len(contexts)} contexts for {len(continuations)} continuations')
+    if not contexts:
+        raise ValueError('no requests')
+    ctxs = _token_ids('context', contexts, vocab)
+    conts = _token_ids('continuation', continuations, vocab)
+    if isinstance(batch_size, bool) or int(batch_size) != batch_size or batch_size < 1:
+        raise ValueError(f'batch_size must be an integer >= 1, got {batch_size!r}')
+    batch_size = int(batch_size)
+    chunk = _chunk_size(prefill_chunk_size)
+    if chunk is None:
+        raise ValueError('score prefills in chunks: prefill_chunk_size must be an integer >= 1')
+    max_length = int(cfg.max_position_embeddings) if max_length is None else max_length
+    if isinstance(max_length, bool) or int(max_length) != max_length or max_length < 1:
+        raise ValueError(f'max_length must be an integer >= 1, got {max_length!r}')
+    max_length = int(max_length)
+    if cfg.model_type == 'opt' and max_length > cfg.max_position_embeddings:
+        raise ValueError(f'max_length {max_length} exceeds the {cfg.max_position_embeddings} learned positions of the model')
+    if max(len(x) for x in conts) > max_length:
+        raise ValueError(f'a continuation is longer than max_length {max_length}')
+    if kv_dtype not in (None, torch.float16, torch.float8_e4m3fn, model.get_input_embeddings().weight.dtype):
+        raise ValueError(f'kv_dtype {kv_dtype} is not supported (None, the model dtype, float16 or float8_e4m3fn)')
+
+    reqs = score_windows(ctxs, conts, max_length)
+    B = min(batch_size, len(reqs))
+    max_len = len(reqs[0][0])                                     # the longest input comes first
+    batches = []
+    for s in range(0, len(reqs), B):
+        part = reqs[s:s + B]
+        inps = [torch.tensor(r[0], dtype=torch.long) for r in part] + [torch.zeros(1, dtype=torch.long)] * (B - len(part))
+        tgts = [torch.tensor(r[1], dtype=torch.long) for r in part] + [torch.zeros(0, dtype=torch.long)] * (B - len(part))
+        batches.append((part, inps, tgts))
+    plans, n_pages = [], None
+    if share_prompt_prefixes:
+        for _, inps, tgts in batches:
+            heads = [p[:p.numel() - t.numel() + 1] for p, t in zip(inps, tgts)]
+            plans.append(plan_prefix_pages(heads, [p.numel() for p in inps], max_pages=-(-max_len // KV_PAGE)))
+        n_pages = max(n for _, n, _ in plans)
+    dec = PromptDecoder(model, max_len=max_len, batch=B, kv_dtype=kv_dtype, n_pages=n_pages,
+                        page_table=plans[0][0] if plans else None)
+    res = [None] * len(ctxs)
+    for k, (part, inps, tgts) in enumerate(batches):
+        kw = dict(starts=plans[k][2], page_table=plans[k][0]) if plans else {}
+        lp, gr = dec.prefill_scores(inps, tgts, chunk, **kw)
+        lp, gr = lp.double().cpu(), gr.cpu()
+        o = 0
+        for inp, cont, idx in part:
+            n = len(cont)
+            ans = (float(lp[o:o + n].sum()), bool(gr[o:o + n].all()))
+            o += n
+            for i in idx:
+                res[i] = ans
+    return res

@@ -267,6 +267,39 @@ def sample(logits, temperature, top_k, top_p, seed, step, out):
     return out
 
 
+def token_logprobs(logits, targets, logprob_out, greedy_out):
+    """quip_token_logprobs on torch tensors: for each row r of logits (R, V) fp16 (rows may be strided: stride(1) == 1,
+    any stride(0) >= V) and targets (R,) int64, logprob_out[r] (fp32) = log_softmax(logits[r])[targets[r]] and
+    greedy_out[r] (uint8) = 1 when targets[r] is the lowest index of the row's largest value (the rule of
+    include/quip_b200.h: NaN rows and targets outside [0, V) give NaN and 0).  CUDA, one device; targets and the
+    outputs contiguous.  Everything is checked before the launch, which runs on the current stream.  Returns
+    (logprob_out, greedy_out)."""
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'token_logprobs: logits must be (R, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    R, V = logits.shape
+    if V < 1 or (R > 1 and logits.stride(0) < V) or (V > 1 and logits.stride(1) != 1):
+        raise ValueError(f'token_logprobs: logits rows must be unit-stride and not overlap, got shape {tuple(logits.shape)}'
+                         f' strides {tuple(logits.stride())}')
+    if R > 2 ** 31 - 1:
+        raise ValueError(f'token_logprobs: {R} rows exceed the launch limit of 2^31 - 1')
+    for name, t, dt in (('targets', targets, torch.int64), ('logprob_out', logprob_out, torch.float32),
+                        ('greedy_out', greedy_out, torch.uint8)):
+        if t.dtype != dt or tuple(t.shape) != (R,):
+            raise ValueError(f'token_logprobs: {name} must be ({R},) {dt}, got {tuple(t.shape)} {t.dtype}')
+    for t in (logits, targets, logprob_out, greedy_out):
+        if not t.is_cuda:
+            raise RuntimeError('token_logprobs runs on a CUDA device only (there is no CPU fallback)')
+        if t.device != logits.device:
+            raise ValueError('token_logprobs: all tensors must be on one device')
+    _check_cuda('token_logprobs', (targets, logprob_out, greedy_out), logits.device)
+    ld = logits.stride(0) if R > 1 else V
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_token_logprobs(logits.data_ptr(), ld, targets.data_ptr(), logprob_out.data_ptr(),
+                                                   greedy_out.data_ptr(), R, V,
+                                                   torch.cuda.current_stream(logits.device).cuda_stream))
+    return logprob_out, greedy_out
+
+
 def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
     """quip_extend_attention(_fp8) on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot
     positions[b] + i of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots

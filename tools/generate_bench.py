@@ -40,6 +40,11 @@ launches alternate and each is timed three times), and on the 7B shape the gener
 prompt with 8 samples (num_return_sequences) and from 32 prompts sharing a 1536-token preamble, shared against unshared:
 prefill time, cache bytes, decode step time and tokens/s.
 
+Section score (llama7b) measures continuation scoring: quip_token_logprobs alone (logits bytes read per second against
+3.35 TB/s, next to torch's log_softmax + gather + argmax) and, on an ARC-like synthetic set (--score-docs documents of 4
+choices), the reference harness's recipe against decode.score unshared, shared and shared with an e4m3 cache:
+requests/s, prefilled tokens, peak allocation and the largest per-request difference against the recipe.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -663,6 +668,114 @@ def paged_generate(model, prompts, n_new, share, chunk=512, sample=False):
     return r, gen
 
 
+def score_kernel_alone(R, V, reps):
+    """quip_token_logprobs on fp16 logits (R, V): logits bytes read per second against 3.35 TB/s, next to torch's
+    log_softmax(x.float()).gather plus argmax on the same tensor."""
+    from quip_b200 import fused
+    g = torch.Generator(device='cuda').manual_seed(R + V)
+    x = torch.randn(R, V, generator=g, device='cuda').half()
+    t = torch.randint(0, V, (R,), generator=g, device='cuda')
+    lp = torch.empty(R, device='cuda')
+    gr = torch.empty(R, dtype=torch.uint8, device='cuda')
+    ms = events_ms(lambda: fused.token_logprobs(x, t, lp, gr), reps)
+
+    def torch_way():
+        y = torch.log_softmax(x.float(), -1).gather(-1, t[:, None])[:, 0]
+        return y, x.argmax(-1) == t
+    tms = events_ms(torch_way, max(reps // 4, 5))
+    y, tg = torch_way()
+    nbytes = R * V * 2
+    return dict(R=R, V=V, kernel_ms=ms, bytes_per_s=nbytes / ms * 1e3, share_of_3_35_TBps=nbytes / ms * 1e3 / HBM_BPS,
+                torch_ms=tms, max_abs_diff=float((lp - y).abs().max()), greedy_equal=bool(torch.equal(gr.bool(), tg)))
+
+
+def score_workload(V, docs, seed=0):
+    """ARC-like synthetic requests: docs documents of 4 choices, a context of 64-512 random tokens shared within a
+    document, continuations of 1-16 tokens."""
+    g = torch.Generator().manual_seed(seed)
+    ctxs, conts = [], []
+    for _ in range(docs):
+        ctx = torch.randint(0, V, (int(torch.randint(64, 513, (1,), generator=g)),), generator=g).tolist()
+        for _ in range(4):
+            ctxs.append(ctx)
+            conts.append(torch.randint(0, V, (int(torch.randint(1, 17, (1,), generator=g)),), generator=g).tolist())
+    return ctxs, conts
+
+
+def score_reference_recipe(model, ctxs, conts, batch_size, max_length):
+    """The reference harness's recipe on the packed model: each batch right-padded to its longest request through
+    model(ids), fp32 log_softmax of the whole (B, S, V) logits, gather, argmax."""
+    from quip_b200.decode import score_windows
+    reqs = score_windows(ctxs, conts, max_length)
+    res, tokens = [None] * len(ctxs), 0
+    for s in range(0, len(reqs), batch_size):
+        part = reqs[s:s + batch_size]
+        P = len(part[0][0])
+        tokens += P * len(part)
+        ids = torch.zeros(len(part), P, dtype=torch.long)
+        for b, (inp, _, _) in enumerate(part):
+            ids[b, :len(inp)] = torch.tensor(inp)
+        with torch.no_grad():
+            lsm = torch.log_softmax(model(ids.cuda()).logits.float(), -1)
+        for b, (inp, cont, idx) in enumerate(part):
+            n = len(cont)
+            x = lsm[b, len(inp) - n:len(inp)]
+            c = torch.tensor(cont, device='cuda')
+            ans = (float(x.gather(-1, c[:, None]).double().sum()), bool((x.argmax(-1) == c).all()))
+            for i in idx:
+                res[i] = ans
+        del lsm
+    return res, tokens
+
+
+def score_arms(model, docs, batch_size, chunk):
+    """requests/s, prefilled tokens, peak allocation and the largest per-request difference against the reference recipe
+    for (a) the recipe, (b) score unshared, (c) score shared, (d) score shared with an e4m3 cache."""
+    import time
+
+    from quip_b200.decode import plan_prefix_pages, score, score_windows
+    V, L = model.config.vocab_size, 2048
+    ctxs, conts = score_workload(V, docs)
+    reqs = score_windows(ctxs, conts, L)
+
+    def prefilled(share):
+        n = 0
+        for s in range(0, len(reqs), batch_size):
+            part = reqs[s:s + batch_size]
+            if not share:
+                n += sum(len(r[0]) for r in part)
+                continue
+            heads = [torch.tensor(r[0][:len(r[0]) - len(r[1]) + 1]) for r in part]
+            starts = plan_prefix_pages(heads, [len(r[0]) for r in part])[2]
+            n += sum(len(r[0]) - st for r, st in zip(part, starts))
+        return n
+
+    arms = dict(recipe=lambda: score_reference_recipe(model, ctxs, conts, batch_size, L),
+                unshared=lambda: (score(model, ctxs, conts, batch_size=batch_size, max_length=L, prefill_chunk_size=chunk,
+                                        share_prompt_prefixes=False), prefilled(False)),
+                shared=lambda: (score(model, ctxs, conts, batch_size=batch_size, max_length=L, prefill_chunk_size=chunk),
+                                prefilled(True)),
+                shared_e4m3=lambda: (score(model, ctxs, conts, batch_size=batch_size, max_length=L,
+                                           prefill_chunk_size=chunk, kv_dtype=torch.float8_e4m3fn), prefilled(True)))
+    out, base = {}, None
+    for name, fn in arms.items():
+        fn()                                                         # warm-up: lazy set-up, workspaces
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        m0 = torch.cuda.memory_allocated()
+        t0 = time.perf_counter()
+        res, tokens = fn()
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+        base = res if base is None else base
+        out[name] = dict(seconds=dt, requests_per_s=len(ctxs) / dt, prefilled_tokens=tokens,
+                         peak_bytes_above_model=torch.cuda.max_memory_allocated() - m0,
+                         max_abs_diff_vs_recipe=max(abs(a[0] - b[0]) for a, b in zip(res, base)),
+                         is_greedy_agreement=sum(a[1] == b[1] for a, b in zip(res, base)) / len(res))
+    out.update(docs=docs, requests=len(ctxs), batch_size=batch_size, chunk=chunk)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -670,7 +783,9 @@ def main():
     ap.add_argument('--layers70b', type=int, default=80, help='decoder layers of the 70B shape to build (of 80)')
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
-    ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged
+    ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
+    #                                                                         score
+    ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
     if not torch.cuda.is_available():
@@ -746,10 +861,29 @@ def main():
                         f'{k} {1e3 * r[k]["contiguous_ms"]:.1f} -> {1e3 * r[k]["paged_ms"]:.1f} us '
                         f'({r[k]["paged_over_contiguous"]:.3f}x, same bits {r[k]["bit_identical"]})'
                         for k in ('decode', 'extend', 'prefill')), flush=True)
-        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (sections & {'chunked', 'paged'} and
-                                                                                  name == 'llama7b'):
+        if 'score' in sections and name == 'llama7b':
+            rec['score_kernel'] = []
+            for R in (64, 1024, 8192):
+                for V in (32000, 50272, 128256):
+                    r = score_kernel_alone(R, V, a.kernel_reps)
+                    rec['score_kernel'].append(r)
+                    print(f'score kernel R={R} V={V}: {1e3 * r["kernel_ms"]:.1f} us, {r["bytes_per_s"] / 1e12:.2f} TB/s '
+                          f'({100 * r["share_of_3_35_TBps"]:.0f}% of 3.35), torch log_softmax+gather+argmax '
+                          f'{1e3 * r["torch_ms"]:.1f} us, max diff {r["max_abs_diff"]:.1e}, greedy equal '
+                          f'{r["greedy_equal"]}', flush=True)
+                    torch.cuda.empty_cache()
+        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
+                sections & {'chunked', 'paged', 'score'} and name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
+        if 'score' in sections and name == 'llama7b':
+            r = score_arms(model, a.score_docs, 32, 512)
+            rec['score'] = r
+            for arm in ('recipe', 'unshared', 'shared', 'shared_e4m3'):
+                x = r[arm]
+                print(f'{name} score {arm}: {x["requests_per_s"]:.1f} requests/s, {x["prefilled_tokens"]} prefilled '
+                      f'tokens, peak {x["peak_bytes_above_model"] / 2**30:.2f} GiB, max |diff| vs recipe '
+                      f'{x["max_abs_diff_vs_recipe"]:.2e}, is_greedy agreement {x["is_greedy_agreement"]:.3f}', flush=True)
         if 'chunked' in sections and name == 'llama7b':
             rec['chunked_prefill'] = []
             for B, P in ((1, 2048), (8, 512), (8, 2048)):
