@@ -293,6 +293,40 @@ int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const vo
                                      int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale,
                                      const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
 
+/* Ragged (packed) chunks over a paged cache: S sequences of different lengths back to back in N token rows, so a step
+ * that mixes decode rows (one token each) and prompt chunks feeds no padding.  seq_start (S + 1) int64 on the device
+ * holds offsets 0 <= seq_start[0] <= ... <= seq_start[S] <= N: token i of sequence s is packed row seq_start[s] + i, at
+ * slot positions[s] + i (positions (S) int64) of row s of page_table (S, max_pages) -- the table rows of the S
+ * sequences.  k_new / v_new are (N, nkv, hd), q / out (N, nh, hd), fp16 token-major; the pools and scales as above.
+ * max_count >= 1 bounds every sequence's length (the attention grid is (query tile, kv head, sequence) with
+ * ceil(G * max_count / 64) tiles; a tile past its sequence's length exits at once).
+ *
+ * Guards: a sequence with positions[s] < 0, positions[s] + its length > max_pages * 64 or a length above max_count
+ * writes nothing and its outputs are NaN (as far as max_count reaches); a page outside the pool follows the paged rule.
+ * A sequence whose offsets break the order above or leave [0, N] is not looked at: nothing is read or written for it.
+ * There are no padding rows: out rows outside every sequence are not written.
+ *
+ * The rule: per sequence s, the ragged launch is bit-identical to the paged launch (quip_kv_append_paged(_fp8),
+ * quip_prefill_attention_paged(_fp8)) with B = S, T = max_count, counts[s] = seq_start[s + 1] - seq_start[s] and row s
+ * of the padded q / k_new / v_new holding the sequence's tokens, over the same cached bytes: each sequence runs the same
+ * query tiles, 64-slot blocks and arithmetic, and only the addressing of the packed rows differs. */
+int quip_kv_append_ragged(const void* k_new, const void* v_new, void* k_pool, void* v_pool, const int64_t* seq_start,
+                          const int64_t* positions, int32_t S, int32_t N, int32_t max_count, int32_t nkv, int32_t hd,
+                          const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
+int quip_kv_append_ragged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool, float* k_scale,
+                              float* v_scale, const int64_t* seq_start, const int64_t* positions, int32_t S, int32_t N,
+                              int32_t max_count, int32_t nkv, int32_t hd, const int32_t* page_table, int32_t max_pages,
+                              int32_t n_pages, void* stream);
+int quip_prefill_attention_ragged(const void* q, const void* k_pool, const void* v_pool, const int64_t* seq_start,
+                                  const int64_t* positions, void* out, int32_t S, int32_t N, int32_t max_count,
+                                  int32_t nh, int32_t nkv, int32_t hd, float scale, const int32_t* page_table,
+                                  int32_t max_pages, int32_t n_pages, void* stream);
+int quip_prefill_attention_ragged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale,
+                                      const float* v_scale, const int64_t* seq_start, const int64_t* positions,
+                                      void* out, int32_t S, int32_t N, int32_t max_count, int32_t nh, int32_t nkv,
+                                      int32_t hd, float scale, const int32_t* page_table, int32_t max_pages,
+                                      int32_t n_pages, void* stream);
+
 /* Token selection of one generation step: for each row b of logits (B, V) fp16 contiguous (rows need no alignment),
  * with T = temperature[b], k = top_k[b], p = top_p[b] and s = seed[b] (each (B), device) and t = *step (device; the
  * index of the token being chosen, 0 for the one after the prompt), tokens[b] (int64) is:

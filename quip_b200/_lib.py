@@ -109,6 +109,15 @@ EXPORTS = {
                                                                                    C.c_int32, C.c_void_p]),
     'quip_prefill_attention_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
                                                                                        C.c_int32, C.c_void_p]),
+    'quip_kv_append_ragged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.c_int32,
+                                                                            C.c_void_p]),
+    'quip_kv_append_ragged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.c_int32,
+                                                                                C.c_void_p]),
+    'quip_prefill_attention_ragged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 6 + [C.c_float, C.c_void_p, C.c_int32,
+                                                                                    C.c_int32, C.c_void_p]),
+    'quip_prefill_attention_ragged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 6 + [C.c_float, C.c_void_p,
+                                                                                        C.c_int32, C.c_int32,
+                                                                                        C.c_void_p]),
     'quip_token_logprobs': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_void_p]),
     'quip_ngram_draft':(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

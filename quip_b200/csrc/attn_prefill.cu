@@ -24,6 +24,13 @@
 // block's P.V.  That factor rides on the accumulator: O is kept as O' * c with c the last block's max s_v, so adding a
 // block rescales O' by alpha * c / max s_v once instead of keeping a second accumulator.
 //
+// RAGGED (paged only): the chunk is packed -- S sequences of different lengths back to back in N token rows, sequence s
+// the rows seq_start[s] .. seq_start[s + 1] - 1 -- so a mixed step of decode rows (one token each) and prompt chunks
+// feeds no padding rows.  The append runs one warp per packed head vector and finds its sequence by binary search over
+// seq_start; the attention grid is (query tile, kv head, sequence) with T = the longest sequence, and a tile past its
+// sequence's length exits at once.  A sequence's tiles, blocks and arithmetic are those of row b = s of the padded
+// launch with counts[s] = its length: only the addressing of q / out and of k_new / v_new differs.
+//
 // Fixed orders everywhere: bit-identical from run to run; a row's result depends on its own q, cache and counts only.
 #include <limits.h>
 #include <math.h>
@@ -90,20 +97,60 @@ __device__ __forceinline__ bool row_ok(int64_t pos, int64_t cnt, int T, int max_
   return pos >= 0 && cnt >= 0 && cnt <= T && pos + cnt <= max_len;
 }
 
+// The token rows of row (RAGGED: sequence) b of a chunk: returns how many there are and sets first (the first one's
+// index in q / out / k_new / v_new) and cnt (how many are real; -1 when the row's offsets are not looked at).  Padded:
+// row b owns rows b * T .. b * T + T - 1, cnt = counts[b].  RAGGED (seq = seq_start): rows seq[b] .. seq[b + 1] - 1, all
+// real; offsets outside 0 <= seq[b] <= seq[b + 1] <= n_tok give no rows (nothing read, written or output).
+template <bool RAGGED>
+__device__ __forceinline__ int seq_rows(const int64_t* __restrict__ seq, int64_t b, int T, int64_t n_tok,
+                                        int64_t& first, int64_t& cnt) {
+  if constexpr (RAGGED) {
+    const int64_t s0 = seq[b], s1 = seq[b + 1];
+    const bool in = s0 >= 0 && s0 <= s1 && s1 <= n_tok && s1 - s0 <= INT_MAX / PF_MAXG;
+    first = in ? s0 : 0;
+    cnt = in ? s1 - s0 : -1;
+    return in ? (int)cnt : 0;
+  } else {
+    first = b * T;
+    cnt = seq[b];
+    return T;
+  }
+}
+
 // One warp per new head vector v = (b, i, h) of k_new / v_new (B, T, nkv, HD): slot positions[b] + i of both caches
-// when i < counts[b] (PAGED: of the page pools, when the slot's page lies in the pool).
-template <bool FP8, bool PAGED, int HD>
+// when i < counts[b] (PAGED: of the page pools, when the slot's page lies in the pool).  RAGGED: v = (n, h) of k_new /
+// v_new (N, nkv, HD), counts is seq_start (S + 1) and B = S; packed row n is token i = n - seq_start[s] of the
+// sequence s holding it.
+template <bool FP8, bool PAGED, bool RAGGED, int HD>
 __global__ void __launch_bounds__(KA_WARPS * 32)
 kv_append_kernel(const __half* __restrict__ k_new, const __half* __restrict__ v_new, void* __restrict__ kc,
                  void* __restrict__ vc, float* __restrict__ ksc, float* __restrict__ vsc,
                  const int64_t* __restrict__ positions, const int64_t* __restrict__ counts, KvPages pg, int64_t nvec,
-                 int T, int nkv, int max_len) {
+                 int B, int T, int nkv, int max_len) {
+  static_assert(PAGED || !RAGGED, "the ragged chunk is paged only");
   const int64_t v = (int64_t)blockIdx.x * KA_WARPS + threadIdx.x / 32;
   if (v >= nvec) return;                      // warp-uniform
   const int lane = threadIdx.x & 31;
-  const int64_t b = v / ((int64_t)T * nkv);
-  const int i = (int)(v / nkv % T), h = (int)(v % nkv);
-  const int64_t pos = positions[b], cnt = counts[b];
+  const int h = (int)(v % nkv);
+  int64_t b, i, first, cnt;
+  if constexpr (RAGGED) {
+    const int64_t n = v / nkv;
+    int lo = 0, hi = B - 1;                   // the last sequence starting at or before n
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (counts[mid] <= n) lo = mid;
+      else hi = mid - 1;
+    }
+    b = lo;
+    const int rows = seq_rows<true>(counts, b, T, nvec / nkv, first, cnt);
+    i = n - first;
+    if (i < 0 || i >= rows) return;
+  } else {
+    b = v / ((int64_t)T * nkv);
+    i = v / nkv % T;
+    seq_rows<false>(counts, b, T, 0, first, cnt);
+  }
+  const int64_t pos = positions[b];
   if (!row_ok(pos, cnt, T, max_len) || i >= cnt) return;
   const int64_t slot = kv_vec<PAGED>(pg, b, h, nkv, max_len, pos + i);
   if (PAGED && slot < 0) return;              // a page outside the pool: not written
@@ -128,13 +175,15 @@ kv_append_kernel(const __half* __restrict__ k_new, const __half* __restrict__ v_
 
 // PAGED: kc / vc (and ksc / vsc) are the page pools and pg the page table; a 64-slot block is one page, looked up by
 // the load that stages it.  A block whose page lies outside the pool is zero-filled, never read, and every row that
-// sees one of its slots gets a NaN output.
-template <bool FP8, bool PAGED, int HD, int G>
+// sees one of its slots gets a NaN output.  RAGGED: q / out are packed (n_tok, nh, HD), counts is seq_start (S + 1),
+// blockIdx.z the sequence and T its longest length; a tile past the sequence's length exits at once.
+template <bool FP8, bool PAGED, bool RAGGED, int HD, int G>
 __global__ void __launch_bounds__(PF_THREADS)
 attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, const void* __restrict__ vc,
                     const float* __restrict__ ksc, const float* __restrict__ vsc, const int64_t* __restrict__ positions,
                     const int64_t* __restrict__ counts, __half* __restrict__ out, KvPages pg, int T, int nh, int nkv,
-                    int max_len, float scale) {
+                    int max_len, int64_t n_tok, float scale) {
+  static_assert(PAGED || !RAGGED, "the ragged chunk is paged only");
   using L = PfLayout<FP8, HD>;
   using CT = std::conditional_t<FP8, uint8_t, __half>;
   constexpr int KS = L::KS, BS = L::BS;
@@ -144,12 +193,14 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
 
   const int tile = gridDim.x - 1 - blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
-  const int R = G * T, r_lo = tile * PF_BM;
-  const int64_t pos = positions[b], cnt64 = counts[b];
+  int64_t first, cnt64;
+  const int R = G * seq_rows<RAGGED>(counts, b, T, n_tok, first, cnt64), r_lo = tile * PF_BM;
+  if (RAGGED && r_lo >= R) return;            // past the sequence: no rows of its own
+  const int64_t pos = positions[b];
   const bool ok = row_ok(pos, cnt64, T, max_len);
   const int cnt = ok ? (int)cnt64 : 0;
   const int i_lo = r_lo / G;                  // the tile's first token
-  auto out_row = [&](int r) { return out + (((int64_t)b * T + r / G) * nh + (int64_t)kvh * G + r % G) * HD; };
+  auto out_row = [&](int r) { return out + ((first + r / G) * nh + (int64_t)kvh * G + r % G) * HD; };
 
   if (i_lo >= cnt) {                          // nothing to attend: zero rows (NaN for a row that is not looked at)
     const uint4 z = ok ? make_uint4(0, 0, 0, 0) : make_uint4(0x7E007E00u, 0x7E007E00u, 0x7E007E00u, 0x7E007E00u);
@@ -182,7 +233,7 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const bool live = rr[h] < R && rr[h] / G < cnt;
-    const __half* qp = q + (((int64_t)b * T + rr[h] / G) * nh + (int64_t)kvh * G + rr[h] % G) * HD + 2 * tig;
+    const __half* qp = q + ((first + rr[h] / G) * nh + (int64_t)kvh * G + rr[h] % G) * HD + 2 * tig;
 #pragma unroll
     for (int kk = 0; kk < KT; ++kk) {
       qa[kk][h] = live ? __ldg(reinterpret_cast<const unsigned int*>(qp + 16 * kk)) : 0u;
@@ -396,25 +447,26 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
 bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
-template <bool FP8, bool PAGED, int HD, int G>
+template <bool FP8, bool PAGED, bool RAGGED, int HD, int G>
 int launch_prefill(dim3 grid, cudaStream_t st, const void* q, const void* kc, const void* vc, const float* ksc,
                    const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, KvPages pg, int T, int nh,
-                   int nkv, int max_len, float scale) {
+                   int nkv, int max_len, int64_t n_tok, float scale) {
   constexpr size_t smem = PfLayout<FP8, HD>::BYTES;
-  auto kern = attn_prefill_kernel<FP8, PAGED, HD, G>;
+  auto kern = attn_prefill_kernel<FP8, PAGED, RAGGED, HD, G>;
   if (smem > 48 * 1024) QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, PF_THREADS, smem, st>>>((const __half*)q, kc, vc, ksc, vsc, pos, cnt, (__half*)out, pg, T, nh, nkv,
-                                       max_len, scale);
+                                       max_len, n_tok, scale);
   QUIP_LAUNCHED("attn_prefill_kernel");
   return QUIP_OK;
 }
 
-template <bool FP8, bool PAGED, int HD>
+template <bool FP8, bool PAGED, bool RAGGED, int HD>
 int launch_prefill_g(int G, dim3 grid, cudaStream_t st, const void* q, const void* kc, const void* vc, const float* ksc,
                      const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, KvPages pg, int T, int nh,
-                     int nkv, int max_len, float scale) {
-#define PF_LAUNCH(g) \
-  return launch_prefill<FP8, PAGED, HD, g>(grid, st, q, kc, vc, ksc, vsc, pos, cnt, out, pg, T, nh, nkv, max_len, scale)
+                     int nkv, int max_len, int64_t n_tok, float scale) {
+#define PF_LAUNCH(g)                                                                                                  \
+  return launch_prefill<FP8, PAGED, RAGGED, HD, g>(grid, st, q, kc, vc, ksc, vsc, pos, cnt, out, pg, T, nh, nkv, max_len, \
+                                                   n_tok, scale)
   switch (G) {
     case 1: PF_LAUNCH(1);
     case 2: PF_LAUNCH(2);
@@ -428,21 +480,22 @@ int launch_prefill_g(int G, dim3 grid, cudaStream_t st, const void* q, const voi
 #undef PF_LAUNCH
 }
 
-// Argument checks and launches of quip_prefill_attention (FP8 false) and quip_prefill_attention_fp8 (FP8 true), and of
-// their paged twins (PAGED true: the caches and scales are page pools, max_len = max_pages * 64).
-template <bool FP8, bool PAGED = false>
+// Argument checks and launches of quip_prefill_attention (FP8 false) and quip_prefill_attention_fp8 (FP8 true), of
+// their paged twins (PAGED true: the caches and scales are page pools, max_len = max_pages * 64) and of the ragged ones
+// (RAGGED true: B = S sequences, counts = seq_start (S + 1) over n_tok packed rows, T = max_count).
+template <bool FP8, bool PAGED = false, bool RAGGED = false>
 int prefill_attention(const char* fn, const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
                       const float* v_scale, const int64_t* positions, const int64_t* counts, void* out, int32_t B,
                       int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* stream,
-                      KvPages pg = {}) {
+                      KvPages pg = {}, int32_t n_tok = 0) {
   QUIP_CHECK_ARG(q && k_cache && v_cache && positions && counts && out && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
   QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
                  "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
                  fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
-  QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
-                 "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
+  QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0 && n_tok >= 0,
+                 "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d, N %d)", fn, B, nh, nkv, max_len, n_tok);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
   QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= PF_MAXG,
                  "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head", fn, nh, nkv,
@@ -453,41 +506,44 @@ int prefill_attention(const char* fn, const void* q, const void* k_cache, const 
   const int G = nh / nkv;
   const dim3 grid(ceil_div((int64_t)G * T, PF_BM), nkv, B);
   const cudaStream_t st = (cudaStream_t)stream;
-  return hd == 64 ? launch_prefill_g<FP8, PAGED, 64>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions,
-                                                     counts, out, pg, T, nh, nkv, max_len, scale)
-                  : launch_prefill_g<FP8, PAGED, 128>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale, positions,
-                                                      counts, out, pg, T, nh, nkv, max_len, scale);
+  return hd == 64 ? launch_prefill_g<FP8, PAGED, RAGGED, 64>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale,
+                                                             positions, counts, out, pg, T, nh, nkv, max_len, n_tok,
+                                                             scale)
+                  : launch_prefill_g<FP8, PAGED, RAGGED, 128>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale,
+                                                              positions, counts, out, pg, T, nh, nkv, max_len, n_tok,
+                                                              scale);
 }
 
-// Argument checks and launches of quip_kv_append (FP8 false) and quip_kv_append_fp8 (FP8 true), and of their paged
-// twins.
-template <bool FP8, bool PAGED = false>
+// Argument checks and launches of quip_kv_append (FP8 false) and quip_kv_append_fp8 (FP8 true), and of their paged and
+// ragged twins (RAGGED: as prefill_attention; n_tok * nkv head vectors).
+template <bool FP8, bool PAGED = false, bool RAGGED = false>
 int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
               float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
-              int32_t hd, int32_t max_len, void* stream, KvPages pg = {}) {
+              int32_t hd, int32_t max_len, void* stream, KvPages pg = {}, int32_t n_tok = 0) {
   QUIP_CHECK_ARG(k_new && v_new && k_cache && v_cache && positions && counts && (!FP8 || (k_scale && v_scale)),
                  "%s: null pointer", fn);
   QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
   QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
                  "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
                  fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
-  QUIP_CHECK_ARG(B >= 0 && max_len > 0 && nkv > 0, "%s: bad sizes (B %d, nkv %d, max_len %d)", fn, B, nkv, max_len);
+  QUIP_CHECK_ARG(B >= 0 && max_len > 0 && nkv > 0 && n_tok >= 0, "%s: bad sizes (B %d, nkv %d, max_len %d, N %d)", fn,
+                 B, nkv, max_len, n_tok);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
   QUIP_CHECK_ARG(al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache), "%s: pointers must be 16-byte aligned",
                  fn);
   QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
-  const int64_t nvec = (int64_t)B * T * nkv;
+  const int64_t nvec = (RAGGED ? (B ? (int64_t)n_tok : 0) : (int64_t)B * T) * nkv;
   if (nvec == 0) return QUIP_OK;
   const unsigned blocks = (unsigned)((nvec + KA_WARPS - 1) / KA_WARPS);
   const cudaStream_t st = (cudaStream_t)stream;
   const __half* kn = (const __half*)k_new;
   const __half* vn = (const __half*)v_new;
   if (hd == 64)
-    kv_append_kernel<FP8, PAGED, 64><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale,
-                                                                       positions, counts, pg, nvec, T, nkv, max_len);
+    kv_append_kernel<FP8, PAGED, RAGGED, 64><<<blocks, KA_WARPS * 32, 0, st>>>(
+        kn, vn, k_cache, v_cache, k_scale, v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
   else
-    kv_append_kernel<FP8, PAGED, 128><<<blocks, KA_WARPS * 32, 0, st>>>(kn, vn, k_cache, v_cache, k_scale, v_scale,
-                                                                        positions, counts, pg, nvec, T, nkv, max_len);
+    kv_append_kernel<FP8, PAGED, RAGGED, 128><<<blocks, KA_WARPS * 32, 0, st>>>(
+        kn, vn, k_cache, v_cache, k_scale, v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
   QUIP_LAUNCHED("kv_append_kernel");
   return QUIP_OK;
 }
@@ -564,4 +620,48 @@ extern "C" int quip_prefill_attention_paged_fp8(const void* q, const void* k_poo
   return prefill_attention<true, true>("quip_prefill_attention_paged_fp8", q, k_pool, v_pool, k_scale, v_scale,
                                        positions, counts, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, stream,
                                        KvPages{page_table, max_pages, n_pages});
+}
+
+// Ragged twins: S packed sequences (seq_start (S + 1), positions (S), page_table (S, max_pages)) over N token rows; T is
+// max_count.
+extern "C" int quip_kv_append_ragged(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                     const int64_t* seq_start, const int64_t* positions, int32_t S, int32_t N,
+                                     int32_t max_count, int32_t nkv, int32_t hd, const int32_t* page_table,
+                                     int32_t max_pages, int32_t n_pages, void* stream) {
+  return kv_append<false, true, true>("quip_kv_append_ragged", k_new, v_new, k_pool, v_pool, nullptr, nullptr,
+                                      positions, seq_start, S, max_count, nkv, hd, paged_len(max_pages), stream,
+                                      KvPages{page_table, max_pages, n_pages}, N);
+}
+
+extern "C" int quip_kv_append_ragged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+                                         float* k_scale, float* v_scale, const int64_t* seq_start,
+                                         const int64_t* positions, int32_t S, int32_t N, int32_t max_count, int32_t nkv,
+                                         int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                         void* stream) {
+  return kv_append<true, true, true>("quip_kv_append_ragged_fp8", k_new, v_new, k_pool, v_pool, k_scale, v_scale,
+                                     positions, seq_start, S, max_count, nkv, hd, paged_len(max_pages), stream,
+                                     KvPages{page_table, max_pages, n_pages}, N);
+}
+
+extern "C" int quip_prefill_attention_ragged(const void* q, const void* k_pool, const void* v_pool,
+                                             const int64_t* seq_start, const int64_t* positions, void* out, int32_t S,
+                                             int32_t N, int32_t max_count, int32_t nh, int32_t nkv, int32_t hd,
+                                             float scale, const int32_t* page_table, int32_t max_pages,
+                                             int32_t n_pages, void* stream) {
+  return prefill_attention<false, true, true>("quip_prefill_attention_ragged", q, k_pool, v_pool, nullptr, nullptr,
+                                              positions, seq_start, out, S, max_count, nh, nkv, hd,
+                                              paged_len(max_pages), scale, stream,
+                                              KvPages{page_table, max_pages, n_pages}, N);
+}
+
+extern "C" int quip_prefill_attention_ragged_fp8(const void* q, const void* k_pool, const void* v_pool,
+                                                 const float* k_scale, const float* v_scale, const int64_t* seq_start,
+                                                 const int64_t* positions, void* out, int32_t S, int32_t N,
+                                                 int32_t max_count, int32_t nh, int32_t nkv, int32_t hd, float scale,
+                                                 const int32_t* page_table, int32_t max_pages, int32_t n_pages,
+                                                 void* stream) {
+  return prefill_attention<true, true, true>("quip_prefill_attention_ragged_fp8", q, k_pool, v_pool, k_scale, v_scale,
+                                             positions, seq_start, out, S, max_count, nh, nkv, hd,
+                                             paged_len(max_pages), scale, stream,
+                                             KvPages{page_table, max_pages, n_pages}, N);
 }

@@ -23,8 +23,12 @@ its step selects by temperature, top-k and top-p with a per-row seed (quip_sampl
 include/quip_b200.h) instead of argmax, from settings held in device buffers, so one captured graph serves any settings.
 `SpecDecoder` (generate(..., prompt_lookup_num_tokens=k)) verifies k prompt-lookup drafts per row in each captured step:
 T = k + 1 tokens per row through the same layer loops, attention by csrc/attn_decode.cu's extend kernel, drafting and
-acceptance by csrc/spec.cu.
+acceptance by csrc/spec.cu.  `ContinuousDecoder` (generate(..., max_batch_size=n)) serves requests continuously: each
+holds a decode row and its own pages only while it runs, and queued prompts join through ragged mixed steps
+(csrc/attn_prefill.cu's ragged kernels), scheduled by `ContinuousSchedule`.
 """
+import collections
+import heapq
 import math
 
 import torch
@@ -1050,6 +1054,322 @@ class SpecDecoder(PromptDecoder):
         return self.logits
 
 
+class _Ragged:
+    """The packed layout of a mixed step: S sequences over N tokens (fused.RaggedChunk `seqs`), the decoder rows they
+    belong to (`rows`, host list, and `rows_t`), each sequence's first position `seq_pos` (S,), its table rows `table`
+    (S, max_pages), and per token its sequence `tok_seq` and position `tok_pos` (N,)."""
+
+    def __init__(self, seqs, rows, rows_t, seq_pos, table, tok_seq, tok_pos):
+        self.seqs, self.rows, self.rows_t, self.seq_pos, self.table = seqs, rows, rows_t, seq_pos, table
+        self.tok_seq, self.tok_pos = tok_seq, tok_pos
+
+
+class ContinuousDecoder(PromptDecoder):
+    """Paged PromptDecoder whose rows serve requests that come and go (generate(..., max_batch_size=batch)).
+
+    Every row has its own device counters: `active` (it holds a request), `n_gen` (tokens generated), `budget` (its
+    max_new_tokens) and `done` (an EOS from `eos`, or n_gen reached budget).  A row is live when active and not done.
+    Two kinds of step run over the same buffers:
+
+      * decode_step: every row feeds tokens[b] at positions[b] (quip_decode_attention_paged(_fp8)); captured once as a
+        CUDA graph and used whenever no row is prefilling.  An idle row's table row is unmapped (-1), so it reads and
+        writes nothing and its NaN logits still select an in-range id;
+      * mixed_step (eager): the layer loops run on one packed sequence of N tokens -- one token of each decoding row and
+        pieces of the prompts being prefilled -- with a per-token position (rotary rows, OPT's learned positions) and
+        attention by quip_kv_append_ragged / quip_prefill_attention_ragged(_fp8).  The final norm and lm_head run only
+        on the tokens that produce one: each decoding row's, and the last prompt token of each prompt that ends here.
+
+    Selection (both kinds): argmax, or with sampling the rule of quip_sample_at at step n_gen[b] (0 for the first
+    token), so a request's tokens depend on its own logits, settings and seed only.  A live row then stores its token
+    in generated[b, n_gen[b]] (the column clamped into the buffer), advances positions and n_gen, and sets done.  A row
+    that is not live advances nothing; a done row still rewrites its own slot positions[b] (inside its reserved pages)
+    until the host retires it.  On the CPU both steps run eagerly, the ragged attention in torch (per-sequence scatter
+    through the table, SDPA under each sequence's causal mask)."""
+
+    def __init__(self, model, max_len, batch, n_pages, max_new, ops=None, kv_dtype=None, sampling=False, eos=()):
+        max_pages = -(-int(max_len) // KV_PAGE)
+        super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
+                         sampling=sampling, n_pages=n_pages,
+                         page_table=torch.full((int(batch), max_pages), -1, dtype=torch.int32))
+        B, dev = self.batch, self.dev
+        self.n_gen = torch.zeros(B, dtype=torch.long, device=dev)
+        self.budget = torch.zeros(B, dtype=torch.long, device=dev)
+        self.active = torch.zeros(B, dtype=torch.bool, device=dev)
+        self.done = torch.zeros(B, dtype=torch.bool, device=dev)
+        self.eos = torch.tensor([int(e) for e in eos], dtype=torch.long, device=dev)
+        self._ragged = None
+
+    # ---- per-row requests
+
+    def admit(self, row, pages, budget, settings=None):
+        """Give row `row` a new request: its pages (host ids, mapped from slot 0 on), its budget of new tokens and, when
+        sampling, its (temperature, top_k, top_p, seed).  Its prompt is then fed by mixed steps."""
+        tbl = torch.full((self.max_pages,), -1, dtype=torch.int32)
+        tbl[:len(pages)] = torch.tensor(pages, dtype=torch.int32)
+        self.page_table[row].copy_(tbl)
+        self.active[row] = True
+        self.done[row] = False
+        self.n_gen[row] = 0
+        self.budget[row] = int(budget)
+        self.positions[row] = 0
+        if self.sampling:
+            t, k, p, s = settings
+            self.temperature[row] = float(t)
+            self.top_k[row] = int(k)
+            self.top_p[row] = float(p)
+            self.seed[row] = s - 2 ** 64 if s >= 2 ** 63 else s
+
+    def retire(self, row):
+        """Unmap row `row`'s pages and make it idle."""
+        self.page_table[row].fill_(-1)
+        self.active[row] = False
+
+    # ---- selection and the per-row update shared by both steps
+
+    def _choose(self, logits, rows):
+        """Tokens for rows (M,) from their logits (M, vocab), each at its own step n_gen."""
+        if not self.sampling:
+            return logits.argmax(-1)
+        args = (self.temperature[rows], self.top_k[rows], self.top_p[rows], self.seed[rows], self.n_gen[rows])
+        if self._kernel:
+            from . import fused
+            out = torch.empty(rows.shape[0], 1, dtype=torch.long, device=self.dev)
+            return fused.sample_at(logits[:, None], *args, out)[:, 0]
+        return _sample_torch_at(logits[:, None], *args)[:, 0]
+
+    def _commit(self, rows, tok):
+        n = self.n_gen[rows]
+        live = self.active[rows] & ~self.done[rows]
+        col = n.clamp(max=self.generated.shape[1] - 1)
+        self.generated[rows, col] = torch.where(live, tok, self.generated[rows, col])
+        self.tokens[rows] = torch.where(live, tok, self.tokens[rows])
+        n = n + live.long()
+        self.n_gen[rows] = n
+        self.positions[rows] = self.positions[rows] + live.long()
+        stop = (tok[:, None] == self.eos[None]).any(1) | (n >= self.budget[rows])
+        self.done[rows] = self.done[rows] | (live & stop)
+
+    def _advance(self):
+        self._commit(self._rows, self._choose(self.logits, self._rows))
+
+    def _capture_state(self):
+        return super()._capture_state() + [self.n_gen, self.active, self.done]
+
+    def decode_step(self):
+        """One decode step of every row (a graph replay once captured); returns the logits (batch, vocab)."""
+        if self.graph is None:
+            with torch.no_grad():
+                self._step()
+        else:
+            self.graph.replay()
+        return self.logits
+
+    # ---- the mixed step
+
+    def mixed_step(self, decoding, pieces):
+        """One eager step over a packed sequence: one token of each row in `decoding` (its tokens[b] at positions[b]),
+        then each piece (row, ids, first, ends) -- prompt tokens ids (1-D) of that row at positions first, first + 1, ..,
+        ends True when they finish the prompt, whose last token then selects the row's first generated token.  Returns
+        the logits (M, vocab) of the tokens that selected one -- the decoding rows', then the ending pieces' -- or None."""
+        dev = self.dev
+        rows = list(decoding) + [p[0] for p in pieces]
+        counts = [1] * len(decoding) + [int(p[1].numel()) for p in pieces]
+        offs = [0]
+        for c in counts:
+            offs.append(offs[-1] + c)
+        S, nd = len(rows), len(decoding)
+        from . import fused
+        seqs = fused.RaggedChunk(offs, dev)
+        with torch.no_grad():
+            rows_t = torch.tensor(rows, dtype=torch.long).to(dev)
+            if pieces:
+                self.positions[rows_t[nd:]] = torch.tensor([int(p[2]) for p in pieces], dtype=torch.long).to(dev)
+            ids = torch.cat([torch.zeros(nd, dtype=torch.long)] +
+                            [torch.as_tensor(p[1]).reshape(-1).long().cpu() for p in pieces]).to(dev)
+            if nd:
+                ids[:nd] = self.tokens[rows_t[:nd]]
+            seq_pos = self.positions[rows_t]
+            tok_seq = torch.repeat_interleave(torch.arange(S), torch.tensor(counts)).to(dev)
+            tok_off = torch.cat([torch.arange(c) for c in counts]).to(dev)
+            self._ragged = _Ragged(seqs, rows, rows_t, seq_pos, self.page_table[rows_t], tok_seq,
+                                   seq_pos[tok_seq] + tok_off)
+            try:
+                h, pend = self._layers(self._embed(ids[None]))
+            finally:
+                self._ragged = None
+            ends = [j for j, p in enumerate(pieces) if p[3]]
+            out_rows = list(decoding) + [pieces[j][0] for j in ends]
+            if not out_rows:
+                return None
+            idx = torch.tensor(list(range(nd)) + [offs[nd + j + 1] - 1 for j in ends], dtype=torch.long).to(dev)
+            out_t = torch.tensor(out_rows, dtype=torch.long).to(dev)
+            if ends:                              # at a prompt's last token: positions[b] is that token's, as for a step
+                last = [int(pieces[j][2]) + int(pieces[j][1].numel()) - 1 for j in ends]
+                self.positions[out_t[nd:]] = torch.tensor(last, dtype=torch.long).to(dev)
+            logits = self._head(h[0, idx][:, None], None if pend is None else pend[0, idx][:, None])
+            self._commit(out_t, self._choose(logits, out_t))
+        return logits
+
+    def _rope_rows(self, pos, T):
+        if self._ragged is None:
+            return super()._rope_rows(pos, T)
+        p = self._ragged.tok_pos
+        return self.cos.index_select(0, p), self.sin.index_select(0, p)
+
+    def _embed(self, tokens=None):
+        if self._ragged is None or self.family == 'llama':
+            return super()._embed(tokens)
+        d = self.model.model.decoder                  # OPT: the learned position of every packed token
+        h = d.embed_tokens(tokens)
+        if d.project_in is not None:
+            h = d.project_in(h)
+        return h + F.embedding(self._ragged.tok_pos + d.embed_positions.offset, d.embed_positions.weight)[None]
+
+    def _attn_mask(self, pos, T=1):
+        return None if self._ragged is not None else super()._attn_mask(pos, T)
+
+    def _attend(self, li, q, k, v, mask, scale):
+        if self._ragged is None:
+            return super()._attend(li, q, k, v, mask, scale)
+        return self._attend_ragged(li, q, k, v, scale)
+
+    def _attend_ragged(self, li, q, k, v, scale):
+        """_attend of a mixed step: q (1, nh, N, hd), k / v (1, nkv, N, hd), token i of sequence s appended at slot
+        seq_pos[s] + i of its row and attending over slots 0 .. seq_pos[s] + i.  Returns (1, N, nh * hd)."""
+        rg, (nh, N, hd), nkv = self._ragged, q.shape[1:], self.nkv
+        qt, kt, vt = (x[0].transpose(0, 1) for x in (q, k, v))                            # (N, heads, hd)
+        if self._kernel:
+            from . import fused
+            kw = dict(k_scale=self.k_scale[li], v_scale=self.v_scale[li]) if self._fp8 else {}
+            fused.kv_append_ragged(kt.contiguous(), vt.contiguous(), self.k_cache[li], self.v_cache[li], rg.seqs,
+                                   rg.seq_pos, rg.table, **kw)
+            o = fused.prefill_attention_ragged(qt.contiguous(), self.k_cache[li], self.v_cache[li], rg.seqs,
+                                               rg.seq_pos, rg.table, scale, **kw)
+            return o.view(1, N, nh * hd)
+        self._store(li, rg.rows_t[rg.tok_seq], rg.tok_pos, kt, vt)
+        kk, vv = self._cached(li, q.dtype)
+        out, offs = [], rg.seqs.offsets
+        for s, b in enumerate(rg.rows):
+            a, e = offs[s], offs[s + 1]
+            p = rg.tok_pos[a:e]
+            seen = (self._arange <= p[-1])[None, :, None]                               # whatever lies past: not read
+            ks, vs = torch.where(seen, kk[b], 0), torch.where(seen, vv[b], 0)
+            if nkv != nh:
+                ks = ks.repeat_interleave(nh // nkv, dim=0)
+                vs = vs.repeat_interleave(nh // nkv, dim=0)
+            mask = (self._arange[None] <= p[:, None])[None]                             # (1, count, max_len)
+            o = F.scaled_dot_product_attention(q[0, :, a:e], ks, vs, attn_mask=mask, scale=scale)
+            out.append(o.transpose(0, 1).reshape(e - a, nh * hd))
+        return torch.cat(out)[None]
+
+
+class ContinuousSchedule:
+    """The host side of continuous batching (generate(..., max_batch_size=rows)): which request holds which decoder row
+    and pages, and what each step feeds.  Deterministic, and free of device work so it can be checked on its own.
+
+      * admission: FIFO in the caller's order.  The head request is admitted when a row is free and the pool has its
+        whole budget free, need = ceil((len + max_new) / 64) pages; it takes the lowest free row and the lowest free page
+        ids.  Pages are reserved at admission, so nothing is allocated mid-flight and nothing is preempted;
+      * steps (plan): one token of each decoding row (admitted, prompt fed, not retired), plus up to `chunk` prompt
+        tokens of the rows still prefilling, taken in admission order -- a long prompt spans several steps and several
+        short ones can share a step;
+      * retirement (retire): the row and its pages go back to the free lists.
+    A request whose budget exceeds the pool raises ValueError here, before any work."""
+
+    def __init__(self, lens, max_new, rows, n_pages, chunk):
+        self.lens, self.max_new = [int(n) for n in lens], [int(m) for m in max_new]
+        self.need = [-(-(n + m) // KV_PAGE) for n, m in zip(self.lens, self.max_new)]
+        self.chunk = int(chunk)
+        if max(self.need) > n_pages:
+            raise ValueError(f'a request needs {max(self.need)} pages of {KV_PAGE} slots (prompt and new tokens), the '
+                             f'pool holds {n_pages}')
+        self.queue = collections.deque(range(len(self.lens)))
+        self.free_rows = list(range(int(rows)))
+        self.free_pages = list(range(int(n_pages)))
+        self.req = [None] * int(rows)                # the request each row holds
+        self.pages = [[] for _ in range(int(rows))]
+        self.fed = [0] * int(rows)                   # prompt tokens fed
+        self.filling = []                            # rows still prefilling, in admission order
+
+    def admit(self):
+        """Admit what the policy allows now: [(row, request, pages)]."""
+        out = []
+        while self.queue and self.free_rows and len(self.free_pages) >= self.need[self.queue[0]]:
+            i = self.queue.popleft()
+            r = heapq.heappop(self.free_rows)
+            pages = [heapq.heappop(self.free_pages) for _ in range(self.need[i])]
+            self.req[r], self.pages[r], self.fed[r] = i, pages, 0
+            self.filling.append(r)
+            out.append((r, i, pages))
+        return out
+
+    def plan(self):
+        """The next step: (decoding rows, pieces), a piece (row, first prompt position, count); the pieces count as fed.
+        No pieces: a decode step."""
+        decoding = [r for r, i in enumerate(self.req) if i is not None and r not in self.filling]
+        pieces, left = [], self.chunk
+        for r in self.filling:
+            if not left:
+                break
+            n = min(self.lens[self.req[r]] - self.fed[r], left)
+            pieces.append((r, self.fed[r], n))
+            self.fed[r] += n
+            left -= n
+        self.filling = [r for r in self.filling if self.fed[r] < self.lens[self.req[r]]]
+        return decoding, pieces
+
+    def retire(self, r):
+        """Free row r and its pages; returns the request it held."""
+        i = self.req[r]
+        for p in self.pages[r]:
+            heapq.heappush(self.free_pages, p)
+        heapq.heappush(self.free_rows, r)
+        self.req[r], self.pages[r] = None, []
+        return i
+
+    @property
+    def finished(self):
+        return not self.queue and all(i is None for i in self.req)
+
+
+def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len):
+    """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages."""
+    lens = [p.numel() for p in prompts]
+    sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk)
+    dec = ContinuousDecoder(model, max_len, rows, kv_pages, max(max_new), kv_dtype=kv_dtype,
+                            sampling=settings is not None, eos=eos)
+    if dec.dev.type == 'cuda':
+        dec.capture()                                # before any row is mapped: the warm-up steps write nothing
+    out = [None] * len(prompts)
+    eos_c = torch.tensor(eos, dtype=torch.long)
+    steps = 0
+    while True:
+        if sched.queue or steps % EOS_CHECK_EVERY == 0:
+            held = [r for r, i in enumerate(sched.req) if i is not None]
+            done = dec.done.cpu()
+            fin = [r for r in held if done[r]]
+            if fin:
+                fin_t = torch.tensor(fin, dtype=torch.long).to(dec.dev)
+                gen, n_gen = dec.generated[fin_t].cpu(), dec.n_gen[fin_t].cpu()
+                for j, r in enumerate(fin):
+                    row = gen[j, :int(n_gen[j])]
+                    hit = torch.isin(row, eos_c).nonzero()
+                    out[sched.retire(r)] = row[:int(hit[0]) + 1] if hit.numel() else row
+                    dec.retire(r)
+            for r, i, pages in sched.admit():
+                dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings])
+        if sched.finished:
+            break
+        decoding, pieces = sched.plan()
+        if pieces:
+            dec.mixed_step(decoding, [(r, prompts[sched.req[r]][lo:lo + n], lo, lo + n == lens[sched.req[r]])
+                                      for r, lo, n in pieces])
+        else:
+            dec.decode_step()
+        steps += 1
+    return out
+
+
 def _ngram_draft_torch(hist, positions, k, n_min, n_max):
     """The rule of quip_ngram_draft (include/quip_b200.h) in torch, one row at a time: (B, 1 + k)."""
     B, max_len = hist.shape
@@ -1258,7 +1578,8 @@ def _sampling_settings(n, temperature, top_k, top_p, seed):
 
 def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
-             spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1):
+             spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
+             max_batch_size=None, kv_pages=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -1293,7 +1614,26 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     prompt, len(prompts) * n tensors in (prompt, sample) order: by definition, what
     generate([p for p in prompts for _ in range(n)], share_prompt_prefixes=True, ...) returns -- an int seed s gives
     output row r the seed s + r, and a list setting takes one value per output row.  A prompt is prefilled once, but
-    for its last partial page and last token."""
+    for its last partial page and last token.
+
+    max_new_tokens may also be a list with one value per prompt (per output row with num_return_sequences): each row is
+    cut to its own budget.
+
+    max_batch_size=n (default None: one fixed batch of every prompt) serves the prompts continuously on n decode rows
+    (ContinuousDecoder, ContinuousSchedule), by this deterministic policy:
+      * admission is FIFO in the caller's order: the next prompt is admitted when a row is free and the page pool has
+        its whole budget free, ceil((len + max_new) / 64) pages of 64 slots, reserved at admission -- nothing is
+        allocated mid-flight and nothing is preempted.  A prompt whose budget exceeds the pool raises ValueError before
+        any work.  kv_pages sets the pool (default: n times the largest budget);
+      * while any row is prefilling, each step is a mixed step: one token of each decoding row plus up to
+        prefill_chunk_size (default 512) prompt tokens of the admitted prompts, taken in FIFO order, packed without
+        padding (ragged kernels).  Otherwise a step is one replay of the captured decode step;
+      * the host reads the rows' done flags after every step while prompts wait, and every EOS_CHECK_EVERY steps once
+        none waits; a done row's pages go back to the pool and its row to the next prompt.
+    Each prompt's tokens are those of generate([p], prefill_chunk_size=C) run alone with its own settings (an int seed
+    gives prompt i the seed seed + i), up to the arithmetic of other GEMM token counts.  prompt_lookup_num_tokens,
+    share_prompt_prefixes and num_return_sequences > 1 do not combine with max_batch_size (sharing pages between live
+    requests would need refcounted pages)."""
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
     n_ret = num_return_sequences
     if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
@@ -1305,14 +1645,25 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     if share and prefill_chunk_size is None:
         prefill_chunk_size = 512
     prompts = [torch.as_tensor(p).reshape(-1) for p in prompts for _ in range(n_ret)]
-    max_new_tokens = int(max_new_tokens)
     if not prompts:
         raise ValueError('no prompts')
-    if max_new_tokens < 1:
+    budgets = _per_prompt('max_new_tokens', max_new_tokens, len(prompts))
+    if any(isinstance(m, bool) or int(m) < 1 for m in budgets):
         raise ValueError(f'max_new_tokens must be at least 1, got {max_new_tokens}')
+    budgets = [int(m) for m in budgets]
+    max_new_tokens = max(budgets)
     lens = [p.numel() for p in prompts]
     if min(lens) == 0:
         raise ValueError('empty prompt')
+    if max_batch_size is not None:
+        if isinstance(max_batch_size, bool) or int(max_batch_size) != max_batch_size or max_batch_size < 1:
+            raise ValueError(f'max_batch_size must be an integer >= 1, got {max_batch_size!r}')
+        for name, on in (('prompt_lookup_num_tokens', prompt_lookup_num_tokens is not None),
+                         ('share_prompt_prefixes', bool(share_prompt_prefixes)), ('num_return_sequences', n_ret > 1)):
+            if on:
+                raise ValueError(f'{name} does not combine with max_batch_size (continuous batching)')
+    elif kv_pages is not None:
+        raise ValueError('kv_pages sizes the page pool of continuous batching: it needs max_batch_size')
     spec = prompt_lookup_num_tokens is not None
     k = 0
     if spec:
@@ -1321,9 +1672,11 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError(f'prompt_lookup_num_tokens must be an integer in [1, 7], got {prompt_lookup_num_tokens}')
         if n_max != max_matching_ngram_size or n_max < 1:
             raise ValueError(f'max_matching_ngram_size must be an integer >= 1, got {max_matching_ngram_size}')
-    max_len = max(lens) + max_new_tokens + k if max_len is None else int(max_len)
-    if max(lens) + max_new_tokens + k > max_len:
-        raise ValueError(f'a prompt of {max(lens)} tokens plus {max_new_tokens} new ones' +
+    # a fixed batch steps every row max(budgets) times; continuous batching steps each row to its own budget
+    n, m = (max(zip(lens, budgets), key=sum) if max_batch_size is not None else (max(lens), max_new_tokens))
+    max_len = n + m + k if max_len is None else int(max_len)
+    if n + m + k > max_len:
+        raise ValueError(f'a prompt of {n} tokens plus {m} new ones' +
                          (f' and {k} drafts' if k else '') + f' exceeds max_len {max_len}')
     cfg = model.config
     if cfg.model_type == 'opt' and max_len > cfg.max_position_embeddings:
@@ -1336,9 +1689,17 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                 raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
     else:
         settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
+    if max_batch_size is not None:
+        rows = min(int(max_batch_size), len(prompts))
+        need = max(-(-(n + m) // KV_PAGE) for n, m in zip(lens, budgets))
+        kv_pages = rows * need if kv_pages is None else kv_pages
+        if isinstance(kv_pages, bool) or int(kv_pages) != kv_pages or kv_pages < 1:
+            raise ValueError(f'kv_pages must be an integer >= 1, got {kv_pages!r}')
+        return _generate_continuous(model, prompts, budgets, eos, kv_dtype, settings if do_sample else None, rows,
+                                    int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len)
     pages, starts = {}, None
     if share:
-        table, n_pages, starts = plan_prefix_pages(prompts, [n + max_new_tokens + k for n in lens],
+        table, n_pages, starts = plan_prefix_pages(prompts, [n + m + k for n, m in zip(lens, budgets)],
                                                    max_pages=-(-max_len // KV_PAGE))
         pages = dict(page_table=table, n_pages=n_pages)
     if spec:
@@ -1354,23 +1715,29 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
     if spec:
-        return _generate_spec(dec, max_new_tokens, eos_t, spec_stats)
+        return _generate_spec(dec, budgets, eos_t, spec_stats)
     n = 1
     while n < max_new_tokens:
-        if eos and n % EOS_CHECK_EVERY == 0 and bool(torch.isin(dec.generated[:, :n], eos_t).any(1).all()):
-            break
+        if (eos or min(budgets) < max_new_tokens) and n % EOS_CHECK_EVERY == 0:
+            fin = torch.tensor([m <= n for m in budgets], device=dec.dev)     # a row past its own budget is finished
+            if eos:
+                fin = fin | torch.isin(dec.generated[:, :n], eos_t).any(1)
+            if bool(fin.all()):
+                break
         dec.step()
         n += 1
     out = []
-    for row in dec.generated[:, :n].cpu():
+    for row, m in zip(dec.generated[:, :n].cpu(), budgets):
+        row = row[:m]
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
     return out
 
 
-def _generate_spec(dec, max_new, eos_t, stats):
+def _generate_spec(dec, budgets, eos_t, stats):
     """generate()'s host loop over SpecDecoder steps: it syncs only every EOS_CHECK_EVERY steps, to stop once every row
-    has max_new tokens or an EOS among its tokens."""
+    has max_new tokens or an EOS among its tokens.  Each row is cut to its own budget."""
+    max_new = max(budgets)
     steps = 0
     cols = torch.arange(dec.generated.shape[1], device=dec.dev)
     while steps < max_new - 1:
@@ -1386,8 +1753,8 @@ def _generate_spec(dec, max_new, eos_t, stats):
         stats['accepted'] = dec.accepted.tolist()
         stats['steps'] = steps
     out = []
-    for row, n in zip(dec.generated.cpu(), dec.n_gen.tolist()):
-        row = row[:n]
+    for row, n, m in zip(dec.generated.cpu(), dec.n_gen.tolist(), budgets):
+        row = row[:min(n, m)]
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
     return out

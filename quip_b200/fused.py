@@ -461,6 +461,122 @@ def prefill_attention(q, k_cache, v_cache, positions, counts, scale, k_scale=Non
     return out
 
 
+class RaggedChunk:
+    """The sequences of a ragged (packed) chunk: seq_start, S + 1 offsets with 0 = seq_start[0] <= ... <= seq_start[S]
+    = N, so sequence s is the packed token rows seq_start[s] .. seq_start[s + 1] - 1 and every row belongs to one
+    sequence.  The offsets are checked on the host when the chunk is made; `seq_start` is their device copy, which every
+    layer's ragged launches read, so a step checks and copies them once."""
+
+    def __init__(self, seq_start, device):
+        offs = seq_start.tolist() if torch.is_tensor(seq_start) else list(seq_start)
+        if len(offs) < 2 or any(int(x) != x for x in offs):
+            raise ValueError(f'seq_start must hold S + 1 >= 2 integer offsets, got {offs}')
+        offs = [int(x) for x in offs]
+        if offs[0] != 0 or any(b < a for a, b in zip(offs, offs[1:])):
+            raise ValueError(f'seq_start must rise monotonically from 0, got {offs}')
+        if len(offs) - 1 > 65535 or offs[-1] > 2 ** 31 - 1:
+            raise ValueError(f'{len(offs) - 1} sequences of {offs[-1]} tokens: at most 65535 sequences and 2^31 - 1 '
+                             'tokens')
+        self.offsets = offs
+        self.S, self.N = len(offs) - 1, offs[-1]
+        self.max_count = max(1, max(b - a for a, b in zip(offs, offs[1:])))
+        self.seq_start = torch.tensor(offs, dtype=torch.int64).to(device)
+
+
+def _check_ragged(fn, k_pool, v_pool, seqs, positions, page_table, k_scale, v_scale):
+    """The checks kv_append_ragged and prefill_attention_ragged share: the chunk, pool and scale dtypes and shapes,
+    positions (S,) int64 and the page table (S, max_pages).  Returns (whether the pools are e4m3, n_pages)."""
+    if not isinstance(seqs, RaggedChunk):
+        raise ValueError(f'{fn}: seqs must be a RaggedChunk (its offsets are checked when it is made)')
+    if page_table is None:
+        raise ValueError(f'{fn}: a ragged chunk is paged only: pass the page_table')
+    fp8 = k_pool.dtype == torch.float8_e4m3fn
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn pools only')
+    if fp8 and (k_scale is None or v_scale is None):
+        raise ValueError(f'{fn}: float8_e4m3fn pools need k_scale and v_scale')
+    cdt = torch.float8_e4m3fn if fp8 else torch.float16
+    if (k_pool.dtype != cdt or v_pool.dtype != cdt or positions.dtype != torch.int64 or
+            (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
+        raise ValueError(f'{fn} takes fp16 or float8_e4m3fn pools (fp32 scales) and int64 positions')
+    if k_pool.dim() != 4:
+        raise ValueError(f'{fn}: the pools must be (n_pages, nkv, {KV_PAGE}, hd), got {tuple(k_pool.shape)}')
+    if tuple(positions.shape) != (seqs.S,):
+        raise ValueError(f'{fn}: positions must be ({seqs.S},) for {seqs.S} sequences, got {tuple(positions.shape)}')
+    rows, slots, _ = _kv_layout(fn, k_pool, seqs.S, page_table)
+    nkv = k_pool.shape[1]
+    if (v_pool.shape != k_pool.shape or
+            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
+        raise ValueError(f'{fn}: shapes pools {tuple(k_pool.shape)} / {tuple(v_pool.shape)}, positions '
+                         f'{tuple(positions.shape)} do not agree with {seqs.S} sequences')
+    if seqs.seq_start.device != k_pool.device:
+        raise ValueError(f'{fn}: the chunk\'s offsets live on {seqs.seq_start.device}, the pools on {k_pool.device}')
+    return fp8, rows
+
+
+def kv_append_ragged(k_new, v_new, k_pool, v_pool, seqs, positions, page_table, k_scale=None, v_scale=None):
+    """quip_kv_append_ragged(_fp8) on torch tensors: packed row seq_start[s] + i of k_new / v_new (N, nkv, hd) fp16 --
+    token i of sequence s (seqs: a RaggedChunk) -- to slot positions[s] + i of row s of page_table (S, max_pages) int32,
+    in one layer's pools (n_pages, nkv, 64, hd): fp16, or float8_e4m3fn with fp32 k_scale / v_scale (n_pages, nkv, 64),
+    quantized on the way.  A sequence whose slots leave the cache, or a slot whose page id lies outside the pool, writes
+    nothing.  CUDA, one device, contiguous; positions (S,) int64.  Everything is checked before the launch, which runs on
+    the current stream."""
+    fp8, n_pages = _check_ragged('kv_append_ragged', k_pool, v_pool, seqs, positions, page_table, k_scale, v_scale)
+    if k_new.dtype != torch.float16 or v_new.dtype != torch.float16:
+        raise ValueError('kv_append_ragged takes fp16 k_new / v_new')
+    nkv, hd = k_pool.shape[1], k_pool.shape[3]
+    if tuple(k_new.shape) != (seqs.N, nkv, hd) or v_new.shape != k_new.shape:
+        raise ValueError(f'kv_append_ragged: k_new {tuple(k_new.shape)} / v_new {tuple(v_new.shape)} must be '
+                         f'(N={seqs.N}, nkv={nkv}, hd={hd})')
+    ts = (k_new, v_new, k_pool, v_pool, positions) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('kv_append_ragged', ts, k_new.device)
+    lib, st = _lib.load(), torch.cuda.current_stream(k_new.device).cuda_stream
+    sizes = (seqs.S, seqs.N, seqs.max_count, nkv, hd)
+    with torch.cuda.device(k_new.device):
+        if fp8:
+            _lib.check(lib.quip_kv_append_ragged_fp8(k_new.data_ptr(), v_new.data_ptr(), k_pool.data_ptr(),
+                                                     v_pool.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+                                                     seqs.seq_start.data_ptr(), positions.data_ptr(), *sizes,
+                                                     *_paged_args(page_table, n_pages), st))
+        else:
+            _lib.check(lib.quip_kv_append_ragged(k_new.data_ptr(), v_new.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                                 seqs.seq_start.data_ptr(), positions.data_ptr(), *sizes,
+                                                 *_paged_args(page_table, n_pages), st))
+
+
+def prefill_attention_ragged(q, k_pool, v_pool, seqs, positions, page_table, scale, k_scale=None, v_scale=None):
+    """quip_prefill_attention_ragged(_fp8) on torch tensors: packed row seq_start[s] + i of q (N, nh, hd) fp16 -- token
+    i of sequence s (seqs: a RaggedChunk) -- attends causally over slots 0 .. positions[s] + i of row s of page_table
+    (S, max_pages), in one layer's pools that already hold the chunk (kv_append_ragged).  Returns (N, nh, hd) fp16, on
+    the current stream.  Per sequence the result is bit-identical to prefill_attention with page_table, B = S,
+    T = seqs.max_count and counts = the sequence lengths (include/quip_b200.h); a sequence that would read a slot
+    outside the cache or a page outside the pool gets NaN.  Pools, scales and checks as kv_append_ragged."""
+    fp8, n_pages = _check_ragged('prefill_attention_ragged', k_pool, v_pool, seqs, positions, page_table, k_scale,
+                                 v_scale)
+    nkv, hd = k_pool.shape[1], k_pool.shape[3]
+    if q.dtype != torch.float16 or q.dim() != 3 or q.shape[0] != seqs.N or q.shape[2] != hd:
+        raise ValueError(f'prefill_attention_ragged: q must be (N={seqs.N}, nh, hd={hd}) fp16, got {tuple(q.shape)} '
+                         f'{q.dtype}')
+    nh = q.shape[1]
+    ts = (q, k_pool, v_pool, positions) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('prefill_attention_ragged', ts, q.device)
+    out = torch.empty_like(q)
+    lib, st = _lib.load(), torch.cuda.current_stream(q.device).cuda_stream
+    sizes = (seqs.S, seqs.N, seqs.max_count, nh, nkv, hd, C.c_float(scale))
+    with torch.cuda.device(q.device):
+        if fp8:
+            _lib.check(lib.quip_prefill_attention_ragged_fp8(q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                                             k_scale.data_ptr(), v_scale.data_ptr(),
+                                                             seqs.seq_start.data_ptr(), positions.data_ptr(),
+                                                             out.data_ptr(), *sizes, *_paged_args(page_table, n_pages),
+                                                             st))
+        else:
+            _lib.check(lib.quip_prefill_attention_ragged(q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                                         seqs.seq_start.data_ptr(), positions.data_ptr(), out.data_ptr(),
+                                                         *sizes, *_paged_args(page_table, n_pages), st))
+    return out
+
+
 def sample_at(logits, temperature, top_k, top_p, seed, steps, out):
     """quip_sample_at: logits (B, T, V) fp16 -> out (B, T) int64, token i of row b by the rule of quip_sample with row b's
     settings and seed at step steps[b] + i (steps (B,) int64).  CUDA, one device, contiguous; on the current stream."""

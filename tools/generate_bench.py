@@ -45,6 +45,15 @@ Section score (llama7b) measures continuation scoring: quip_token_logprobs alone
 choices), the reference harness's recipe against decode.score unshared, shared and shared with an e4m3 cache:
 requests/s, prefilled tokens, peak allocation and the largest per-request difference against the recipe.
 
+Section continuous (llama7b) measures continuous batching (generate(..., max_batch_size=32), ContinuousDecoder): 256
+requests with prompt lengths uniform in [32, 1536] and budgets uniform in [16, 512] from a fixed seed, fp16 cache, greedy,
+no EOS.  The static arm runs consecutive groups of 32 through generate() (prefill_chunk_size=512, per-prompt budgets);
+the continuous arm runs generate()'s continuous loop (32 rows, chunks of 512 prompt tokens), instrumented with CUDA
+events per step.  Reported: output tokens/s end to end, the GEMM tokens each arm's prefill feeds (padded rows included,
+counted from shapes), mean and p99 time between a request's tokens, the time in graph steps and in mixed steps, the host
+time per mixed step, and how many requests' tokens agree exactly.  Also ragged against padded chunked prefill alone on
+8 prompts of 64 .. 2048 tokens.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -668,6 +677,136 @@ def paged_generate(model, prompts, n_new, share, chunk=512, sample=False):
     return r, gen
 
 
+def continuous_workload(V, n=256, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    lens = torch.randint(32, 1537, (n,), generator=g).tolist()
+    budgets = torch.randint(16, 513, (n,), generator=g).tolist()
+    return [torch.randint(0, V, (k,), generator=g) for k in lens], budgets
+
+
+def continuous_static(model, prompts, budgets, rows, chunk):
+    """Consecutive groups of `rows` prompts through generate(): seconds, outputs and the GEMM tokens of the chunked
+    prefill (each chunk runs rows x its width)."""
+    import time
+    from quip_b200.decode import generate
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    outs, gemm = [], 0
+    for s in range(0, len(prompts), rows):
+        ps = prompts[s:s + rows]
+        outs += generate(model, ps, budgets[s:s + rows], prefill_chunk_size=chunk)
+        P = max(p.numel() for p in ps)
+        gemm += sum(len(ps) * min(chunk, P - c0) for c0 in range(0, P, chunk))
+    torch.cuda.synchronize()
+    return time.perf_counter() - t0, outs, gemm
+
+
+def continuous_serve(model, prompts, budgets, rows, chunk):
+    """generate()'s continuous loop (decode._generate_continuous), with a CUDA event after every step: seconds, outputs,
+    per-step (kind, device ms, host ms, prompt tokens, decode tokens) and each request's token times."""
+    import time
+    from quip_b200.decode import EOS_CHECK_EVERY, KV_PAGE, ContinuousDecoder, ContinuousSchedule
+    lens = [p.numel() for p in prompts]
+    need = max(-(-(n + m) // KV_PAGE) for n, m in zip(lens, budgets))
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    sched = ContinuousSchedule(lens, budgets, rows, rows * need, chunk)
+    dec = ContinuousDecoder(model, max(n + m for n, m in zip(lens, budgets)), rows, rows * need, max(budgets))
+    dec.capture()
+    out = [None] * len(prompts)
+    steps, log = 0, []
+    start = torch.cuda.Event(enable_timing=True)
+    start.record()
+    with torch.no_grad():
+        while True:
+            if sched.queue or steps % EOS_CHECK_EVERY == 0:
+                done = dec.done.cpu()
+                for r, i in enumerate(sched.req):
+                    if i is not None and done[r]:
+                        out[sched.retire(r)] = dec.generated[r, :int(dec.n_gen[r])].cpu()
+                        dec.retire(r)
+                for r, i, pages in sched.admit():
+                    dec.admit(r, pages, budgets[i])
+            if sched.finished:
+                break
+            decoding, pieces = sched.plan()
+            holders = list(sched.req)
+            h0 = time.perf_counter()
+            if pieces:
+                ends = [r for r, lo, n in pieces if lo + n == lens[sched.req[r]]]
+                dec.mixed_step(decoding, [(r, prompts[sched.req[r]][lo:lo + n], lo, r in ends) for r, lo, n in pieces])
+                made = [holders[r] for r in list(decoding) + ends]
+            else:
+                dec.decode_step()
+                made = [i for i in holders if i is not None]
+            host_ms = 1e3 * (time.perf_counter() - h0)
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            log.append(('mixed' if pieces else 'graph', ev, host_ms, sum(n for _, _, n in pieces), len(decoding), made))
+            steps += 1
+    torch.cuda.synchronize()
+    secs = time.perf_counter() - t0
+    times, prev = {i: [] for i in range(len(prompts))}, 0.0
+    split = dict(graph=[0.0, 0], mixed=[0.0, 0])
+    for kind, ev, host_ms, pt, dt, made in log:
+        t = start.elapsed_time(ev)
+        split[kind][0] += t - prev
+        split[kind][1] += 1
+        prev = t
+        for i in made:
+            if len(times[i]) < out[i].numel():               # a request's first n tokens come from its first n steps
+                times[i].append(t)
+    del dec
+    torch.cuda.empty_cache()
+    return secs, out, log, times, split
+
+
+def ragged_vs_padded_prefill(model, V, chunk=512, reps=3, seed=1):
+    """8 prompts of 64 .. 2048 tokens prefilled in chunks of `chunk`: the paged PromptDecoder (every row through every
+    chunk, padding included) against ContinuousDecoder mixed steps (packed prompt tokens only), ms each (median)."""
+    from quip_b200.decode import KV_PAGE, ContinuousDecoder, ContinuousSchedule, PromptDecoder
+    g = torch.Generator().manual_seed(seed)
+    lens = [64, 128, 256, 512, 768, 1024, 1536, 2048]
+    prompts = [torch.randint(0, V, (n,), generator=g) for n in lens]
+    max_len = max(lens) + 1
+    mp = -(-max_len // KV_PAGE)
+    table = torch.arange(len(lens) * mp, dtype=torch.int32).view(len(lens), mp)
+    pad = PromptDecoder(model, max_len=max_len, batch=len(lens), n_pages=len(lens) * mp, page_table=table)
+    rag = ContinuousDecoder(model, max_len, len(lens), len(lens) * mp, 1)
+
+    def padded():
+        pad.prefill(prompts, chunk=chunk)
+
+    def ragged():
+        s = ContinuousSchedule(lens, [1] * len(lens), len(lens), len(lens) * mp, chunk)
+        for r, i, pages in s.admit():
+            rag.admit(r, pages, 1)
+        while s.filling:
+            _, pieces = s.plan()
+            rag.mixed_step([], [(r, prompts[s.req[r]][lo:lo + n], lo, lo + n == lens[s.req[r]]) for r, lo, n in pieces])
+        for r in range(len(lens)):
+            rag.retire(r)
+    res = {}
+    with torch.no_grad():
+        for name, fn in (('padded', padded), ('ragged', ragged)) * 2:           # the first round warms up
+            ts = []
+            for _ in range(reps):
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fn()
+                e1.record()
+                torch.cuda.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            res[name] = sorted(ts)[len(ts) // 2]
+    P = max(lens)
+    res.update(lens=lens, padded_gemm_tokens=sum(len(lens) * min(chunk, P - c0) for c0 in range(0, P, chunk)),
+               ragged_gemm_tokens=sum(lens))
+    del pad, rag
+    torch.cuda.empty_cache()
+    return res
+
+
 def score_kernel_alone(R, V, reps):
     """quip_token_logprobs on fp16 logits (R, V): logits bytes read per second against 3.35 TB/s, next to torch's
     log_softmax(x.float()).gather plus argmax on the same tensor."""
@@ -784,7 +923,7 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
-    #                                                                         score
+    #                                                                         score, continuous
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
@@ -873,7 +1012,7 @@ def main():
                           f'{r["greedy_equal"]}', flush=True)
                     torch.cuda.empty_cache()
         if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
-                sections & {'chunked', 'paged', 'score'} and name == 'llama7b'):
+                sections & {'chunked', 'paged', 'score', 'continuous'} and name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         if 'score' in sections and name == 'llama7b':
@@ -919,6 +1058,39 @@ def main():
                       f'-> {s_["cache_bytes"] / 2**30:.2f} GiB, step {u["decode_ms_per_step"]:.2f} -> '
                       f'{s_["decode_ms_per_step"]:.2f} ms, {u["tokens_per_s"]:.0f} -> {s_["tokens_per_s"]:.0f} tok/s, '
                       f'same tokens {same:.3f}', flush=True)
+        if 'continuous' in sections and name == 'llama7b':
+            import numpy as np
+            r = ragged_vs_padded_prefill(model, cfg.vocab_size)
+            print(f'{name} prefill of 8 prompts 64..2048 in chunks of 512: padded {r["padded"]:.0f} ms '
+                  f'({r["padded_gemm_tokens"]} GEMM tokens), ragged {r["ragged"]:.0f} ms ({r["ragged_gemm_tokens"]})',
+                  flush=True)
+            prompts, budgets = continuous_workload(cfg.vocab_size)
+            s_secs, s_out, s_gemm = continuous_static(model, prompts, budgets, 32, 512)
+            c_secs, c_out, log, times, split = continuous_serve(model, prompts, budgets, 32, 512)
+            gaps = np.concatenate([np.diff(t) for t in times.values() if len(t) > 1])
+            n_out = sum(budgets)
+            mixed_host = [h for kind, _, h, *_ in log if kind == 'mixed']
+            same = sum(torch.equal(a_, b_) for a_, b_ in zip(s_out, c_out))
+            agree = [int((a_ != b_).nonzero()[0]) if not torch.equal(a_, b_) else a_.numel()
+                     for a_, b_ in zip(s_out, c_out)]
+            rec['continuous'] = dict(
+                prefill_alone=r, requests=len(prompts), output_tokens=n_out,
+                static=dict(seconds=s_secs, tokens_per_s=n_out / s_secs, prefill_gemm_tokens=s_gemm),
+                continuous=dict(seconds=c_secs, tokens_per_s=n_out / c_secs,
+                                prefill_gemm_tokens=sum(pt + dt for kind, _, _, pt, dt, _ in log if kind == 'mixed'),
+                                prompt_tokens=sum(p.numel() for p in prompts),
+                                token_gap_ms_mean=float(gaps.mean()), token_gap_ms_p99=float(np.percentile(gaps, 99)),
+                                graph_ms=split['graph'][0], graph_steps=split['graph'][1], mixed_ms=split['mixed'][0],
+                                mixed_steps=split['mixed'][1], mixed_host_ms_mean=float(np.mean(mixed_host))),
+                same_requests=same, mean_agreeing_prefix=float(np.mean(agree)))
+            c = rec['continuous']['continuous']
+            print(f'{name} continuous 256 requests: static {n_out / s_secs:.0f} tok/s ({s_secs:.1f} s, prefill GEMM '
+                  f'tokens {s_gemm}), continuous {c["tokens_per_s"]:.0f} tok/s ({c_secs:.1f} s, mixed-step GEMM tokens '
+                  f'{c["prefill_gemm_tokens"]} of which {c["prompt_tokens"]} prompt); token gap mean '
+                  f'{c["token_gap_ms_mean"]:.1f} ms p99 {c["token_gap_ms_p99"]:.1f} ms; graph {c["graph_ms"] / 1e3:.1f} s '
+                  f'({c["graph_steps"]} steps), mixed {c["mixed_ms"] / 1e3:.1f} s ({c["mixed_steps"]} steps, host '
+                  f'{c["mixed_host_ms_mean"]:.1f} ms each); identical requests {same} / {len(prompts)}, mean agreeing '
+                  f'prefix {np.mean(agree):.1f} tokens', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
