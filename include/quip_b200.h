@@ -365,6 +365,60 @@ int quip_sample_at(const void* logits, const float* temperature, const int32_t* 
 int quip_token_logprobs(const void* logits, int64_t ld, const int64_t* targets, float* logprob, uint8_t* is_greedy,
                         int32_t R, int32_t V, void* stream);
 
+/* Beam search (HF's GenerationMixin._beam_search, prompt by prompt).  B prompts of K beams each are the rows
+ * r = b * K + j (2 <= K <= 16 in generate).  C = max(2, 1 + n_eos) * K <= 64 candidates per prompt.
+ *
+ * quip_beam_candidates: for each row r of fp16 logits (R, V), row stride ld (rows need only 2-byte alignment), with
+ * j = r % K and score = scores[r] (fp32, device):
+ *   s_v = ((x_v - m) - log(sum exp(x - m))) + score, m = max x, in fp32 (expf / logf; the per-thread sums are combined
+ *         in a fixed order, so launches are bit-identical).  A NaN anywhere in the row makes every s NaN; a row whose
+ *         maximum is -inf gives s = -inf throughout;
+ *   rank: s descending, then the lower flat index j * V + v.  NaN ranks below every number (-inf included), -0 == +0;
+ *   cand_s[r, :], cand_i[r, :] (fp32, int32) = the first min(C, V) entries in rank order as (s, j * V + v); when
+ *   V < C the rest are (NaN, -1), ranked after every entry.  The K lists of a prompt hold its top C over all K * V.
+ *
+ * quip_beam_select: one prompt b at step t = *step (device; n = t + 1 tokens after this step) with n_b = budget[b]:
+ *   0. done[b] set: parents[r] = r and adv[r] = 0 for its rows; nothing else is read or written (likewise t outside
+ *      [0, max_new));
+ *   1. merge its K candidate lists into the top C by the rank above (ties across lists: lower flat index, then row);
+ *   2. a candidate hits when its token (index % V) is one of the n_eos <= 3 ids eos[] or n >= n_b;
+ *   3. running beams: the top K of r_i = s_i + (hit ? -1e9 : 0) (ties: lower rank).  Beam k gets parent j_i, token,
+ *      score[b*K+k] = r_i, history hist[b, k, :t] = hist[b, j_i, :t] with hist[b, k, t] = token (gathered from the copy
+ *      hist_tmp); tokens[r] = token (the next input), parents[r] = b * K + j_i, adv[r] = 1;
+ *   4. finished slots (fin_score, fin_len, fin_tok, fin_filled; K per prompt, kept sorted): every candidate i < C is
+ *      offered with v_i = s_i / pen[n] (IEEE division; pen[n] = fp32(n ** length_penalty), n = 0 .. max_new) plus, in
+ *      this order, -1e9 when early_stopping == 1 (True) and every slot is filled, -1e9 when heur[b] is 0, and -1e9
+ *      unless i < K and i hits.  The slots keep the top K of (old slots, offered) by value (ties: the lower merged
+ *      index, old slots first); an offered candidate's slot holds (v_i, n, its history and token, filled = i < K and
+ *      hit);
+ *   5. heur[b] &= any over slots k of best > (filled_k ? min of the slot values : -1e9), best = the top running score
+ *      / pen[never_long ? n_b : n] (never_long: early_stopping 'never' with length_penalty > 0);
+ *   6. done[b] = !heur[b] || (early_stopping == 1 && every slot filled) || every one of the C candidates hits.
+ * early_stopping: 0 False, 1 True, 2 'never'.  Histories are (B, K, max_new) int64, fin_tmp / hist_tmp scratch of
+ * that shape.  One CTA per prompt; everything is read from device memory, so one captured graph serves every step.
+ *
+ * quip_kv_beam_fork(_fp8): after a select, with len = lens[r] (the slots row r has filled, the last at pos = len - 1,
+ * cur = pos / 64) and p = parents[r] != r: table[r, :cur] = the old table[p, :cur] (read from table_tmp, a copy made by
+ * the first phase, so rows may swap); slots 64 * cur .. pos of row p's current page are copied (every layer, k and v,
+ * and on e4m3 pools their scales) into row r's current page, through scratch page scratch0 + r in two phases (gather
+ * every parent, then scatter), so cycles and fan-out are safe.  Pools (L, n_pages, nkv, 64, hd) (scales
+ * (L, n_pages, nkv, 64)), 16-byte aligned, hd * element size % 16 == 0; scratch0 + R <= n_pages.  A page id outside
+ * [0, n_pages) is never dereferenced; rows with p == r or p outside [0, R) change nothing.  Two launches. */
+int quip_beam_candidates(const void* logits, int64_t ld, const float* scores, float* cand_s, int32_t* cand_i,
+                         int32_t R, int32_t V, int32_t K, int32_t C, void* stream);
+int quip_beam_select(const float* cand_s, const int32_t* cand_i, const int64_t* eos, int32_t n_eos,
+                     const int64_t* budget, const int64_t* step, const float* pen, float* score, int64_t* hist,
+                     int64_t* hist_tmp, float* fin_score, int64_t* fin_len, int64_t* fin_tok, int64_t* fin_tmp,
+                     uint8_t* fin_filled, uint8_t* heur, uint8_t* done, int64_t* tokens, int64_t* parents,
+                     int64_t* adv, int32_t B, int32_t K, int32_t C, int32_t V, int32_t max_new,
+                     int32_t early_stopping, int32_t never_long, void* stream);
+int quip_kv_beam_fork(void* k_pool, void* v_pool, int32_t* table, int32_t* table_tmp, const int64_t* parents,
+                      const int64_t* lens, int32_t R, int32_t L, int32_t n_pages, int32_t nkv, int32_t hd,
+                      int32_t max_pages, int32_t scratch0, void* stream);
+int quip_kv_beam_fork_fp8(void* k_pool, void* v_pool, float* k_scale, float* v_scale, int32_t* table,
+                          int32_t* table_tmp, const int64_t* parents, const int64_t* lens, int32_t R, int32_t L,
+                          int32_t n_pages, int32_t nkv, int32_t hd, int32_t max_pages, int32_t scratch0, void* stream);
+
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout
  * (bits 3: int32 (K*3/32, N) as Quant3Linear.pack writes it; bits 4: (K/8, N); bits 2: (K/16, N)):

@@ -1263,6 +1263,275 @@ class ContinuousDecoder(PromptDecoder):
         return torch.cat(out)[None]
 
 
+class BeamDecoder(PromptDecoder):
+    """Paged PromptDecoder whose B * K rows are the K beams of B prompts (generate(..., num_beams=K)): row b * K + j is
+    beam j of prompt b.  One captured step runs the layers and head, then
+      * quip_beam_candidates: the top C = max(2, 1 + n_eos) * K of s = log_softmax(logits) + score per row;
+      * quip_beam_select: per prompt, the top C of its K lists, the next K running beams (parents, tokens, scores and
+        histories), the K finished slots and the early-stop and done flags, by the rule of include/quip_b200.h (HF's
+        _beam_search);
+      * positions advance for the prompts that were live, then quip_kv_beam_fork(_fp8): a beam takes its parent's table
+        entries for every completed 64-slot span (those pages are never written again, so no refcount) and a copy of its
+        parent's slots of the current span into its own current page.
+    The first select runs on the prefill's logits (all K rows of a prompt hold the same ones; beams 1 .. K-1 start at
+    -1e9).  A done prompt's rows keep stepping at a frozen position inside their own pages.  Pages are never reused and
+    nothing is allocated mid-run: the pool is the plan's pages (page_table, n_plan) plus B * K scratch pages for the
+    fork.  On the CPU the same step in torch (_beam_candidates_torch, _beam_select_torch, _beam_fork_torch)."""
+
+    def __init__(self, model, max_len, n_prompts, num_beams, max_new, page_table, n_plan, budgets, eos=(),
+                 length_penalty=1.0, early_stopping=False, kv_dtype=None, ops=None):
+        B, K = int(n_prompts), int(num_beams)
+        super().__init__(model, max_len=max_len, batch=B * K, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
+                         page_table=page_table, n_pages=int(n_plan) + B * K)
+        dev = self.dev
+        self.B, self.K, self.scratch0 = B, K, int(n_plan)
+        self.C = max(2, 1 + len(eos)) * K
+        self.V = model.lm_head.out_features
+        self.early_stopping = early_stopping
+        self.never_long = early_stopping == 'never' and length_penalty > 0
+        self.eos = torch.tensor([int(e) for e in eos], dtype=torch.long, device=dev)
+        self.budget = torch.tensor([int(n) for n in budgets], dtype=torch.long, device=dev)
+        self.pen = torch.tensor([float(n) ** float(length_penalty) if n else 1.0 for n in range(self.max_new + 1)],
+                                dtype=torch.float32, device=dev)
+        z = lambda *shape, dt=torch.long: torch.zeros(shape, dtype=dt, device=dev)
+        self.beam = dict(score=z(B * K, dt=torch.float32), hist=z(B, K, self.max_new), hist_tmp=z(B, K, self.max_new),
+                         fin_score=z(B, K, dt=torch.float32), fin_len=z(B, K), fin_tok=z(B, K, self.max_new),
+                         fin_tmp=z(B, K, self.max_new), fin_filled=z(B, K, dt=torch.uint8), heur=z(B, dt=torch.uint8),
+                         done=z(B, dt=torch.uint8), tokens=self.tokens, parents=z(B * K), adv=z(B * K))
+        self.cand_s = z(B * K, self.C, dt=torch.float32)
+        self.cand_i = z(B * K, self.C, dt=torch.int32)
+        self.table_tmp = torch.full((B * K, self.max_pages), -1, dtype=torch.int32, device=dev)
+        self._init_beams()
+
+    def _init_beams(self):
+        st = self.beam
+        for name in ('hist', 'fin_len', 'fin_tok', 'fin_filled', 'done', 'parents', 'adv'):
+            st[name].zero_()
+        st['score'].fill_(-1e9)
+        st['score'][::self.K] = 0.0
+        st['fin_score'].fill_(-1e9)
+        st['heur'].fill_(1)
+
+    @property
+    def done(self):
+        return self.beam['done']
+
+    def _beam_step(self, logits, advance):
+        st, K = self.beam, self.K
+        if self._kernel:
+            from . import fused
+            fused.beam_candidates(logits, st['score'], K, self.C, self.cand_s, self.cand_i)
+            fused.beam_select(self.cand_s, self.cand_i, self.eos, self.budget, self._t, self.pen, st, K, self.V,
+                              self.early_stopping, self.never_long)
+        else:
+            cs, ci = _beam_candidates_torch(logits, st['score'], K, self.C)
+            self.cand_s.copy_(cs)
+            self.cand_i.copy_(ci)
+            _beam_select_torch(self.cand_s, self.cand_i, self.eos, self.budget, self._t, self.pen, st, K, self.V,
+                               self.early_stopping, self.never_long)
+        if advance:
+            self.positions.add_(st['adv'])
+        kw = dict(k_scale=self.k_scale, v_scale=self.v_scale) if self._fp8 else {}
+        if self._kernel:
+            from . import fused
+            fused.kv_beam_fork(self.k_cache, self.v_cache, self.page_table, self.table_tmp, st['parents'],
+                               self.positions, self.scratch0, **kw)
+        else:
+            _beam_fork_torch(self.k_cache, self.v_cache, self.page_table, st['parents'], self.positions, **kw)
+        self._t.add_(1)
+
+    def _advance(self):
+        self._beam_step(self.logits, advance=True)
+
+    def _first_token(self, logits):
+        self._t.zero_()
+        self._beam_step(logits, advance=False)
+        self._t_host = 1
+
+    def _capture_state(self):
+        return super()._capture_state() + [t for n, t in self.beam.items() if n != 'tokens'] + [self.page_table]
+
+    def reset(self):
+        super().reset()
+        self._init_beams()
+
+    def results(self, n_ret):
+        """The n_ret best finished slots of each prompt, best first: ([new-token tensors in (prompt, rank) order],
+        [their scores]), each cut after its first EOS."""
+        st = self.beam
+        fs, fl, ft = st['fin_score'].cpu(), st['fin_len'].cpu(), st['fin_tok'].cpu()
+        eos = self.eos.cpu()
+        out, scores = [], []
+        for b in range(self.B):
+            for k in range(n_ret):
+                row = ft[b, k, :int(fl[b, k])]
+                hit = torch.isin(row, eos).nonzero()
+                out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+                scores.append(float(fs[b, k]))
+        return out, scores
+
+
+def _beam_generate(model, prompts, budgets, K, eos, kv_dtype, chunk, max_len, length_penalty, early_stopping, n_ret,
+                   stats):
+    """generate()'s beam search: a BeamDecoder over the K copies of each prompt, planned by plan_prefix_pages (a
+    prompt's full pages are prefilled and stored once), replayed until every prompt is done (read every
+    EOS_CHECK_EVERY steps)."""
+    B = len(prompts)
+    V = model.lm_head.out_features
+    if len(eos) > 3:
+        raise ValueError(f'beam search takes at most 3 EOS ids, got {len(eos)}')
+    C = max(2, 1 + len(eos)) * K
+    if K * V < C:
+        raise ValueError(f'{K} beams over a vocabulary of {V} cannot fill {C} candidates')
+    rows = [p for p in prompts for _ in range(K)]
+    table, n_plan, starts = plan_prefix_pages(rows, [rows[r].numel() + budgets[r // K] for r in range(B * K)],
+                                              max_pages=-(-max_len // KV_PAGE))
+    max_new = max(budgets)
+    dec = BeamDecoder(model, max_len, B, K, max_new, table, n_plan, budgets, eos=eos, length_penalty=length_penalty,
+                      early_stopping=early_stopping, kv_dtype=kv_dtype)
+    if dec.dev.type == 'cuda' and max_new > 1:
+        dec.capture()                                                # before prefill maps the table
+    dec.prefill(rows, chunk=chunk, starts=starts)                    # and the first select, on the prefill's logits
+    steps = 1
+    while steps < max_new:
+        if steps % EOS_CHECK_EVERY == 0 and bool(dec.done.all()):
+            break
+        dec.step()
+        steps += 1
+    out, scores = dec.results(n_ret)
+    if stats is not None:
+        stats['scores'] = scores
+        stats['steps'] = steps
+    return out
+
+
+def _beam_order_key(x):
+    """The order-preserving key of the beam rules (include/quip_b200.h) of fp32 x: int64, larger for larger x, -0 == +0,
+    NaN lowest (0)."""
+    x = torch.where(x == 0, torch.zeros_like(x), x)
+    u = x.contiguous().view(torch.int32).long() & 0xFFFFFFFF
+    k = torch.where(u >= 2 ** 31, ~u & 0xFFFFFFFF, u | 2 ** 31)
+    return torch.where(torch.isnan(x), torch.zeros_like(k), k)
+
+
+def _rank(*keys):
+    """Indices sorted by keys, most significant first, each ascending; ties by position."""
+    order = torch.arange(keys[0].numel())
+    for k in reversed(keys):
+        order = order[torch.argsort(k[order], stable=True)]
+    return order
+
+
+def _beam_candidates_torch(logits, scores, K, C):
+    """The rule of quip_beam_candidates (include/quip_b200.h) in torch: per row, the top min(C, V) of
+    s = log_softmax(fp32 logits) + score by (s descending, NaN last, lower index), as (R, C) fp32 values and int32 flat
+    indices (r % K) * V + v, padded with (NaN, -1) when V < C."""
+    x = logits.detach().float().cpu()
+    R, V = x.shape
+    s = torch.log_softmax(x, -1) + scores.detach().float().cpu()[:, None]
+    s = torch.where((x.amax(-1, keepdim=True) == float('-inf')) & ~torch.isnan(x).any(-1, keepdim=True),
+                    torch.full_like(s, float('-inf')), s)
+    out_s = torch.full((R, C), float('nan'))
+    out_i = torch.full((R, C), -1, dtype=torch.int32)
+    n = min(C, V)
+    for r in range(R):
+        top = _rank(-_beam_order_key(s[r]))[:n]
+        out_s[r, :n] = s[r, top]
+        out_i[r, :n] = (top + (r % K) * V).int()
+    return out_s.to(logits.device), out_i.to(logits.device)
+
+
+def _beam_select_torch(cand_s, cand_i, eos, budget, step, pen, st, K, V, early_stopping, never_long):
+    """The rule of quip_beam_select (include/quip_b200.h) in torch, in place on the state tensors st (fused.beam_select
+    has their names and shapes)."""
+    R, C = cand_s.shape
+    B, t = R // K, int(step.reshape(-1)[0])
+    max_new = st['hist'].shape[-1]
+    NEG = torch.tensor(-1e9, dtype=torch.float32)
+    zero = torch.tensor(0.0, dtype=torch.float32)
+    eos_l = [int(e) for e in eos.tolist()]
+    for b in range(B):
+        rows = slice(b * K, (b + 1) * K)
+        if bool(st['done'][b]) or not 0 <= t < max_new:
+            st['parents'][rows] = torch.arange(b * K, (b + 1) * K)
+            st['adv'][rows] = 0
+            continue
+        n, bud = t + 1, int(budget[b])
+        es_, ei = cand_s[rows].reshape(-1).cpu(), cand_i[rows].reshape(-1).cpu().long()
+        order = _rank(-_beam_order_key(es_), torch.where(ei < 0, 2 ** 40, ei), torch.arange(K * C))[:C]
+        cs, ci = es_[order], ei[order]
+        tok, par = ci % V, ci // V
+        hit = torch.tensor([n >= bud or int(v) in eos_l for v in tok.tolist()])
+        r = cs + torch.where(hit, NEG, zero)
+        run = _rank(-_beam_order_key(r))[:K]
+        old = {k: st[k][b].cpu().clone() for k in ('fin_score', 'fin_len', 'fin_tok', 'fin_filled')}
+        hist_old = st['hist'][b].cpu().clone()
+        full = bool(old['fin_filled'].bool().all()) and early_stopping is True
+        h_ok = bool(st['heur'][b])
+        did = hit & (torch.arange(C) < K)
+        v = cs / pen[n].cpu()
+        v = v + (NEG if full else zero)
+        v = v + (zero if h_ok else NEG)
+        v = v + torch.where(did, zero, NEG)
+        fv = torch.cat([old['fin_score'], v])
+        fsrc = _rank(-_beam_order_key(fv))[:K]
+        new_hist = hist_old.clone()
+        for k, i in enumerate(run.tolist()):
+            new_hist[k, :t] = hist_old[int(par[i]), :t]
+            new_hist[k, t] = tok[i]
+        st['hist'][b] = new_hist.to(st['hist'].device)
+        st['tokens'][rows] = tok[run].to(st['tokens'].device)
+        st['parents'][rows] = (b * K + par[run]).to(st['parents'].device)
+        st['score'][rows] = r[run].to(st['score'].device)
+        st['adv'][rows] = 1
+        fin_tok = torch.zeros_like(old['fin_tok'])
+        fs, fl, ff = torch.empty(K), torch.empty(K, dtype=torch.long), torch.empty(K, dtype=torch.bool)
+        for k, src in enumerate(fsrc.tolist()):
+            fs[k] = fv[src]
+            if src < K:
+                fin_tok[k] = old['fin_tok'][src]
+                fl[k], ff[k] = old['fin_len'][src], bool(old['fin_filled'][src])
+            else:
+                i = src - K
+                fin_tok[k, :t] = hist_old[int(par[i]), :t]
+                fin_tok[k, t] = tok[i]
+                fl[k], ff[k] = n, bool(did[i])
+        for name, val in (('fin_score', fs), ('fin_len', fl), ('fin_tok', fin_tok), ('fin_filled', ff)):
+            st[name][b] = val.to(st[name].dtype).to(st[name].device)
+        mn = fs.min()
+        best = r[run[0]] / pen[min(bud, max_new) if never_long else n].cpu()
+        heur = h_ok and bool((best > torch.where(ff, mn, NEG)).any())
+        st['heur'][b] = int(heur)
+        st['done'][b] = int(not heur or (early_stopping is True and bool(ff.all())) or bool(hit.all()))
+
+
+def _beam_fork_torch(k_pool, v_pool, table, parents, lens, k_scale=None, v_scale=None):
+    """The rule of quip_kv_beam_fork(_fp8) (include/quip_b200.h) in torch, in place: pools (L, n_pages, nkv, 64, hd),
+    scales (L, n_pages, nkv, 64), table (R, max_pages) int32."""
+    R, max_pages = table.shape
+    n_pages = k_pool.shape[1]
+    old = table.clone()
+    moves = []
+    for r in range(R):
+        p, ln = int(parents[r]), int(lens[r])
+        if not 0 <= p < R or p == r or not 1 <= ln <= max_pages * KV_PAGE:
+            continue
+        cur, ns = (ln - 1) // KV_PAGE, (ln - 1) % KV_PAGE + 1
+        src = int(old[p, cur])
+        data = None
+        if 0 <= src < n_pages:
+            data = [None if x is None else x[:, src, :, :ns].clone() for x in (k_pool, v_pool, k_scale, v_scale)]
+        moves.append((r, p, cur, ns, data))
+    for r, p, cur, ns, data in moves:
+        table[r, :cur] = old[p, :cur]
+        dst = int(old[r, cur])
+        if data is None or not 0 <= dst < n_pages:
+            continue
+        for x, d in zip((k_pool, v_pool, k_scale, v_scale), data):
+            if x is not None:
+                x[:, dst, :, :ns] = d
+
+
 class ContinuousSchedule:
     """The host side of continuous batching (generate(..., max_batch_size=rows)): which request holds which decoder row
     and pages, and what each step feeds.  Deterministic, and free of device work so it can be checked on its own.
@@ -1579,7 +1848,8 @@ def _sampling_settings(n, temperature, top_k, top_p, seed):
 def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv_dtype=None, do_sample=False,
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
-             max_batch_size=None, kv_pages=None):
+             max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
+             beam_stats=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -1633,18 +1903,47 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     Each prompt's tokens are those of generate([p], prefill_chunk_size=C) run alone with its own settings (an int seed
     gives prompt i the seed seed + i), up to the arithmetic of other GEMM token counts.  prompt_lookup_num_tokens,
     share_prompt_prefixes and num_return_sequences > 1 do not combine with max_batch_size (sharing pages between live
-    requests would need refcounted pages)."""
+    requests would need refcounted pages).
+
+    num_beams=K (2 .. 16; default 1: the paths above, unchanged) runs beam search (BeamDecoder): for each prompt p the
+    result is what HF's model.generate(p[None], num_beams=K, do_sample=False, max_new_tokens=n_p, length_penalty,
+    early_stopping, num_return_sequences, eos_token_id) returns with the prompt alone -- transformers'
+    GenerationMixin._beam_search, with ties ranked by lower index (include/quip_b200.h has the rule) -- in any batch,
+    up to ties and rounding.  length_penalty (a float): a finished hypothesis of n new tokens scores
+    sum log p / n ** length_penalty.  early_stopping: False (HF's heuristic), True (stop once K hypotheses are finished)
+    or 'never'.  num_return_sequences=r <= K then returns the r best finished hypotheses of each prompt, best first:
+    len(prompts) * r tensors in (prompt, rank) order, each cut after its first EOS.  beam_stats: a dict that receives
+    'scores' (HF's sequences_scores, in the same order) and 'steps'.  At most 3 EOS ids.  The K beams of a prompt share
+    its full prompt pages (prefilled once, prefill_chunk_size default 512) and fork by page-table rows; the page pool is
+    fixed before any work.  do_sample, prompt_lookup_num_tokens, max_batch_size and share_prompt_prefixes do not combine
+    with num_beams > 1."""
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
     n_ret = num_return_sequences
     if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
         raise ValueError(f'num_return_sequences must be an integer >= 1, got {num_return_sequences!r}')
     n_ret = int(n_ret)
-    if n_ret > 1 and not do_sample:
+    if isinstance(num_beams, bool) or int(num_beams) != num_beams or not 1 <= num_beams <= 16:
+        raise ValueError(f'num_beams must be an integer in [1, 16], got {num_beams!r}')
+    nb = int(num_beams)
+    if nb > 1:
+        for name, on in (('do_sample', bool(do_sample)), ('prompt_lookup_num_tokens', prompt_lookup_num_tokens is not None),
+                         ('max_batch_size', max_batch_size is not None), ('kv_pages', kv_pages is not None),
+                         ('share_prompt_prefixes', bool(share_prompt_prefixes))):
+            if on:
+                raise ValueError(f'{name} does not combine with num_beams > 1 (beam search)')
+        if n_ret > nb:
+            raise ValueError(f'num_return_sequences={n_ret} exceeds num_beams={nb}')
+        if isinstance(length_penalty, bool) or not isinstance(length_penalty, (int, float)) or \
+                not math.isfinite(length_penalty):
+            raise ValueError(f'length_penalty must be a finite number, got {length_penalty!r}')
+        if not (early_stopping is True or early_stopping is False or early_stopping == 'never'):
+            raise ValueError(f"early_stopping must be False, True or 'never', got {early_stopping!r}")
+    elif n_ret > 1 and not do_sample:
         raise ValueError(f'num_return_sequences={n_ret} needs do_sample=True (greedy samples would all be the same)')
-    share = bool(share_prompt_prefixes) or n_ret > 1
-    if share and prefill_chunk_size is None:
+    share = bool(share_prompt_prefixes) or (n_ret > 1 and nb == 1)
+    if (share or nb > 1) and prefill_chunk_size is None:
         prefill_chunk_size = 512
-    prompts = [torch.as_tensor(p).reshape(-1) for p in prompts for _ in range(n_ret)]
+    prompts = [torch.as_tensor(p).reshape(-1) for p in prompts for _ in range(n_ret if nb == 1 else 1)]
     if not prompts:
         raise ValueError('no prompts')
     budgets = _per_prompt('max_new_tokens', max_new_tokens, len(prompts))
@@ -1689,6 +1988,9 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                 raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
     else:
         settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
+    if nb > 1:
+        return _beam_generate(model, prompts, budgets, nb, eos, kv_dtype, prefill_chunk_size, max_len,
+                              float(length_penalty), early_stopping, n_ret, beam_stats)
     if max_batch_size is not None:
         rows = min(int(max_batch_size), len(prompts))
         need = max(-(-(n + m) // KV_PAGE) for n, m in zip(lens, budgets))

@@ -753,3 +753,128 @@ def llama_stack(layers, h, kwargs, ops=None, trace=None, fold_gathers=None):
             pend = mlp.down_proj(act)
         rec(li, 'down', pend)
     return h if pend is None else h + pend
+
+
+BEAM_MAX_K, BEAM_MAX_C, BEAM_MAX_EOS = 16, 64, 3
+
+
+def beam_candidates(logits, scores, K, C, cand_s, cand_i):
+    """quip_beam_candidates: for each row r of logits (R, V) fp16 (stride(1) == 1, any stride(0) >= V) with score
+    scores[r] (fp32), the top C of s = log_softmax(row) + score in rank order (s descending, then lower flat index
+    (r % K) * V + v; NaN last) into cand_s (R, C) fp32 and cand_i (R, C) int32 (include/quip_b200.h has the rule; rows
+    with V < C are padded with (NaN, -1)).  CUDA, one device; everything is checked before the launch, which runs on
+    the current stream.  Returns (cand_s, cand_i)."""
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'beam_candidates: logits must be (R, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    R, V = logits.shape
+    if V < 1 or (R > 1 and logits.stride(0) < V) or (V > 1 and logits.stride(1) != 1):
+        raise ValueError(f'beam_candidates: logits rows must be unit-stride and not overlap, got shape '
+                         f'{tuple(logits.shape)} strides {tuple(logits.stride())}')
+    if not (1 <= K <= BEAM_MAX_K and 1 <= C <= BEAM_MAX_C) or V > 2 ** 24 or K * V > 2 ** 31 - 1:
+        raise ValueError(f'beam_candidates: need 1 <= K <= {BEAM_MAX_K}, 1 <= C <= {BEAM_MAX_C}, V <= 2^24, got K {K}, '
+                         f'C {C}, V {V}')
+    for name, t, dt, shape in (('scores', scores, torch.float32, (R,)), ('cand_s', cand_s, torch.float32, (R, C)),
+                               ('cand_i', cand_i, torch.int32, (R, C))):
+        if t.dtype != dt or tuple(t.shape) != shape:
+            raise ValueError(f'beam_candidates: {name} must be {shape} {dt}, got {tuple(t.shape)} {t.dtype}')
+    if not logits.is_cuda:
+        raise RuntimeError('beam_candidates runs on a CUDA device only (there is no CPU fallback)')
+    _check_cuda('beam_candidates', (scores, cand_s, cand_i), logits.device)
+    ld = logits.stride(0) if R > 1 else V
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_beam_candidates(logits.data_ptr(), ld, scores.data_ptr(), cand_s.data_ptr(),
+                                                    cand_i.data_ptr(), R, V, K, C,
+                                                    torch.cuda.current_stream(logits.device).cuda_stream))
+    return cand_s, cand_i
+
+
+ES_MODES = {False: 0, True: 1, 'never': 2}
+
+
+def beam_select(cand_s, cand_i, eos, budget, step, pen, st, K, V, early_stopping, never_long):
+    """quip_beam_select: merge each prompt's K candidate lists (cand_s / cand_i (B * K, C), beam_candidates) and apply
+    HF's running-beam, finished-slot, early-stop and done rules (include/quip_b200.h) at step step (1,) int64, with
+    eos (n_eos <= 3,) int64, budget (B,) int64 and pen (max_new + 1,) fp32 = n ** length_penalty.  st: the state
+    tensors by name -- score (B * K,) fp32; hist, hist_tmp, fin_tok, fin_tmp (B, K, max_new) int64; fin_score (B, K)
+    fp32; fin_len (B, K) int64; fin_filled (B, K), heur (B,), done (B,) uint8; tokens, parents, adv (B * K,) int64 --
+    updated in place.  early_stopping: False, True or 'never'.  CUDA, one device, contiguous; checked before the
+    launch, which runs on the current stream."""
+    if early_stopping not in ES_MODES:
+        raise ValueError(f"beam_select: early_stopping must be False, True or 'never', got {early_stopping!r}")
+    if cand_s.dim() != 2 or cand_s.dtype != torch.float32 or cand_i.dtype != torch.int32 or cand_i.shape != cand_s.shape:
+        raise ValueError(f'beam_select: cand_s (R, C) fp32 and cand_i (R, C) int32, got {tuple(cand_s.shape)} '
+                         f'{cand_s.dtype} / {tuple(cand_i.shape)} {cand_i.dtype}')
+    R, C = cand_s.shape
+    if not (1 <= K <= BEAM_MAX_K and K <= C <= BEAM_MAX_C) or R % K or K * V > 2 ** 31 - 1 or V < 1:
+        raise ValueError(f'beam_select: need 1 <= K <= {BEAM_MAX_K}, K <= C <= {BEAM_MAX_C}, K | R, got R {R}, K {K}, '
+                         f'C {C}, V {V}')
+    B = R // K
+    max_new = st['hist'].shape[-1] if st['hist'].dim() == 3 else -1
+    if max_new < 1 or eos.dim() != 1 or eos.numel() > BEAM_MAX_EOS:
+        raise ValueError(f'beam_select: hist must be (B, K, max_new >= 1) and eos at most {BEAM_MAX_EOS} ids')
+    want = dict(score=((R,), torch.float32), hist=((B, K, max_new), torch.int64),
+                hist_tmp=((B, K, max_new), torch.int64), fin_score=((B, K), torch.float32),
+                fin_len=((B, K), torch.int64), fin_tok=((B, K, max_new), torch.int64),
+                fin_tmp=((B, K, max_new), torch.int64), fin_filled=((B, K), torch.uint8), heur=((B,), torch.uint8),
+                done=((B,), torch.uint8), tokens=((R,), torch.int64), parents=((R,), torch.int64),
+                adv=((R,), torch.int64))
+    args = [('eos', eos, eos.shape, torch.int64), ('budget', budget, (B,), torch.int64),
+            ('step', step, (1,), torch.int64), ('pen', pen, (max_new + 1,), torch.float32)]
+    args += [(n, st[n], shape, dt) for n, (shape, dt) in want.items()]
+    for name, t, shape, dt in args:
+        if t.dtype != dt or tuple(t.shape) != tuple(shape):
+            raise ValueError(f'beam_select: {name} must be {tuple(shape)} {dt}, got {tuple(t.shape)} {t.dtype}')
+    _check_cuda('beam_select', [cand_s, cand_i] + [t for _, t, _, _ in args], cand_s.device)
+    with torch.cuda.device(cand_s.device):
+        _lib.check(_lib.load().quip_beam_select(
+            cand_s.data_ptr(), cand_i.data_ptr(), eos.data_ptr() if eos.numel() else None, eos.numel(),
+            budget.data_ptr(), step.data_ptr(), pen.data_ptr(), *[st[n].data_ptr() for n in want if n != 'adv'],
+            st['adv'].data_ptr(), B, K, C, V, max_new, ES_MODES[early_stopping], int(bool(never_long)),
+            torch.cuda.current_stream(cand_s.device).cuda_stream))
+
+
+def kv_beam_fork(k_pool, v_pool, table, table_tmp, parents, lens, scratch0, k_scale=None, v_scale=None):
+    """quip_kv_beam_fork(_fp8): after a beam select, row r with parents[r] != r takes its parent's table entries for
+    the spans before its current one and a copy of its parent's slots 64 * cur .. lens[r] - 1 of the current span, in
+    every layer of the pools k_pool / v_pool (L, n_pages, nkv, 64, hd) (fp16, or float8_e4m3fn with fp32 k_scale /
+    v_scale (L, n_pages, nkv, 64)), through scratch pages scratch0 .. scratch0 + R - 1 (include/quip_b200.h).  table /
+    table_tmp (R, max_pages) int32, parents / lens (R,) int64.  CUDA, one device, contiguous; checked before the
+    launches (two, on the current stream)."""
+    fp8 = k_pool.dtype == torch.float8_e4m3fn
+    if fp8 != (k_scale is not None) or (k_scale is None) != (v_scale is None):
+        raise ValueError('kv_beam_fork: float8_e4m3fn pools need k_scale and v_scale, fp16 pools take none')
+    if k_pool.dtype not in (torch.float16, torch.float8_e4m3fn) or v_pool.dtype != k_pool.dtype:
+        raise ValueError(f'kv_beam_fork: fp16 or float8_e4m3fn pools, got {k_pool.dtype} / {v_pool.dtype}')
+    if k_pool.dim() != 5 or k_pool.shape[3] != KV_PAGE or v_pool.shape != k_pool.shape:
+        raise ValueError(f'kv_beam_fork: pools must be (L, n_pages, nkv, {KV_PAGE}, hd), got {tuple(k_pool.shape)} / '
+                         f'{tuple(v_pool.shape)}')
+    L, n_pages, nkv, _, hd = k_pool.shape
+    if (hd * k_pool.element_size()) % 16:
+        raise ValueError(f'kv_beam_fork: a head vector must be a multiple of 16 bytes, got hd {hd}')
+    if fp8 and (k_scale.dtype != torch.float32 or tuple(k_scale.shape) != (L, n_pages, nkv, KV_PAGE) or
+                v_scale.shape != k_scale.shape or v_scale.dtype != torch.float32):
+        raise ValueError(f'kv_beam_fork: scales must be {(L, n_pages, nkv, KV_PAGE)} fp32')
+    if table.dtype != torch.int32 or table.dim() != 2 or table_tmp.shape != table.shape or table_tmp.dtype != torch.int32:
+        raise ValueError(f'kv_beam_fork: table and table_tmp must be (R, max_pages) int32, got {tuple(table.shape)} / '
+                         f'{tuple(table_tmp.shape)}')
+    R, max_pages = table.shape
+    if max_pages < 1 or max_pages > (2 ** 31 - 1) // KV_PAGE:
+        raise ValueError(f'kv_beam_fork: {max_pages} pages per row')
+    _check_i64('kv_beam_fork', parents=(parents, (R,)), lens=(lens, (R,)))
+    if isinstance(scratch0, bool) or int(scratch0) != scratch0 or not 0 <= scratch0 <= n_pages - R:
+        raise ValueError(f'kv_beam_fork: scratch pages {scratch0} .. {scratch0} + {R} - 1 lie outside the pool of '
+                         f'{n_pages}')
+    ts = (k_pool, v_pool, table, table_tmp, parents, lens) + ((k_scale, v_scale) if fp8 else ())
+    _check_cuda('kv_beam_fork', ts, k_pool.device)
+    if k_pool.data_ptr() % 16 or v_pool.data_ptr() % 16:
+        raise ValueError('kv_beam_fork: the pools must be 16-byte aligned')
+    lib, stream = _lib.load(), torch.cuda.current_stream(k_pool.device).cuda_stream
+    sizes = (R, L, n_pages, nkv, hd, max_pages, int(scratch0), stream)
+    with torch.cuda.device(k_pool.device):
+        if fp8:
+            _lib.check(lib.quip_kv_beam_fork_fp8(k_pool.data_ptr(), v_pool.data_ptr(), k_scale.data_ptr(),
+                                                 v_scale.data_ptr(), table.data_ptr(), table_tmp.data_ptr(),
+                                                 parents.data_ptr(), lens.data_ptr(), *sizes))
+        else:
+            _lib.check(lib.quip_kv_beam_fork(k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr(),
+                                             table_tmp.data_ptr(), parents.data_ptr(), lens.data_ptr(), *sizes))

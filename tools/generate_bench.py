@@ -915,6 +915,60 @@ def score_arms(model, docs, batch_size, chunk):
     return out
 
 
+def beam_arms(model, cfg, B, K, fp8, P=512, n_new=128, steps=32, reps=50, seed=0):
+    """Beam search on the synthetic model: B prompts of P tokens, K beams, no EOS.  The captured beam step (layers, head,
+    candidates, select, fork) against a plain PromptDecoder step at B * K rows over the same prompts, then each beam
+    kernel alone on the run's buffers (CUDA events): candidates over the step's logits, select at mid-run, and the fork
+    with every row taking another row of its prompt as parent at a full current span (the most it copies)."""
+    from quip_b200 import fused
+    from quip_b200.decode import KV_PAGE, BeamDecoder, PromptDecoder, plan_prefix_pages
+    kv = torch.float8_e4m3fn if fp8 else None
+    g = torch.Generator().manual_seed(seed)
+    prompts = [torch.randint(0, cfg.vocab_size, (P,), generator=g) for _ in range(B)]
+    rows = [p for p in prompts for _ in range(K)]
+    max_len = P + n_new
+    table, n_plan, starts = plan_prefix_pages(rows, [max_len] * (B * K), max_pages=-(-max_len // KV_PAGE))
+    bound = B * ((P - 1) // KV_PAGE + K * (-(-max_len // KV_PAGE) - (P - 1) // KV_PAGE)) + B * K
+    dec = BeamDecoder(model, max_len, B, K, n_new, table, n_plan, [n_new] * B, kv_dtype=kv).capture()
+    dec.prefill(rows, chunk=512, starts=starts)
+    for _ in range(4):
+        dec.step()
+    torch.cuda.synchronize()
+    beam_ms = events_ms(dec.graph.replay, steps, warm=0)
+    base = PromptDecoder(model, max_len=max_len, batch=B * K, max_new=n_new, kv_dtype=kv).capture()
+    base.prefill(rows, chunk=512)
+    for _ in range(4):
+        base.step()
+    plain_ms = events_ms(base.graph.replay, steps, warm=0)
+    del base
+    torch.cuda.empty_cache()
+    st, R, V = dec.beam, B * K, dec.V
+    logits = dec.logits
+    cand_ms = events_ms(lambda: fused.beam_candidates(logits, st['score'], K, dec.C, dec.cand_s, dec.cand_i), reps)
+    st['done'].zero_()
+    st['heur'].fill_(1)
+    t_mid = torch.tensor([n_new // 2], device=logits.device)
+    sel_ms = events_ms(lambda: fused.beam_select(dec.cand_s, dec.cand_i, dec.eos, dec.budget, t_mid, dec.pen, st, K, V,
+                                                 False, False), reps)
+    parents = torch.tensor([(r // K) * K + (r % K + 1) % K for r in range(R)], device=logits.device)
+    lens = torch.full((R,), (P // KV_PAGE + 1) * KV_PAGE, dtype=torch.long, device=logits.device)   # 64 slots to copy
+    kw = dict(k_scale=dec.k_scale, v_scale=dec.v_scale) if fp8 else {}
+    fork_ms = events_ms(lambda: fused.kv_beam_fork(dec.k_cache, dec.v_cache, dec.page_table, dec.table_tmp, parents,
+                                                   lens, dec.scratch0, **kw), reps)
+    L, _, nkv, _, hd = dec.k_cache.shape
+    forked = R if K > 1 else 0                          # K = 1: every parent is the row itself, nothing moves
+    moved = forked * 2 * L * nkv * KV_PAGE * (hd * dec.k_cache.element_size() + (4 if fp8 else 0))
+    r = dict(B=B, K=K, kv='e4m3' if fp8 else 'fp16', beam_step_ms=beam_ms, plain_step_ms=plain_ms,
+             candidates_ms=cand_ms, select_ms=sel_ms, fork_ms=fork_ms,
+             kernels_share_of_step=(cand_ms + sel_ms + fork_ms) / beam_ms,
+             candidates_bytes_per_s=2 * V * R / (cand_ms * 1e-3),
+             fork_copied_bytes=moved, fork_copied_bytes_per_s=moved / (fork_ms * 1e-3) if moved else 0.0,
+             pool_pages=dec.n_pages, pool_bound=bound)
+    del dec
+    torch.cuda.empty_cache()
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -923,7 +977,7 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
-    #                                                                         score, continuous
+    #                                                                         score, continuous, beam
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
@@ -1012,7 +1066,7 @@ def main():
                           f'{r["greedy_equal"]}', flush=True)
                     torch.cuda.empty_cache()
         if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
-                sections & {'chunked', 'paged', 'score', 'continuous'} and name == 'llama7b'):
+                sections & {'chunked', 'paged', 'score', 'continuous', 'beam'} and name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         if 'score' in sections and name == 'llama7b':
@@ -1091,6 +1145,19 @@ def main():
                   f'({c["graph_steps"]} steps), mixed {c["mixed_ms"] / 1e3:.1f} s ({c["mixed_steps"]} steps, host '
                   f'{c["mixed_host_ms_mean"]:.1f} ms each); identical requests {same} / {len(prompts)}, mean agreeing '
                   f'prefix {np.mean(agree):.1f} tokens', flush=True)
+        if 'beam' in sections and name == 'llama7b':
+            rec['beam'] = []
+            for fp8 in (False, True):
+                for B in (1, 8):
+                    for K in (1, 2, 4, 8):
+                        r = beam_arms(model, cfg, B, K, fp8)
+                        rec['beam'].append(r)
+                        print(f'{name} beam {r["kv"]} B={B} K={K}: step {r["beam_step_ms"]:.3f} ms (plain '
+                              f'{r["plain_step_ms"]:.3f} ms at {B * K} rows); candidates {1e3 * r["candidates_ms"]:.1f} us '
+                              f'({r["candidates_bytes_per_s"] / 1e12:.2f} TB/s), select {1e3 * r["select_ms"]:.1f} us, '
+                              f'fork {1e3 * r["fork_ms"]:.1f} us ({r["fork_copied_bytes_per_s"] / 1e12:.2f} TB/s copied); '
+                              f'kernels {100 * r["kernels_share_of_step"]:.1f}% of the step; pool {r["pool_pages"]} pages '
+                              f'(bound {r["pool_bound"]})', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
