@@ -365,6 +365,35 @@ int quip_sample_at(const void* logits, const float* temperature, const int32_t* 
 int quip_token_logprobs(const void* logits, int64_t ld, const int64_t* targets, float* logprob, uint8_t* is_greedy,
                         int32_t R, int32_t V, void* stream);
 
+/* Logits processors of generation (HF's RepetitionPenalty, NoRepeatNGram, NoBadWords and MinNewTokensLength, in that
+ * order), in place on fp16 logits (R, V) with row stride ld (elements; rows need only 2-byte alignment).  Logits row r
+ * is offset i = r % T of decoder row b = rows[r / T] (rows (R / T) int64; null: b = r / T); T = 1 except in speculative
+ * steps.  Its history h is hist[b, 0 .. c] (hist (B, max_len) int64, c = last[b]) followed by the drafts
+ * tokens[b, 1 .. i] (tokens (B, T) int64; may be null when T = 1); L = c + 1 + i, n_new = L - prompt_len[b].  Per decoder
+ * row (device): penalty rho (fp32), ngram size n (int32, 0 = off), min_new m (int32).  For the call: eos (n_eos int64)
+ * and the bad-word sequences bad (n_bad, 16) int64 with lengths bad_len (n_bad) int32.
+ *   1. repetition penalty (rho != 1): for each distinct v of h, x_v <- x_v < 0 ? x_v * rho : x_v / rho in fp32 (IEEE),
+ *      rounded once to fp16 (NaN stays NaN, -0 -> -0 / rho);
+ *   2. no-repeat n-gram (n >= 1): for every 0 <= e <= L - n with h[e .. e+n-2] == h[L-n+1 .. L-1], x_{h[e+n-1]} <- -inf
+ *      (n = 1 bans every token of h);
+ *   3. bad words: the sequences of length 1 equal to an eos id are dropped.  A sequence w of length l bans w[l-1] when
+ *      l == 1, or l <= L and the last l - 1 tokens of h equal w[0 .. l-2].  HF adds a bias row b (-inf at banned
+ *      tokens, +0 elsewhere), so with n_bad > 0 a banned x becomes x + (-inf) (NaN for +inf and NaN) and every -0 of the
+ *      row becomes +0;
+ *   4. min_new_tokens: if n_new < m, every eos id gets -inf.
+ * Steps 2 and 4 assign -inf and step 3 adds it, so a token banned by 2 or 4 ends at -inf whatever 3 does.  A token id
+ * outside [0, V) (in h, eos or bad) is never dereferenced; a row with b outside [0, B) or c outside [0, max_len) is not
+ * touched, nor is a row with rho == 1, n == 0, no eos ban due and n_bad == 0 (bit for bit).  Only the penalised and
+ * banned entries (and, with bad words, the -0 entries) are written.  The launch depends on (R, T, V, B, max_len, n_eos,
+ * n_bad) only, so one captured graph serves any settings written between replays.  One CTA per row; no workspace.
+ * Bounds: 1 <= V <= 2^18, 0 <= n_eos <= 8, 0 <= n_bad <= 256, 1 <= bad_len <= 16 (a longer or empty sequence is
+ * ignored), R % T == 0; hist, last, tokens, prompt_len, eos and bad 8-byte aligned. */
+int quip_logits_process(void* logits, int64_t ld, int32_t R, int32_t T, int32_t V, const int64_t* rows,
+                        const int64_t* hist, const int64_t* last, const int64_t* tokens, const int64_t* prompt_len,
+                        const float* penalty, const int32_t* ngram, const int32_t* min_new, const int64_t* eos,
+                        int32_t n_eos, const int64_t* bad, const int32_t* bad_len, int32_t n_bad, int32_t B,
+                        int32_t max_len, void* stream);
+
 /* Beam search (HF's GenerationMixin._beam_search, prompt by prompt).  B prompts of K beams each are the rows
  * r = b * K + j (2 <= K <= 16 in generate).  C = max(2, 1 + n_eos) * K <= 64 candidates per prompt.
  *

@@ -34,6 +34,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .fused import PROC_BAD_LEN, PROC_MAX_BAD, PROC_MAX_EOS
+
 KV_PAGE = 64                                           # slots per page of a paged KV cache (include/quip_b200.h)
 
 
@@ -419,6 +421,11 @@ class PromptDecoder(GraphDecoder):
       * sampling=True: the selection is quip_sample (csrc/sample.cu) over the device buffers temperature, top_k, top_p
         and seed (B each, filled by set_sampling) at step t = _t, the index of the token in generated; a row's token
         depends on its logits, settings, seed and t only.  On the CPU the same rule in torch (_sample_torch);
+      * processing=True: between the head and the selection, quip_logits_process (csrc/logits_process.cu; the rule is
+        in include/quip_b200.h) applies the repetition penalty, no-repeat n-gram, bad-word and min_new_tokens
+        processors in place, from device buffers filled by set_processing, over the row's history `hist` (B, max_len):
+        the prompt by position (written by prefill) and each selected token (written inside the step).  On the CPU the
+        same rule in torch (_process_torch).  Needs max_new >= 1;
       * kv_dtype=torch.float8_e4m3fn: k_cache / v_cache e4m3 with k_scale / v_scale (L, B, nkv, max_len) fp32, one scale
         per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
         (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
@@ -434,7 +441,7 @@ class PromptDecoder(GraphDecoder):
     The whole model, no layer pipeline."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False,
-                 page_table=None, n_pages=None):
+                 page_table=None, n_pages=None, processing=False):
         if n_pages is None and page_table is not None:
             raise ValueError('a page_table needs n_pages, the size of the page pool')
         self.n_pages = None if n_pages is None else int(n_pages)
@@ -463,6 +470,73 @@ class PromptDecoder(GraphDecoder):
             self.top_k = torch.zeros(B, dtype=torch.int32, device=self.dev)
             self.top_p = torch.ones(B, dtype=torch.float32, device=self.dev)
             self.seed = torch.zeros(B, dtype=torch.int64, device=self.dev)
+        self.processing = bool(processing)
+        if self.processing:
+            if self.max_new < 1:
+                raise ValueError('processing=True acts between the head and the selection: max_new must be at least 1')
+            z = lambda *shape, dt=torch.long: torch.zeros(shape, dtype=dt, device=self.dev)
+            self.hist, self.prompt_len = z(B, self.max_len), z(B)
+            self.penalty = torch.ones(B, dtype=torch.float32, device=self.dev)
+            self.ngram, self.min_new = z(B, dt=torch.int32), z(B, dt=torch.int32)
+            self.proc_eos, self.bad, self.bad_len = z(0), z(0, PROC_BAD_LEN), z(0, dt=torch.int32)
+
+    def set_processing(self, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
+                       eos=()):
+        """Write the logits-processor settings into the device buffers a captured step reads: repetition_penalty,
+        no_repeat_ngram_size and min_new_tokens each a scalar for every row or one value per row; bad_words_ids (a list
+        of non-empty id lists) and eos (ids) for the whole batch.  Once a step is captured, the number of bad words and
+        of eos ids is fixed."""
+        if not self.processing:
+            raise ValueError('set_processing needs a PromptDecoder made with processing=True')
+        B, V = self.batch, self.model.lm_head.out_features
+        pen, ngram, min_new, bad, eos = _processing_settings(B, V, repetition_penalty, no_repeat_ngram_size,
+                                                             min_new_tokens, bad_words_ids, eos)
+        if self.graph is not None and (len(bad) != self.bad.shape[0] or len(eos) != self.proc_eos.numel()):
+            raise ValueError(f'the captured step processes {self.bad.shape[0]} bad words and {self.proc_eos.numel()} '
+                             f'eos ids; got {len(bad)} and {len(eos)}')
+        self.penalty.copy_(torch.tensor(pen, dtype=torch.float32))
+        self.ngram.copy_(torch.tensor(ngram, dtype=torch.int32))
+        self.min_new.copy_(torch.tensor(min_new, dtype=torch.int32))
+        if self.graph is None:
+            self.proc_eos = torch.tensor(eos, dtype=torch.long, device=self.dev)
+            self.bad = torch.zeros(len(bad), PROC_BAD_LEN, dtype=torch.long, device=self.dev)
+            self.bad_len = torch.zeros(len(bad), dtype=torch.int32, device=self.dev)
+        self.proc_eos.copy_(torch.tensor(eos, dtype=torch.long))
+        pad = torch.zeros(len(bad), PROC_BAD_LEN, dtype=torch.long)
+        for j, w in enumerate(bad):
+            pad[j, :len(w)] = torch.tensor(w, dtype=torch.long)
+        self.bad.copy_(pad)
+        self.bad_len.copy_(torch.tensor([len(w) for w in bad], dtype=torch.int32))
+
+    def _process(self, logits, last, rows=None, tokens=None):
+        """The processors in place on logits (R, vocab) or (B, T, vocab), each logits row's history ending at
+        hist[b, last[b]] (then, with T > 1, the drafts tokens[b, 1 ..]); rows: the decoder row of each logits row."""
+        x = logits.reshape(-1, logits.shape[-1])
+        T = 1 if tokens is None else tokens.shape[1]
+        args = (x, T, self.hist, last, self.prompt_len, self.penalty, self.ngram, self.min_new, self.proc_eos, self.bad,
+                self.bad_len)
+        if self._kernel:
+            from . import fused
+            fused.logits_process(*args, tokens=tokens, rows=rows)
+        else:
+            _process_torch(*args, tokens=tokens, rows=rows)
+
+    def _hist_append(self, rows, tok, live=None):
+        """hist[rows, positions[rows]] = tok (where live), at positions below max_len."""
+        pos = self.positions[rows]
+        ok = pos < self.max_len if live is None else live & (pos < self.max_len)
+        col = pos.clamp(max=self.max_len - 1)
+        self.hist[rows, col] = torch.where(ok, tok, self.hist[rows, col])
+
+    def _prompt_history(self, ids, lens_t):
+        """A decoder that keeps a history (processing, SpecDecoder): the prompts ids (B, P) into hist[b, :len_b]; with
+        processing, their lengths into prompt_len."""
+        if getattr(self, 'hist', None) is not None:
+            P = ids.shape[1]
+            keep = torch.arange(P, device=self.dev)[None] < lens_t[:, None]
+            self.hist[:, :P] = torch.where(keep, ids, self.hist[:, :P])
+        if self.processing:
+            self.prompt_len.copy_(lens_t)
 
     def _checked_page_map(self, page_table):
         """page_table as the host int32 (batch, max_pages) map prefill installs, after checking its shape and ids."""
@@ -658,10 +732,14 @@ class PromptDecoder(GraphDecoder):
         return o.transpose(1, 2).reshape(B, T, nh * hd)
 
     def _advance(self):
+        if self.processing:
+            self._process(self.logits, self.positions)                 # the token just fed is hist[b, positions[b]]
         self.positions.add_(1)
         if self.max_new:
             self._select(self.logits)
             self.generated.index_copy_(1, self._t, self.tokens[:, None])
+            if self.processing:
+                self._hist_append(self._rows, self.tokens)
             self._t.add_(1)
 
     def _capture_state(self):
@@ -670,7 +748,7 @@ class PromptDecoder(GraphDecoder):
         # decoder is captured before prefill maps its table (generate does so): the warm-up steps then run against an
         # unmapped table and write nothing -- with a page shared by several rows, a warm-up write to slot 0 would
         # corrupt another row's prefix.
-        return [self.positions, self.tokens, self._t, self.generated]
+        return [self.positions, self.tokens, self._t, self.generated] + ([self.hist] if self.processing else [])
 
     def _counters_in_range(self):
         self.positions.clamp_(max=self.max_len - 1)
@@ -689,6 +767,9 @@ class PromptDecoder(GraphDecoder):
         self._t_host = 0
         if self.paged:
             self.page_table.fill_(-1)
+        if self.processing:
+            self.hist.zero_()
+            self.prompt_len.zero_()
 
     def _pad_past_end(self):
         return self.paged and self._chunk is not None
@@ -770,6 +851,7 @@ class PromptDecoder(GraphDecoder):
                 logits = self._prefill_chunks(ids, lens, chunk, starts)
             self.positions.copy_(lens_t)
             self._pos_host = list(lens)
+            self._prompt_history(ids, lens_t)
             if self.max_new:
                 self._first_token(logits)
         return logits
@@ -890,10 +972,15 @@ class PromptDecoder(GraphDecoder):
         return logprob, greedy.bool()
 
     def _first_token(self, logits):
-        """Select the first generated token from the prefill's logits (B, vocab), at t = 0."""
+        """Select the first generated token from the prefill's logits (B, vocab), at t = 0 (processed with the prompt
+        as the history)."""
         self._t.zero_()
+        if self.processing:
+            self._process(logits, self.positions - 1)
         self._select(logits)
         self.generated[:, 0].copy_(self.tokens)
+        if self.processing:
+            self._hist_append(self._rows, self.tokens)
         self._t.fill_(1)
         self._t_host = 1
 
@@ -948,7 +1035,7 @@ class SpecDecoder(PromptDecoder):
     prompt + max_new + draft_tokens (a finished row's step still writes its T slots)."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=1, draft_tokens=4, max_ngram=3, ops=None, kv_dtype=None,
-                 sampling=False, page_table=None, n_pages=None):
+                 sampling=False, page_table=None, n_pages=None, processing=False):
         k, n_max = int(draft_tokens), int(max_ngram)
         if not 1 <= k <= 7:
             raise ValueError(f'draft_tokens must lie in [1, 7], got {draft_tokens}')
@@ -959,7 +1046,7 @@ class SpecDecoder(PromptDecoder):
         if int(max_len) < k + 2:
             raise ValueError(f'max_len {max_len} leaves no room for a step of {k + 1} tokens')
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
-                         sampling=sampling, page_table=page_table, n_pages=n_pages)
+                         sampling=sampling, page_table=page_table, n_pages=n_pages, processing=processing)
         B, dev = self.batch, self.dev
         self.k, self.n_min, self.n_max = k, 1, n_max
         self.T = k + 1
@@ -985,6 +1072,8 @@ class SpecDecoder(PromptDecoder):
 
     def _advance(self):
         logits = self.logits                                                            # (B, T, vocab)
+        if self.processing:                  # row i's history: hist[b, :positions[b] + 1], then drafts 1 .. i
+            self._process(logits, self.positions, tokens=self.tokens)
         if not self.sampling:
             self.targets.copy_(logits.argmax(-1))
         elif self._kernel:
@@ -1022,15 +1111,14 @@ class SpecDecoder(PromptDecoder):
             raise ValueError(f'a prompt of {max(lens)} tokens, {self.max_new} new ones and {self.k} drafts exceed the '
                              f'cache of {self.max_len} positions')
         logits = super().prefill(prompts, chunk=chunk, starts=starts)
-        with torch.no_grad():
-            for b, p in enumerate(prompts):
-                self.hist[b, :lens[b]] = torch.as_tensor(p).reshape(-1).to(self.dev)
         self.accepted.zero_()
         self._steps_host = 0
         return logits
 
     def _first_token(self, logits):
         self._t.zero_()
+        if self.processing:
+            self._process(logits, self.positions - 1)
         self._select(logits, out=self._first)
         self.generated[:, 0].copy_(self._first)
         self.hist[self._rows, self.positions] = self._first
@@ -1086,10 +1174,11 @@ class ContinuousDecoder(PromptDecoder):
     until the host retires it.  On the CPU both steps run eagerly, the ragged attention in torch (per-sequence scatter
     through the table, SDPA under each sequence's causal mask)."""
 
-    def __init__(self, model, max_len, batch, n_pages, max_new, ops=None, kv_dtype=None, sampling=False, eos=()):
+    def __init__(self, model, max_len, batch, n_pages, max_new, ops=None, kv_dtype=None, sampling=False, eos=(),
+                 processing=False):
         max_pages = -(-int(max_len) // KV_PAGE)
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
-                         sampling=sampling, n_pages=n_pages,
+                         sampling=sampling, n_pages=n_pages, processing=processing,
                          page_table=torch.full((int(batch), max_pages), -1, dtype=torch.int32))
         B, dev = self.batch, self.dev
         self.n_gen = torch.zeros(B, dtype=torch.long, device=dev)
@@ -1101,9 +1190,10 @@ class ContinuousDecoder(PromptDecoder):
 
     # ---- per-row requests
 
-    def admit(self, row, pages, budget, settings=None):
-        """Give row `row` a new request: its pages (host ids, mapped from slot 0 on), its budget of new tokens and, when
-        sampling, its (temperature, top_k, top_p, seed).  Its prompt is then fed by mixed steps."""
+    def admit(self, row, pages, budget, settings=None, prompt=None, proc=None):
+        """Give row `row` a new request: its pages (host ids, mapped from slot 0 on), its budget of new tokens, when
+        sampling its (temperature, top_k, top_p, seed) and, with processing, its prompt (the start of its history) and
+        (repetition_penalty, no_repeat_ngram_size, min_new_tokens).  Its prompt is then fed by mixed steps."""
         tbl = torch.full((self.max_pages,), -1, dtype=torch.int32)
         tbl[:len(pages)] = torch.tensor(pages, dtype=torch.int32)
         self.page_table[row].copy_(tbl)
@@ -1118,6 +1208,11 @@ class ContinuousDecoder(PromptDecoder):
             self.top_k[row] = int(k)
             self.top_p[row] = float(p)
             self.seed[row] = s - 2 ** 64 if s >= 2 ** 63 else s
+        if self.processing:
+            prompt = torch.as_tensor(prompt).reshape(-1)
+            self.hist[row, :prompt.numel()] = prompt.to(self.dev)
+            self.prompt_len[row] = prompt.numel()
+            self.penalty[row], self.ngram[row], self.min_new[row] = float(proc[0]), int(proc[1]), int(proc[2])
 
     def retire(self, row):
         """Unmap row `row`'s pages and make it idle."""
@@ -1146,10 +1241,14 @@ class ContinuousDecoder(PromptDecoder):
         n = n + live.long()
         self.n_gen[rows] = n
         self.positions[rows] = self.positions[rows] + live.long()
+        if self.processing:
+            self._hist_append(rows, tok, live)
         stop = (tok[:, None] == self.eos[None]).any(1) | (n >= self.budget[rows])
         self.done[rows] = self.done[rows] | (live & stop)
 
     def _advance(self):
+        if self.processing:
+            self._process(self.logits, self.positions)
         self._commit(self._rows, self._choose(self.logits, self._rows))
 
     def _capture_state(self):
@@ -1207,6 +1306,8 @@ class ContinuousDecoder(PromptDecoder):
                 last = [int(pieces[j][2]) + int(pieces[j][1].numel()) - 1 for j in ends]
                 self.positions[out_t[nd:]] = torch.tensor(last, dtype=torch.long).to(dev)
             logits = self._head(h[0, idx][:, None], None if pend is None else pend[0, idx][:, None])
+            if self.processing:
+                self._process(logits, self.positions, rows=out_t)
             self._commit(out_t, self._choose(logits, out_t))
         return logits
 
@@ -1601,12 +1702,16 @@ class ContinuousSchedule:
         return not self.queue and all(i is None for i in self.req)
 
 
-def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len):
-    """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages."""
+def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len,
+                         proc=None):
+    """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages;
+    proc: the per-prompt (penalties, ngram sizes, min_new_tokens) and the bad words of the logits processors, or None."""
     lens = [p.numel() for p in prompts]
     sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk)
     dec = ContinuousDecoder(model, max_len, rows, kv_pages, max(max_new), kv_dtype=kv_dtype,
-                            sampling=settings is not None, eos=eos)
+                            sampling=settings is not None, eos=eos, processing=proc is not None)
+    if proc is not None:
+        dec.set_processing(bad_words_ids=proc[3] or None, eos=eos)
     if dec.dev.type == 'cuda':
         dec.capture()                                # before any row is mapped: the warm-up steps write nothing
     out = [None] * len(prompts)
@@ -1626,7 +1731,8 @@ def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows,
                     out[sched.retire(r)] = row[:int(hit[0]) + 1] if hit.numel() else row
                     dec.retire(r)
             for r, i, pages in sched.admit():
-                dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings])
+                dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings],
+                          prompts[i], None if proc is None else [s[i] for s in proc[:3]])
         if sched.finished:
             break
         decoding, pieces = sched.plan()
@@ -1690,6 +1796,77 @@ def _sample_torch_at(logits, temperature, top_k, top_p, seed, steps):
             out[b, i] = _sample_torch(logits[b, i][None], temperature[b:b + 1], top_k[b:b + 1], top_p[b:b + 1],
                                       seed[b:b + 1], int(steps[b]) + i)[0]
     return out.to(logits.device)
+
+def _process_torch(logits, T, hist, last, prompt_len, penalty, ngram, min_new, eos, bad, bad_len, tokens=None,
+                   rows=None):
+    """The rule of quip_logits_process (include/quip_b200.h) in torch, in place on logits (R, V) (fp32 on the CPU,
+    fp16 on the GPU: the penalty in fp32, rounded once), one row at a time; arguments as fused.logits_process."""
+    R, V = logits.shape
+    B, max_len = hist.shape
+    eos_l = [int(e) for e in eos.tolist()]
+    bad_l = [w[:n] for w, n in zip(bad.tolist(), bad_len.tolist()) if 1 <= n <= PROC_BAD_LEN]
+    bad_l = [w for w in bad_l if not (len(w) == 1 and w[0] in eos_l)]
+    rows_l = None if rows is None else rows.tolist()
+    hist_c, last_l, plen = hist.cpu(), last.tolist(), prompt_len.tolist()
+    drafts = None if tokens is None else tokens.cpu()
+    pen, ngs, mns = penalty.to(logits.device), ngram.tolist(), min_new.tolist()
+    neg = torch.tensor(float('-inf'), dtype=torch.float32, device=logits.device)
+    for r in range(R):
+        b = r // T if rows_l is None else rows_l[r // T]
+        if not 0 <= b < B or not 0 <= last_l[b] < max_len:
+            continue
+        i = r % T
+        h = hist_c[b, :last_l[b] + 1].tolist() + ([] if i == 0 else drafts[b, 1:i + 1].tolist())
+        L, n, x = len(h), ngs[b], logits[r]
+        if float(penalty[b]) != 1.0:
+            ids = torch.tensor(sorted({v for v in h if 0 <= v < V}), dtype=torch.long, device=logits.device)
+            xs = x[ids].float()
+            x[ids] = torch.where(xs < 0, xs * pen[b], xs / pen[b]).to(x.dtype)
+        hard = set()
+        if 1 <= n <= L:
+            hard.update(h[e + n - 1] for e in range(L - n + 1) if h[e:e + n - 1] == h[L - n + 1:])
+        biased = {w[-1] for w in bad_l if len(w) == 1 or (len(w) <= L and h[L - len(w) + 1:] == w[:-1])}
+        if eos_l and L - plen[b] < mns[b]:
+            hard.update(eos_l)
+        if bad.shape[0]:                              # x + bias row: -inf at the banned tokens, +0 elsewhere
+            x[x == 0] = 0
+            ids = torch.tensor(sorted(v for v in biased if 0 <= v < V), dtype=torch.long, device=logits.device)
+            x[ids] = (x[ids].float() + neg).to(x.dtype)
+        ids = torch.tensor(sorted(v for v in hard if 0 <= v < V), dtype=torch.long, device=logits.device)
+        x[ids] = float('-inf')
+    return logits
+
+
+def _processing_settings(n, V, repetition_penalty, no_repeat_ngram_size, min_new_tokens, bad_words_ids, eos):
+    """Validated per-row (penalties, ngram sizes, min_new_tokens) for n rows and the call's (bad words, eos ids):
+    raises ValueError on any malformed or out-of-bound value."""
+    pen = [float(p) for p in _per_prompt('repetition_penalty', repetition_penalty, n)]
+    if any(not (math.isfinite(p) and p > 0) for p in pen):
+        raise ValueError(f'repetition_penalty must be finite and > 0, got {repetition_penalty}')
+    out = [pen]
+    for name, v in (('no_repeat_ngram_size', no_repeat_ngram_size), ('min_new_tokens', min_new_tokens)):
+        vals = _per_prompt(name, v, n)
+        if any(isinstance(x, bool) or int(x) != x or not 0 <= x < 2 ** 31 for x in vals):
+            raise ValueError(f'{name} must be an integer >= 0, got {v}')
+        out.append([int(x) for x in vals])
+    bad = []
+    if bad_words_ids is not None:
+        if not isinstance(bad_words_ids, (list, tuple)) or not bad_words_ids:
+            raise ValueError(f'bad_words_ids must be a non-empty list of id lists, got {bad_words_ids!r}')
+        for w in bad_words_ids:
+            w = w.tolist() if torch.is_tensor(w) else w
+            if not isinstance(w, (list, tuple)) or not 1 <= len(w) <= PROC_BAD_LEN:
+                raise ValueError(f'each bad word must be a list of 1 .. {PROC_BAD_LEN} ids, got {w!r}')
+            if any(isinstance(x, bool) or int(x) != x or not 0 <= x < V for x in w):
+                raise ValueError(f'bad word ids must be integers in [0, {V}), got {w!r}')
+            bad.append([int(x) for x in w])
+        if len(bad) > PROC_MAX_BAD:
+            raise ValueError(f'at most {PROC_MAX_BAD} bad words, got {len(bad)}')
+    eos = [int(e) for e in eos]
+    if len(eos) > PROC_MAX_EOS:
+        raise ValueError(f'the logits processors take at most {PROC_MAX_EOS} eos ids, got {len(eos)}')
+    return out[0], out[1], out[2], bad, eos
+
 
 def _token_logprobs_torch(logits, targets):
     """The rule of quip_token_logprobs (include/quip_b200.h) in torch, for the CPU path: (fp32 log_softmax gathered at
@@ -1849,7 +2026,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
              max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
-             beam_stats=None):
+             beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -1916,7 +2093,19 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     'scores' (HF's sequences_scores, in the same order) and 'steps'.  At most 3 EOS ids.  The K beams of a prompt share
     its full prompt pages (prefilled once, prefill_chunk_size default 512) and fork by page-table rows; the page pool is
     fixed before any work.  do_sample, prompt_lookup_num_tokens, max_batch_size and share_prompt_prefixes do not combine
-    with num_beams > 1."""
+    with num_beams > 1.
+
+    Logits processors (HF's, applied in HF's order between the head and the selection by quip_logits_process inside
+    the captured step; the rule is in include/quip_b200.h): repetition_penalty (finite, > 0; 1: off), no_repeat_ngram_size
+    (0: off) and min_new_tokens (0: off; needs eos_token_id), each a scalar or one value per prompt (per output row with
+    num_return_sequences, as the sampling settings), and bad_words_ids, one non-empty list of at most 256 id lists of 1 ..
+    16 ids in [0, vocab).  For each prompt p the result is what HF's model.generate(p[None], ...the same settings...,
+    eos_token_id=...) returns with the prompt alone, in any batch; it may differ by ties and by the single fp16 rounding
+    of a penalised logit on the GPU (HF processes fp32).  A sampled row is what quip_sample picks from the processed row.
+    They combine with greedy and sampled decoding, num_return_sequences, share_prompt_prefixes, prefill_chunk_size,
+    kv_dtype, prompt_lookup_num_tokens (the tokens stay those of plain generation) and max_batch_size; with at most 8 EOS
+    ids.  Any setting other than the default with num_beams > 1 raises ValueError (HF processes the beams' log-softmax,
+    which quip_beam_candidates computes itself).  With every default, nothing of this runs."""
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
     n_ret = num_return_sequences
     if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
@@ -1988,6 +2177,18 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                 raise ValueError(f'{name}={v} is a sampling setting: pass do_sample=True (greedy decoding ignores it)')
     else:
         settings = _sampling_settings(len(prompts), temperature, top_k, top_p, seed)
+    pen, ngram, min_new, bad, _ = _processing_settings(len(prompts), model.lm_head.out_features, repetition_penalty,
+                                                       no_repeat_ngram_size, min_new_tokens, bad_words_ids, ())
+    proc = (pen, ngram, min_new, bad) if (any(p != 1.0 for p in pen) or any(ngram) or any(min_new) or
+                                          bad_words_ids is not None) else None
+    if proc is not None:
+        if nb > 1:
+            raise ValueError('repetition_penalty, no_repeat_ngram_size, min_new_tokens and bad_words_ids do not combine '
+                             'with num_beams > 1 (beam search)')
+        if any(min_new) and not eos:
+            raise ValueError('min_new_tokens bans the EOS ids: it needs eos_token_id')
+        if len(eos) > PROC_MAX_EOS:
+            raise ValueError(f'the logits processors take at most {PROC_MAX_EOS} eos ids, got {len(eos)}')
     if nb > 1:
         return _beam_generate(model, prompts, budgets, nb, eos, kv_dtype, prefill_chunk_size, max_len,
                               float(length_penalty), early_stopping, n_ret, beam_stats)
@@ -1998,12 +2199,15 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         if isinstance(kv_pages, bool) or int(kv_pages) != kv_pages or kv_pages < 1:
             raise ValueError(f'kv_pages must be an integer >= 1, got {kv_pages!r}')
         return _generate_continuous(model, prompts, budgets, eos, kv_dtype, settings if do_sample else None, rows,
-                                    int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len)
+                                    int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len,
+                                    proc)
     pages, starts = {}, None
     if share:
         table, n_pages, starts = plan_prefix_pages(prompts, [n + m + k for n, m in zip(lens, budgets)],
                                                    max_pages=-(-max_len // KV_PAGE))
         pages = dict(page_table=table, n_pages=n_pages)
+    if proc is not None:
+        pages['processing'] = True
     if spec:
         dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
                           max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
@@ -2012,6 +2216,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
                             sampling=bool(do_sample), **pages)
     if do_sample:
         dec.set_sampling(*settings)
+    if proc is not None:
+        dec.set_processing(*proc[:3], proc[3] or None, eos)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()                                                # before prefill maps a paged table
     dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)

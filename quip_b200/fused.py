@@ -878,3 +878,60 @@ def kv_beam_fork(k_pool, v_pool, table, table_tmp, parents, lens, scratch0, k_sc
         else:
             _lib.check(lib.quip_kv_beam_fork(k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr(),
                                              table_tmp.data_ptr(), parents.data_ptr(), lens.data_ptr(), *sizes))
+
+
+PROC_MAX_V, PROC_MAX_EOS, PROC_MAX_BAD, PROC_BAD_LEN = 2 ** 18, 8, 256, 16
+
+
+def logits_process(logits, T, hist, last, prompt_len, penalty, ngram, min_new, eos, bad, bad_len, tokens=None,
+                   rows=None):
+    """quip_logits_process: the repetition penalty, no-repeat n-gram, bad-word and min_new_tokens rule of
+    include/quip_b200.h, in place on logits (R, V) fp16 (stride(1) == 1, any stride(0) >= V).  Row r is offset r % T of
+    decoder row rows[r // T] (rows (R // T,) int64; default r // T), whose history is hist[b, :last[b] + 1] (hist
+    (B, max_len) int64, last (B,) int64) and the drafts tokens[b, 1 .. r % T] (tokens (B, T) int64, needed when T > 1).
+    prompt_len (B,) int64, penalty (B,) fp32, ngram and min_new (B,) int32; eos (n_eos <= 8,) int64; bad (n_bad <= 256,
+    16) int64 with bad_len (n_bad,) int32 in [1, 16].  CUDA, one device; everything is checked before the launch, which
+    runs on the current stream.  Returns logits."""
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'logits_process: logits must be (R, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    R, V = logits.shape
+    if not 1 <= V <= PROC_MAX_V or (R > 1 and logits.stride(0) < V) or (V > 1 and logits.stride(1) != 1):
+        raise ValueError(f'logits_process: logits rows must be unit-stride, not overlap and hold 1 .. {PROC_MAX_V} '
+                         f'values, got shape {tuple(logits.shape)} strides {tuple(logits.stride())}')
+    if isinstance(T, bool) or int(T) != T or T < 1 or R % T:
+        raise ValueError(f'logits_process: T must be an integer >= 1 dividing R = {R}, got {T!r}')
+    if hist.dim() != 2:
+        raise ValueError(f'logits_process: hist must be (B, max_len), got {tuple(hist.shape)}')
+    B, max_len = hist.shape
+    n_eos, n_bad = eos.numel(), bad.shape[0] if bad.dim() == 2 else -1
+    if not 0 <= n_eos <= PROC_MAX_EOS or not 0 <= n_bad <= PROC_MAX_BAD:
+        raise ValueError(f'logits_process: at most {PROC_MAX_EOS} eos ids and {PROC_MAX_BAD} bad words, got {n_eos} '
+                         f'and {n_bad}')
+    if T > 1 and tokens is None:
+        raise ValueError('logits_process: T > 1 needs the drafts (tokens)')
+    if rows is None and R // T != B:
+        raise ValueError(f'logits_process: {R // T} logits rows of T = {T} for {B} history rows: pass rows')
+    checks = [('hist', hist, torch.int64, (B, max_len)), ('last', last, torch.int64, (B,)),
+              ('prompt_len', prompt_len, torch.int64, (B,)), ('penalty', penalty, torch.float32, (B,)),
+              ('ngram', ngram, torch.int32, (B,)), ('min_new', min_new, torch.int32, (B,)),
+              ('eos', eos, torch.int64, (n_eos,)), ('bad', bad, torch.int64, (n_bad, PROC_BAD_LEN)),
+              ('bad_len', bad_len, torch.int32, (n_bad,))]
+    if tokens is not None:
+        checks.append(('tokens', tokens, torch.int64, (B, T)))
+    if rows is not None:
+        checks.append(('rows', rows, torch.int64, (R // T,)))
+    for name, t, dt, shape in checks:
+        if t.dtype != dt or tuple(t.shape) != shape:
+            raise ValueError(f'logits_process: {name} must be {shape} {dt}, got {tuple(t.shape)} {t.dtype}')
+    if not logits.is_cuda:
+        raise RuntimeError('logits_process runs on a CUDA device only (there is no CPU fallback)')
+    _check_cuda('logits_process', [t for _, t, _, _ in checks], logits.device)
+    ld = logits.stride(0) if R > 1 else V
+    p = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_logits_process(logits.data_ptr(), ld, R, int(T), V, p(rows), hist.data_ptr(),
+                                                   last.data_ptr(), p(tokens), prompt_len.data_ptr(),
+                                                   penalty.data_ptr(), ngram.data_ptr(), min_new.data_ptr(), p(eos),
+                                                   n_eos, p(bad), p(bad_len), n_bad, B, max_len,
+                                                   torch.cuda.current_stream(logits.device).cuda_stream))
+    return logits

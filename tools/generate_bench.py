@@ -54,6 +54,11 @@ counted from shapes), mean and p99 time between a request's tokens, the time in 
 time per mixed step, and how many requests' tokens agree exactly.  Also ragged against padded chunked prefill alone on
 8 prompts of 64 .. 2048 tokens.
 
+Section logits (llama7b) measures the logits processors (quip_logits_process, csrc/logits_process.cu): the kernel alone
+at B in {1, 32, 128}, V in {32000, 128256} and histories of 512 and 4096 tokens with every processor on (n-gram size 3,
+16 bad words), and the captured PromptDecoder step with and without processors at B in {1, 32}, 512-token prompts and
+128 new tokens, alternated over three trials.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -969,6 +974,65 @@ def beam_arms(model, cfg, B, K, fp8, P=512, n_new=128, steps=32, reps=50, seed=0
     return r
 
 
+def logits_kernel_alone(B, V, hist_len, reps, n=3, n_bad=16, seed=0):
+    """quip_logits_process alone on B fp16 rows of V logits: every processor on (penalty 1.2, n-gram size n, n_bad
+    bad words of 1 .. 4 ids, min_new_tokens due with one EOS id), histories of hist_len ids drawn from 64 tokens so that
+    n-grams repeat.  Timed as 20 launches captured in one CUDA graph (CUDA events around the replays).  Bytes: each
+    row's history (int64) and one pass over its logits (the -0 pass of the bad words)."""
+    from quip_b200 import fused
+    dev = torch.device('cuda:0')
+    g = torch.Generator().manual_seed(seed)
+    x = (torch.randn(B, V, generator=g) * 3).half().to(dev)
+    hist = torch.randint(0, 64, (B, hist_len), generator=g).to(dev)
+    last = torch.full((B,), hist_len - 1, dtype=torch.long, device=dev)
+    bad = torch.zeros(n_bad, 16, dtype=torch.long)
+    bad_len = torch.tensor([1 + j % 4 for j in range(n_bad)], dtype=torch.int32)
+    for j in range(n_bad):
+        bad[j, :int(bad_len[j])] = torch.randint(0, 64, (int(bad_len[j]),), generator=g)
+    args = (x, 1, hist, last, last - 8, torch.full((B,), 1.2, device=dev), torch.full((B,), n, dtype=torch.int32,
+            device=dev), torch.full((B,), 16, dtype=torch.int32, device=dev), torch.tensor([2], device=dev),
+            bad.to(dev), bad_len.to(dev))
+    fused.logits_process(*args)
+    graph, per = torch.cuda.CUDAGraph(), 20               # in a graph, as in a decode step: no host time between launches
+    with torch.cuda.graph(graph):
+        for _ in range(per):
+            fused.logits_process(*args)
+    ms = events_ms(graph.replay, max(reps // per, 5)) / per
+    read = B * (hist_len * 8 + V * 2)
+    return dict(B=B, V=V, hist_len=hist_len, n=n, bad_words=n_bad, kernel_ms=ms, bytes_per_s=read / (ms * 1e-3))
+
+
+def logits_decode(model, cfg, B, P=512, n_new=128, trials=3, seed=0):
+    """Decode with and without the logits processors on the synthetic model: B prompts of P tokens, greedy, the
+    captured PromptDecoder step replayed for the n_new - 1 steps after the prefill (CUDA events), the two decoders
+    alternating over `trials`.  Processors: repetition_penalty 1.2, no_repeat_ngram_size 3, 16 bad words, min_new_tokens
+    16 with one EOS id."""
+    from quip_b200.decode import PromptDecoder
+    g = torch.Generator().manual_seed(seed)
+    prompts = [torch.randint(0, cfg.vocab_size, (P,), generator=g) for _ in range(B)]
+    bad = [torch.randint(0, cfg.vocab_size, (1 + j % 4,), generator=g).tolist() for j in range(16)]
+    decs = {}
+    for proc in (False, True):
+        d = PromptDecoder(model, max_len=P + n_new, batch=B, max_new=n_new, processing=proc)
+        if proc:
+            d.set_processing(1.2, 3, 16, bad, [2])
+        decs[proc] = d.capture()
+    ms = {False: [], True: []}
+    for _ in range(trials):
+        for proc, d in decs.items():
+            d.prefill(prompts, chunk=512)
+            torch.cuda.synchronize()
+            ms[proc].append(events_ms(d.graph.replay, n_new - 1, warm=0))
+    same = float((decs[False].generated == decs[True].generated).float().mean())
+    r = dict(B=B, P=P, n_new=n_new, plain_ms=min(ms[False]), processed_ms=min(ms[True]), trials_ms=ms,
+             same_token_share_with_processors=same)
+    r['plain_tok_s'], r['processed_tok_s'] = B * 1e3 / r['plain_ms'], B * 1e3 / r['processed_ms']
+    r['slowdown'] = r['processed_ms'] / r['plain_ms'] - 1
+    del decs
+    torch.cuda.empty_cache()
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -977,7 +1041,7 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
-    #                                                                         score, continuous, beam
+    #                                                                         score, continuous, beam, logits
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
@@ -1065,8 +1129,17 @@ def main():
                           f'{1e3 * r["torch_ms"]:.1f} us, max diff {r["max_abs_diff"]:.1e}, greedy equal '
                           f'{r["greedy_equal"]}', flush=True)
                     torch.cuda.empty_cache()
+        if 'logits' in sections and name == 'llama7b':
+            rec['logits_kernel'] = []
+            for B in (1, 32, 128):
+                for V in (32000, 128256):
+                    for hist_len in (512, 4096):
+                        r = logits_kernel_alone(B, V, hist_len, a.kernel_reps)
+                        rec['logits_kernel'].append(r)
+                        print(f'logits process B={B} V={V} history={hist_len}: {1e3 * r["kernel_ms"]:.1f} us '
+                              f'({r["bytes_per_s"] / 1e12:.2f} TB/s of history and logits)', flush=True)
         if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
-                sections & {'chunked', 'paged', 'score', 'continuous', 'beam'} and name == 'llama7b'):
+                sections & {'chunked', 'paged', 'score', 'continuous', 'beam', 'logits'} and name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         if 'score' in sections and name == 'llama7b':
@@ -1158,6 +1231,14 @@ def main():
                               f'fork {1e3 * r["fork_ms"]:.1f} us ({r["fork_copied_bytes_per_s"] / 1e12:.2f} TB/s copied); '
                               f'kernels {100 * r["kernels_share_of_step"]:.1f}% of the step; pool {r["pool_pages"]} pages '
                               f'(bound {r["pool_bound"]})', flush=True)
+        if 'logits' in sections and name == 'llama7b':
+            rec['logits_decode'] = []
+            for B in (1, 32):
+                r = logits_decode(model, cfg, B)
+                rec['logits_decode'].append(r)
+                print(f'{name} decode B={B} P=512, 128 new: plain {r["plain_ms"]:.3f} ms/step ({r["plain_tok_s"]:.0f} '
+                      f'tok/s), with processors {r["processed_ms"]:.3f} ms/step ({r["processed_tok_s"]:.0f} tok/s), '
+                      f'{100 * r["slowdown"]:+.2f}%; trials {r["trials_ms"]}', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
