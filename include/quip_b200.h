@@ -364,6 +364,25 @@ int quip_sample_at(const void* logits, const float* temperature, const int32_t* 
  * other rows.  R >= 0 (0: nothing to do), V >= 1, ld >= V; targets 8-byte and logprob 4-byte aligned. */
 int quip_token_logprobs(const void* logits, int64_t ld, const int64_t* targets, float* logprob, uint8_t* is_greedy,
                         int32_t R, int32_t V, void* stream);
+/* Log-probabilities of generation, from the raw fp16 logits (R, V) with row stride ld (elements; rows need only
+ * 2-byte alignment).  Logits row r is offset i = r % T of decoder row b = rows[r / T] (rows (R / T) int64; null:
+ * b = r / T), its chosen token tokens[r] (int64), and its results go to column c = cols[b * cols_per_row] + i (cols
+ * int64 on the device: one counter per decoder row, cols_per_row = 1, or one shared by every row, 0) of the outputs
+ * lp (B, gen_cols) fp32, top_ids (B, gen_cols, n) int64 and top_lp (B, gen_cols, n) fp32.  A row with b outside
+ * [0, B) or c outside [0, gen_cols) writes nothing (c is not clamped: a done row's last entry is kept).  Otherwise
+ *   lp[b, c]        = what quip_token_logprobs gives for the row and target tokens[r], bit for bit (NaN for a row
+ *                     holding a NaN or a token outside [0, V));
+ *   top_ids[b, c, j], top_lp[b, c, j], j < min(n, V): the row's ids ranked by fp16 logit descending, equal values
+ *                     (-0 == +0) by lower id, and for each the logprob quip_token_logprobs gives with that id as the
+ *                     target, bit for bit (the same row pass: logprob_row.cuh).  The order agrees with the logprob
+ *                     order, as both subtract the same constants;
+ *   j >= min(n, V), and every j of a row holding a NaN: (-1, NaN).
+ * top_ids and top_lp may be null when n = 0.  The launch depends on (R, T, V, n, B, gen_cols) only, so one captured
+ * graph serves every step.  One CTA per row; no workspace.  Bounds: 1 <= T <= 8 dividing R, 1 <= V <= 2^24, ld >= V,
+ * 0 <= n <= 20; int64 arrays 8-byte and fp32 arrays 4-byte aligned. */
+int quip_token_topk_logprobs(const void* logits, int64_t ld, int32_t R, int32_t T, int32_t V, const int64_t* rows,
+                             const int64_t* tokens, const int64_t* cols, int32_t cols_per_row, float* lp,
+                             int64_t* top_ids, float* top_lp, int32_t n, int32_t B, int32_t gen_cols, void* stream);
 
 /* Logits processors of generation (HF's RepetitionPenalty, NoRepeatNGram, NoBadWords and MinNewTokensLength, in that
  * order), in place on fp16 logits (R, V) with row stride ld (elements; rows need only 2-byte alignment).  Logits row r

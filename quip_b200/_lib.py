@@ -120,7 +120,9 @@ EXPORTS = {
                                                                                         C.c_void_p]),
     'quip_token_logprobs': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_void_p]),
-    'quip_beam_candidates': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 4 +
+    'quip_token_topk_logprobs': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_int32] * 3 + [C.c_void_p] * 3 +
+                                 [C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_void_p]),
+    'quip_beam_candidates':(C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 4 +
                              [C.c_void_p]),
     'quip_beam_select': (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 16 + [C.c_int32] * 7 + [C.c_void_p]),
     'quip_kv_beam_fork': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 7 + [C.c_void_p]),

@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'build')
 LIB = os.path.join(HERE, 'libquip_b200.so')
-SOURCES = ['api.cu', 'pack.cu', 'rot.cu', 'rot_small.cu', 'rot_fewtok.cu', 'rot_side.cu', 'rot_side_fewtok.cu', 'glue.cu', 'vecquant.cu', 'ldlq.cu', 'hessian.cu', 'qgemm_skinny.cu', 'qgemv.cu', 'qgemm_tc.cu', 'attn_decode.cu', 'attn_prefill.cu', 'sample.cu', 'spec.cu', 'logprob.cu', 'beam.cu', 'logits_process.cu']
+SOURCES = ['api.cu', 'pack.cu', 'rot.cu', 'rot_small.cu', 'rot_fewtok.cu', 'rot_side.cu', 'rot_side_fewtok.cu', 'glue.cu', 'vecquant.cu', 'ldlq.cu', 'hessian.cu', 'qgemm_skinny.cu', 'qgemv.cu', 'qgemm_tc.cu', 'attn_decode.cu', 'attn_prefill.cu', 'sample.cu', 'spec.cu', 'logprob.cu', 'beam.cu', 'logits_process.cu', 'topk_logprobs.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
@@ -35,7 +35,7 @@ def build(force=False, verbose=False):
     if not os.path.exists(stamp) or open(stamp).read() != flags:
         force = True
     headers = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'), os.path.join(CSRC, 'kv_fp8.cuh'), os.path.join(CSRC, 'kv_page.cuh'),
-               os.path.join(os.path.dirname(HERE), 'include', 'quip_b200.h')]
+               os.path.join(CSRC, 'logprob_row.cuh'), os.path.join(os.path.dirname(HERE), 'include', 'quip_b200.h')]
     jobs = []
     for src in SOURCES:
         s = os.path.join(CSRC, src)

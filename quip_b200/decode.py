@@ -34,7 +34,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-from .fused import PROC_BAD_LEN, PROC_MAX_BAD, PROC_MAX_EOS
+from .fused import PROC_BAD_LEN, PROC_MAX_BAD, PROC_MAX_EOS, TOPK_MAX_N
 
 KV_PAGE = 64                                           # slots per page of a paged KV cache (include/quip_b200.h)
 
@@ -426,6 +426,12 @@ class PromptDecoder(GraphDecoder):
         processors in place, from device buffers filled by set_processing, over the row's history `hist` (B, max_len):
         the prompt by position (written by prefill) and each selected token (written inside the step).  On the CPU the
         same rule in torch (_process_torch).  Needs max_new >= 1;
+      * logprobs=n (0 .. 20; default None: off, nothing allocated or launched): after the selection,
+        quip_token_topk_logprobs (csrc/topk_logprobs.cu; the rule is in include/quip_b200.h) writes the raw logprob of
+        each selected token, and with n >= 1 the n most likely ids and their logprobs, into lp (B, max_new), top_ids and
+        top_lp (B, max_new, n) at the token's column of generated.  Raw: log_softmax of the head's fp16 logits before
+        any processor or temperature; with processing=True the step first copies the rows the processors change in
+        place.  On the CPU the same rule in torch (_token_topk_logprobs_torch).  Needs max_new >= 1;
       * kv_dtype=torch.float8_e4m3fn: k_cache / v_cache e4m3 with k_scale / v_scale (L, B, nkv, max_len) fp32, one scale
         per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
         (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
@@ -441,7 +447,7 @@ class PromptDecoder(GraphDecoder):
     The whole model, no layer pipeline."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False,
-                 page_table=None, n_pages=None, processing=False):
+                 page_table=None, n_pages=None, processing=False, logprobs=None):
         if n_pages is None and page_table is not None:
             raise ValueError('a page_table needs n_pages, the size of the page pool')
         self.n_pages = None if n_pages is None else int(n_pages)
@@ -479,6 +485,17 @@ class PromptDecoder(GraphDecoder):
             self.penalty = torch.ones(B, dtype=torch.float32, device=self.dev)
             self.ngram, self.min_new = z(B, dt=torch.int32), z(B, dt=torch.int32)
             self.proc_eos, self.bad, self.bad_len = z(0), z(0, PROC_BAD_LEN), z(0, dt=torch.int32)
+        self.lp = self.top_ids = self.top_lp = None
+        if logprobs is not None:
+            if isinstance(logprobs, bool) or int(logprobs) != logprobs or not 0 <= logprobs <= TOPK_MAX_N:
+                raise ValueError(f'logprobs must be None or an integer in [0, {TOPK_MAX_N}], got {logprobs!r}')
+            if self.max_new < 1:
+                raise ValueError('logprobs=n records the selected tokens: max_new must be at least 1')
+            G, n = self.generated.shape[1], int(logprobs)
+            self.lp = torch.full((B, G), float('nan'), dtype=torch.float32, device=self.dev)
+            if n:
+                self.top_ids = torch.full((B, G, n), -1, dtype=torch.long, device=self.dev)
+                self.top_lp = torch.full((B, G, n), float('nan'), dtype=torch.float32, device=self.dev)
 
     def set_processing(self, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
                        eos=()):
@@ -527,6 +544,27 @@ class PromptDecoder(GraphDecoder):
         ok = pos < self.max_len if live is None else live & (pos < self.max_len)
         col = pos.clamp(max=self.max_len - 1)
         self.hist[rows, col] = torch.where(ok, tok, self.hist[rows, col])
+
+    def _raw(self, logits):
+        """The logits the logprobs read: a copy when the processors are about to change them in place."""
+        return logits.clone() if self.lp is not None and self.processing else logits
+
+    def _logprobs(self, logits, tokens, cols, rows=None):
+        """With logprobs on: the raw logprob of tokens (R,) or (B, T) and the top n of logits (R, vocab) or
+        (B, T, vocab) into lp / top_ids / top_lp at column cols[b] + i ((B,), or (1,) for every row) of decoder row
+        b = rows[r // T] (default r // T); nothing past the buffers' columns."""
+        if self.lp is None:
+            return
+        T = tokens.shape[1] if tokens.dim() == 2 else 1
+        args = (logits.reshape(-1, logits.shape[-1]), tokens.reshape(-1), cols, self.lp, self.top_ids, self.top_lp)
+        if self._kernel:
+            from . import fused
+            fused.token_topk_logprobs(*args, T=T, rows=rows)
+        else:
+            _token_topk_logprobs_torch(*args, T=T, rows=rows)
+
+    def _logprob_buffers(self):
+        return [t for t in (self.lp, self.top_ids, self.top_lp) if t is not None]
 
     def _prompt_history(self, ids, lens_t):
         """A decoder that keeps a history (processing, SpecDecoder): the prompts ids (B, P) into hist[b, :len_b]; with
@@ -732,11 +770,13 @@ class PromptDecoder(GraphDecoder):
         return o.transpose(1, 2).reshape(B, T, nh * hd)
 
     def _advance(self):
+        raw = self._raw(self.logits)
         if self.processing:
             self._process(self.logits, self.positions)                 # the token just fed is hist[b, positions[b]]
         self.positions.add_(1)
         if self.max_new:
             self._select(self.logits)
+            self._logprobs(raw, self.tokens, self._t)
             self.generated.index_copy_(1, self._t, self.tokens[:, None])
             if self.processing:
                 self._hist_append(self._rows, self.tokens)
@@ -748,7 +788,8 @@ class PromptDecoder(GraphDecoder):
         # decoder is captured before prefill maps its table (generate does so): the warm-up steps then run against an
         # unmapped table and write nothing -- with a page shared by several rows, a warm-up write to slot 0 would
         # corrupt another row's prefix.
-        return [self.positions, self.tokens, self._t, self.generated] + ([self.hist] if self.processing else [])
+        return ([self.positions, self.tokens, self._t, self.generated] + ([self.hist] if self.processing else []) +
+                self._logprob_buffers())
 
     def _counters_in_range(self):
         self.positions.clamp_(max=self.max_len - 1)
@@ -770,6 +811,8 @@ class PromptDecoder(GraphDecoder):
         if self.processing:
             self.hist.zero_()
             self.prompt_len.zero_()
+        for t in self._logprob_buffers():
+            t.fill_(-1 if t.dtype == torch.long else float('nan'))
 
     def _pad_past_end(self):
         return self.paged and self._chunk is not None
@@ -975,9 +1018,11 @@ class PromptDecoder(GraphDecoder):
         """Select the first generated token from the prefill's logits (B, vocab), at t = 0 (processed with the prompt
         as the history)."""
         self._t.zero_()
+        raw = self._raw(logits)
         if self.processing:
             self._process(logits, self.positions - 1)
         self._select(logits)
+        self._logprobs(raw, self.tokens, self._t)
         self.generated[:, 0].copy_(self.tokens)
         if self.processing:
             self._hist_append(self._rows, self.tokens)
@@ -1035,7 +1080,7 @@ class SpecDecoder(PromptDecoder):
     prompt + max_new + draft_tokens (a finished row's step still writes its T slots)."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=1, draft_tokens=4, max_ngram=3, ops=None, kv_dtype=None,
-                 sampling=False, page_table=None, n_pages=None, processing=False):
+                 sampling=False, page_table=None, n_pages=None, processing=False, logprobs=None):
         k, n_max = int(draft_tokens), int(max_ngram)
         if not 1 <= k <= 7:
             raise ValueError(f'draft_tokens must lie in [1, 7], got {draft_tokens}')
@@ -1046,7 +1091,8 @@ class SpecDecoder(PromptDecoder):
         if int(max_len) < k + 2:
             raise ValueError(f'max_len {max_len} leaves no room for a step of {k + 1} tokens')
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
-                         sampling=sampling, page_table=page_table, n_pages=n_pages, processing=processing)
+                         sampling=sampling, page_table=page_table, n_pages=n_pages, processing=processing,
+                         logprobs=logprobs)
         B, dev = self.batch, self.dev
         self.k, self.n_min, self.n_max = k, 1, n_max
         self.T = k + 1
@@ -1072,6 +1118,7 @@ class SpecDecoder(PromptDecoder):
 
     def _advance(self):
         logits = self.logits                                                            # (B, T, vocab)
+        raw = self._raw(logits)
         if self.processing:                  # row i's history: hist[b, :positions[b] + 1], then drafts 1 .. i
             self._process(logits, self.positions, tokens=self.tokens)
         if not self.sampling:
@@ -1081,6 +1128,7 @@ class SpecDecoder(PromptDecoder):
             fused.sample_at(logits, self.temperature, self.top_k, self.top_p, self.seed, self.n_gen, self.targets)
         else:
             self.targets.copy_(_sample_torch_at(logits, self.temperature, self.top_k, self.top_p, self.seed, self.n_gen))
+        self._logprobs(raw, self.targets, self.n_gen)              # accepted targets: columns n_gen .. n_gen + e - 1
         if self._kernel:
             from . import fused
             fused.spec_accept(self.tokens, self.targets, self.generated, self.hist, self.positions, self.n_gen,
@@ -1117,9 +1165,11 @@ class SpecDecoder(PromptDecoder):
 
     def _first_token(self, logits):
         self._t.zero_()
+        raw = self._raw(logits)
         if self.processing:
             self._process(logits, self.positions - 1)
         self._select(logits, out=self._first)
+        self._logprobs(raw, self._first, self._t)
         self.generated[:, 0].copy_(self._first)
         self.hist[self._rows, self.positions] = self._first
         self.n_gen.fill_(1)
@@ -1175,10 +1225,10 @@ class ContinuousDecoder(PromptDecoder):
     through the table, SDPA under each sequence's causal mask)."""
 
     def __init__(self, model, max_len, batch, n_pages, max_new, ops=None, kv_dtype=None, sampling=False, eos=(),
-                 processing=False):
+                 processing=False, logprobs=None):
         max_pages = -(-int(max_len) // KV_PAGE)
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
-                         sampling=sampling, n_pages=n_pages, processing=processing,
+                         sampling=sampling, n_pages=n_pages, processing=processing, logprobs=logprobs,
                          page_table=torch.full((int(batch), max_pages), -1, dtype=torch.int32))
         B, dev = self.batch, self.dev
         self.n_gen = torch.zeros(B, dtype=torch.long, device=dev)
@@ -1247,9 +1297,12 @@ class ContinuousDecoder(PromptDecoder):
         self.done[rows] = self.done[rows] | (live & stop)
 
     def _advance(self):
+        raw = self._raw(self.logits)
         if self.processing:
             self._process(self.logits, self.positions)
-        self._commit(self._rows, self._choose(self.logits, self._rows))
+        tok = self._choose(self.logits, self._rows)
+        self._logprobs(raw, tok, self.n_gen)                   # a done row's column n_gen lies past its own tokens
+        self._commit(self._rows, tok)
 
     def _capture_state(self):
         return super()._capture_state() + [self.n_gen, self.active, self.done]
@@ -1306,9 +1359,12 @@ class ContinuousDecoder(PromptDecoder):
                 last = [int(pieces[j][2]) + int(pieces[j][1].numel()) - 1 for j in ends]
                 self.positions[out_t[nd:]] = torch.tensor(last, dtype=torch.long).to(dev)
             logits = self._head(h[0, idx][:, None], None if pend is None else pend[0, idx][:, None])
+            raw = self._raw(logits)
             if self.processing:
                 self._process(logits, self.positions, rows=out_t)
-            self._commit(out_t, self._choose(logits, out_t))
+            tok = self._choose(logits, out_t)
+            self._logprobs(raw, tok, self.n_gen, rows=out_t)
+            self._commit(out_t, tok)
         return logits
 
     def _rope_rows(self, pos, T):
@@ -1703,18 +1759,22 @@ class ContinuousSchedule:
 
 
 def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len,
-                         proc=None):
+                         proc=None, logprobs=None, top_logprobs=0):
     """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages;
-    proc: the per-prompt (penalties, ngram sizes, min_new_tokens) and the bad words of the logits processors, or None."""
+    proc: the per-prompt (penalties, ngram sizes, min_new_tokens) and the bad words of the logits processors, or None;
+    logprobs: generate()'s dict, or None.  A request's logprob entries are read with its tokens, before its row takes
+    the next prompt (admission resets n_gen, and the next request writes the same columns)."""
     lens = [p.numel() for p in prompts]
     sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk)
     dec = ContinuousDecoder(model, max_len, rows, kv_pages, max(max_new), kv_dtype=kv_dtype,
-                            sampling=settings is not None, eos=eos, processing=proc is not None)
+                            sampling=settings is not None, eos=eos, processing=proc is not None,
+                            logprobs=None if logprobs is None else top_logprobs)
     if proc is not None:
         dec.set_processing(bad_words_ids=proc[3] or None, eos=eos)
     if dec.dev.type == 'cuda':
         dec.capture()                                # before any row is mapped: the warm-up steps write nothing
     out = [None] * len(prompts)
+    lps = [None] * len(prompts)
     eos_c = torch.tensor(eos, dtype=torch.long)
     steps = 0
     while True:
@@ -1725,10 +1785,16 @@ def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows,
             if fin:
                 fin_t = torch.tensor(fin, dtype=torch.long).to(dec.dev)
                 gen, n_gen = dec.generated[fin_t].cpu(), dec.n_gen[fin_t].cpu()
+                cut = []
                 for j, r in enumerate(fin):
                     row = gen[j, :int(n_gen[j])]
                     hit = torch.isin(row, eos_c).nonzero()
-                    out[sched.retire(r)] = row[:int(hit[0]) + 1] if hit.numel() else row
+                    cut.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+                if logprobs is not None:
+                    for r, e in zip(fin, _read_logprobs(dec, fin, cut)):
+                        lps[sched.req[r]] = e
+                for r, row in zip(fin, cut):
+                    out[sched.retire(r)] = row
                     dec.retire(r)
             for r, i, pages in sched.admit():
                 dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings],
@@ -1742,6 +1808,8 @@ def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows,
         else:
             dec.decode_step()
         steps += 1
+    if logprobs is not None:
+        _put_logprobs(logprobs, lps)
     return out
 
 
@@ -1878,6 +1946,36 @@ def _token_logprobs_torch(logits, targets):
     lp = torch.log_softmax(x, -1).gather(-1, t[:, None])[:, 0]
     lp = torch.where(ok, lp, torch.full_like(lp, float('nan')))
     return lp, ((x.argmax(-1) == t) & ok).to(torch.uint8)
+
+
+def _token_topk_logprobs_torch(logits, tokens, cols, lp, top_ids=None, top_lp=None, T=1, rows=None):
+    """The rule of quip_token_topk_logprobs (include/quip_b200.h) in torch, in place, arguments as
+    fused.token_topk_logprobs; logits fp16, or fp32 on the CPU (ranked by their own values).  Each value is gathered
+    from the log_softmax _token_logprobs_torch takes, so a greedy row's top value is its token's, bit for bit."""
+    R, V = logits.shape
+    B, G = lp.shape
+    dev = lp.device
+    r = torch.arange(R, device=dev)
+    b = r // T if rows is None else rows.to(dev)[r // T]
+    c = cols.to(dev)[b.clamp(0, B - 1) if cols.numel() == B else torch.zeros_like(b)] + r % T
+    ok = (b >= 0) & (b < B) & (c >= 0) & (c < G)
+    b, c = b[ok], c[ok]
+    x = logits[ok.to(logits.device)]
+    tok_lp, _ = _token_logprobs_torch(x, tokens[ok.to(tokens.device)])
+    lp[b, c] = tok_lp.to(dev)
+    if top_ids is None:
+        return lp
+    n, k = top_ids.shape[-1], min(top_ids.shape[-1], V)
+    xf = x.float()
+    ids = torch.full((x.shape[0], n), -1, dtype=torch.long, device=x.device)
+    vals = torch.full((x.shape[0], n), float('nan'), dtype=torch.float32, device=x.device)
+    ids[:, :k] = torch.sort(xf + 0.0, dim=-1, descending=True, stable=True).indices[:, :k]   # -0 + 0 = +0: ties by id
+    vals[:, :k] = torch.log_softmax(xf, -1).gather(-1, ids[:, :k])
+    nan = torch.isnan(xf).any(-1)
+    ids[nan], vals[nan] = -1, float('nan')
+    top_ids[b, c] = ids.to(dev)
+    top_lp[b, c] = vals.to(dev)
+    return lp
 
 
 def _e4m3_quantize(x):
@@ -2026,7 +2124,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
              temperature=1.0, top_k=0, top_p=1.0, seed=0, prompt_lookup_num_tokens=None, max_matching_ngram_size=3,
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
              max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
-             beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None):
+             beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
+             logprobs=None, top_logprobs=0):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -2105,7 +2204,23 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     They combine with greedy and sampled decoding, num_return_sequences, share_prompt_prefixes, prefill_chunk_size,
     kv_dtype, prompt_lookup_num_tokens (the tokens stay those of plain generation) and max_batch_size; with at most 8 EOS
     ids.  Any setting other than the default with num_beams > 1 raises ValueError (HF processes the beams' log-softmax,
-    which quip_beam_candidates computes itself).  With every default, nothing of this runs."""
+    which quip_beam_candidates computes itself).  With every default, nothing of this runs.
+
+    logprobs: a dict that receives the log-probabilities of the returned tokens under the model's raw distribution --
+    log_softmax of the fp16 lm_head logits, before any processor, temperature, top-k or top-p (HF's output_logits) --
+    computed inside the captured step by quip_token_topk_logprobs (the rule is in include/quip_b200.h).  For output row
+    i (the order of the returned list) with len_i tokens, logprobs['token'][i] is an fp32 tensor (len_i,); with
+    top_logprobs=n (1 .. 20) logprobs['top_ids'][i] (int64) and logprobs['top'][i] (fp32) are (len_i, n): the n most
+    likely ids at each position, by logit descending and then lower id, and their logprobs.  They are the same for
+    greedy, sampled and speculative runs and combine with every path but num_beams > 1 (beam_stats has the beams'
+    scores).  With logprobs=None nothing is allocated or launched; the returned tokens never change."""
+    if logprobs is not None and not isinstance(logprobs, dict):
+        raise ValueError(f'logprobs must be None or a dict that receives the results, got {type(logprobs).__name__}')
+    if isinstance(top_logprobs, bool) or not isinstance(top_logprobs, int) or not 0 <= top_logprobs <= TOPK_MAX_N:
+        raise ValueError(f'top_logprobs must be an integer in [0, {TOPK_MAX_N}], got {top_logprobs!r}')
+    if top_logprobs and logprobs is None:
+        raise ValueError('top_logprobs needs a logprobs dict to receive the results')
+    n_lp = None if logprobs is None else int(top_logprobs)
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
     n_ret = num_return_sequences
     if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
@@ -2114,6 +2229,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     if isinstance(num_beams, bool) or int(num_beams) != num_beams or not 1 <= num_beams <= 16:
         raise ValueError(f'num_beams must be an integer in [1, 16], got {num_beams!r}')
     nb = int(num_beams)
+    if nb > 1 and logprobs is not None:
+        raise ValueError('logprobs does not combine with num_beams > 1 (beam_stats has the beams\' scores)')
     if nb > 1:
         for name, on in (('do_sample', bool(do_sample)), ('prompt_lookup_num_tokens', prompt_lookup_num_tokens is not None),
                          ('max_batch_size', max_batch_size is not None), ('kv_pages', kv_pages is not None),
@@ -2200,7 +2317,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError(f'kv_pages must be an integer >= 1, got {kv_pages!r}')
         return _generate_continuous(model, prompts, budgets, eos, kv_dtype, settings if do_sample else None, rows,
                                     int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len,
-                                    proc)
+                                    proc, logprobs, int(top_logprobs))
     pages, starts = {}, None
     if share:
         table, n_pages, starts = plan_prefix_pages(prompts, [n + m + k for n, m in zip(lens, budgets)],
@@ -2208,6 +2325,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         pages = dict(page_table=table, n_pages=n_pages)
     if proc is not None:
         pages['processing'] = True
+    if n_lp is not None:
+        pages['logprobs'] = n_lp
     if spec:
         dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
                           max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
@@ -2223,7 +2342,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
     if spec:
-        return _generate_spec(dec, budgets, eos_t, spec_stats)
+        return _generate_spec(dec, budgets, eos_t, spec_stats, logprobs)
     n = 1
     while n < max_new_tokens:
         if (eos or min(budgets) < max_new_tokens) and n % EOS_CHECK_EVERY == 0:
@@ -2239,10 +2358,28 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         row = row[:m]
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+    if logprobs is not None:
+        _put_logprobs(logprobs, _read_logprobs(dec, list(range(len(out))), out))
     return out
 
 
-def _generate_spec(dec, budgets, eos_t, stats):
+def _read_logprobs(dec, rows, outs):
+    """The logprob entries of decoder rows `rows`, each cut to the length of its returned tokens outs[i]:
+    [(token (len,), top_ids (len, n) or None, top (len, n) or None)]."""
+    idx = torch.tensor(rows, dtype=torch.long, device=dec.dev)
+    bufs = [None if t is None else t[idx].cpu() for t in (dec.lp, dec.top_ids, dec.top_lp)]
+    return [tuple(None if t is None else t[j, :o.numel()] for t in bufs) for j, o in enumerate(outs)]
+
+
+def _put_logprobs(dest, entries):
+    """generate()'s logprobs dict from the entries of _read_logprobs, in output order."""
+    dest['token'] = [e[0] for e in entries]
+    if entries[0][1] is not None:
+        dest['top_ids'] = [e[1] for e in entries]
+        dest['top'] = [e[2] for e in entries]
+
+
+def _generate_spec(dec, budgets, eos_t, stats, logprobs=None):
     """generate()'s host loop over SpecDecoder steps: it syncs only every EOS_CHECK_EVERY steps, to stop once every row
     has max_new tokens or an EOS among its tokens.  Each row is cut to its own budget."""
     max_new = max(budgets)
@@ -2265,6 +2402,8 @@ def _generate_spec(dec, budgets, eos_t, stats):
         row = row[:min(n, m)]
         hit = torch.isin(row, eos_t.cpu()).nonzero()
         out.append(row[:int(hit[0]) + 1] if hit.numel() else row)
+    if logprobs is not None:
+        _put_logprobs(logprobs, _read_logprobs(dec, list(range(len(out))), out))
     return out
 
 

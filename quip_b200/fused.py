@@ -300,6 +300,62 @@ def token_logprobs(logits, targets, logprob_out, greedy_out):
     return logprob_out, greedy_out
 
 
+TOPK_MAX_N, TOPK_MAX_T, TOPK_MAX_V = 20, 8, 2 ** 24
+
+
+def token_topk_logprobs(logits, tokens, cols, lp, top_ids=None, top_lp=None, T=1, rows=None):
+    """quip_token_topk_logprobs: for each row r of raw logits (R, V) fp16 (stride(1) == 1, any stride(0) >= V), offset
+    r % T of decoder row b = rows[r // T] (rows (R // T,) int64; default r // T), writes at column
+    c = cols[b] + r % T (cols (B,) int64, or (1,) shared by every row) lp[b, c] = log_softmax(logits[r])[tokens[r]]
+    and the row's top n ids and logprobs into top_ids[b, c, :] / top_lp[b, c, :] (the rule of include/quip_b200.h;
+    nothing is written when c is outside [0, gen_cols)).  tokens (R,) int64; lp (B, gen_cols) fp32; top_ids
+    (B, gen_cols, n) int64 and top_lp (B, gen_cols, n) fp32 with 1 <= n <= 20, or both None.  CUDA, one device,
+    outputs contiguous; everything is checked before the launch, which runs on the current stream.  Returns lp."""
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'token_topk_logprobs: logits must be (R, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    R, V = logits.shape
+    if not 1 <= V <= TOPK_MAX_V or (R > 1 and logits.stride(0) < V) or (V > 1 and logits.stride(1) != 1):
+        raise ValueError(f'token_topk_logprobs: logits rows must be unit-stride, not overlap and hold 1 .. {TOPK_MAX_V}'
+                         f' values, got shape {tuple(logits.shape)} strides {tuple(logits.stride())}')
+    if isinstance(T, bool) or int(T) != T or not 1 <= T <= TOPK_MAX_T or R % T:
+        raise ValueError(f'token_topk_logprobs: T must be an integer in [1, {TOPK_MAX_T}] dividing R = {R}, got {T!r}')
+    if R > 2 ** 31 - 1:
+        raise ValueError(f'token_topk_logprobs: {R} rows exceed the launch limit of 2^31 - 1')
+    if lp.dim() != 2:
+        raise ValueError(f'token_topk_logprobs: lp must be (B, gen_cols), got {tuple(lp.shape)}')
+    B, G = lp.shape
+    if (top_ids is None) != (top_lp is None):
+        raise ValueError('token_topk_logprobs: pass top_ids and top_lp together, or neither')
+    n = 0 if top_ids is None else (top_ids.shape[-1] if top_ids.dim() == 3 else -1)
+    if top_ids is not None and not 1 <= n <= TOPK_MAX_N:
+        raise ValueError(f'token_topk_logprobs: top_ids must be (B, gen_cols, n) with 1 <= n <= {TOPK_MAX_N}, got '
+                         f'{tuple(top_ids.shape)}')
+    if rows is None and R // T != B:
+        raise ValueError(f'token_topk_logprobs: {R // T} logits rows of T = {T} for {B} output rows: pass rows')
+    checks = [('tokens', tokens, torch.int64, (R,)), ('lp', lp, torch.float32, (B, G))]
+    if cols.dtype != torch.int64 or tuple(cols.shape) not in ((B,), (1,)):
+        raise ValueError(f'token_topk_logprobs: cols must be ({B},) or (1,) int64, got {tuple(cols.shape)} {cols.dtype}')
+    checks.append(('cols', cols, torch.int64, tuple(cols.shape)))
+    if top_ids is not None:
+        checks += [('top_ids', top_ids, torch.int64, (B, G, n)), ('top_lp', top_lp, torch.float32, (B, G, n))]
+    if rows is not None:
+        checks.append(('rows', rows, torch.int64, (R // T,)))
+    for name, t, dt, shape in checks:
+        if t.dtype != dt or tuple(t.shape) != shape:
+            raise ValueError(f'token_topk_logprobs: {name} must be {shape} {dt}, got {tuple(t.shape)} {t.dtype}')
+    if not logits.is_cuda:
+        raise RuntimeError('token_topk_logprobs runs on a CUDA device only (there is no CPU fallback)')
+    _check_cuda('token_topk_logprobs', [t for _, t, _, _ in checks], logits.device)
+    ld = logits.stride(0) if R > 1 else V
+    p = lambda t: None if t is None else t.data_ptr()
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_token_topk_logprobs(logits.data_ptr(), ld, R, int(T), V, p(rows), tokens.data_ptr(),
+                                                        cols.data_ptr(), int(cols.numel() == B), lp.data_ptr(),
+                                                        p(top_ids), p(top_lp),
+                                                        n, B, G, torch.cuda.current_stream(logits.device).cuda_stream))
+    return lp
+
+
 def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
     """quip_extend_attention(_fp8) on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot
     positions[b] + i of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots

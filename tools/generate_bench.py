@@ -59,6 +59,12 @@ at B in {1, 32, 128}, V in {32000, 128256} and histories of 512 and 4096 tokens 
 16 bad words), and the captured PromptDecoder step with and without processors at B in {1, 32}, 512-token prompts and
 128 new tokens, alternated over three trials.
 
+Section logprobs (llama7b) measures the log-probabilities of generation (quip_token_topk_logprobs,
+csrc/topk_logprobs.cu): the kernel alone on R in {1, 8, 32, 256} rows of V = 32000 fp16 logits with n in {0, 5, 20}
+(time, and one pass over the logits per second), and the captured PromptDecoder step at B in {1, 8, 32} (256-token
+prompts, 64 new tokens, greedy) with logprobs off, n = 0 and n = 20, with the logits processors off and on, the three
+decoders alternating over three trials.
+
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
 whose cache (twice over: GraphDecoder.capture keeps a copy) does not fit the free device memory is skipped and listed.
@@ -1033,6 +1039,58 @@ def logits_decode(model, cfg, B, P=512, n_new=128, trials=3, seed=0):
     return r
 
 
+def logprobs_kernel_alone(R, V, n, reps, seed=0):
+    """quip_token_topk_logprobs alone on R fp16 rows of V logits (randn * 3), one output column per row, top n.  Timed
+    as 20 launches captured in one CUDA graph (CUDA events around the replays).  Bytes: one pass over the logits (the
+    kernel reads each row once for the lse and, with n > 0, three more times, mostly from L2)."""
+    from quip_b200 import fused
+    dev = torch.device('cuda:0')
+    g = torch.Generator().manual_seed(seed)
+    x = (torch.randn(R, V, generator=g) * 3).half().to(dev)
+    tok = torch.randint(0, V, (R,), generator=g).to(dev)
+    cols = torch.zeros(R, dtype=torch.long, device=dev)
+    lp = torch.empty(R, 1, device=dev)
+    ids = torch.empty(R, 1, n, dtype=torch.long, device=dev) if n else None
+    top = torch.empty(R, 1, n, device=dev) if n else None
+    fused.token_topk_logprobs(x, tok, cols, lp, ids, top)
+    graph, per = torch.cuda.CUDAGraph(), 20
+    with torch.cuda.graph(graph):
+        for _ in range(per):
+            fused.token_topk_logprobs(x, tok, cols, lp, ids, top)
+    ms = events_ms(graph.replay, max(reps // per, 5)) / per
+    return dict(R=R, V=V, n=n, kernel_ms=ms, bytes_per_s=R * V * 2 / (ms * 1e-3))
+
+
+def logprobs_decode(model, cfg, B, proc, P=256, n_new=64, trials=3, seed=0):
+    """The captured PromptDecoder step with logprobs off, n = 0 and n = 20: B prompts of P tokens, greedy, the step
+    replayed for the n_new - 1 steps after the prefill (CUDA events), the three decoders alternating over `trials`.
+    proc: the logits processors on (repetition_penalty 1.2, no_repeat_ngram_size 3, 16 bad words), so the step also
+    copies its raw logits."""
+    from quip_b200.decode import PromptDecoder
+    g = torch.Generator().manual_seed(seed)
+    prompts = [torch.randint(0, cfg.vocab_size, (P,), generator=g) for _ in range(B)]
+    bad = [torch.randint(0, cfg.vocab_size, (1 + j % 4,), generator=g).tolist() for j in range(16)]
+    decs = {}
+    for n in (None, 0, 20):
+        d = PromptDecoder(model, max_len=P + n_new, batch=B, max_new=n_new, processing=proc, logprobs=n)
+        if proc:
+            d.set_processing(1.2, 3, 0, bad, [2])
+        decs[n] = d.capture()
+    ms = {n: [] for n in decs}
+    for _ in range(trials):
+        for n, d in decs.items():
+            d.prefill(prompts, chunk=256)
+            torch.cuda.synchronize()
+            ms[n].append(events_ms(d.graph.replay, n_new - 1, warm=0))
+    same = all(torch.equal(decs[None].generated, d.generated) for d in decs.values())
+    r = dict(B=B, P=P, n_new=n_new, processing=proc, off_ms=min(ms[None]), n0_ms=min(ms[0]), n20_ms=min(ms[20]),
+             trials_ms={str(k): v for k, v in ms.items()}, tokens_identical=same)
+    r['n0_overhead'], r['n20_overhead'] = r['n0_ms'] / r['off_ms'] - 1, r['n20_ms'] / r['off_ms'] - 1
+    del decs
+    torch.cuda.empty_cache()
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
@@ -1041,7 +1099,8 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
-    #                                                                         score, continuous, beam, logits
+    #                                                                         score, continuous, beam, logits,
+    #                                                                         logprobs
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
@@ -1138,8 +1197,17 @@ def main():
                         rec['logits_kernel'].append(r)
                         print(f'logits process B={B} V={V} history={hist_len}: {1e3 * r["kernel_ms"]:.1f} us '
                               f'({r["bytes_per_s"] / 1e12:.2f} TB/s of history and logits)', flush=True)
+        if 'logprobs' in sections and name == 'llama7b':
+            rec['logprobs_kernel'] = []
+            for R in (1, 8, 32, 256):
+                for n in (0, 5, 20):
+                    r = logprobs_kernel_alone(R, 32000, n, a.kernel_reps)
+                    rec['logprobs_kernel'].append(r)
+                    print(f'logprobs kernel R={R} V=32000 n={n}: {1e3 * r["kernel_ms"]:.1f} us '
+                          f'({r["bytes_per_s"] / 1e12:.2f} TB/s of logits)', flush=True)
         if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
-                sections & {'chunked', 'paged', 'score', 'continuous', 'beam', 'logits'} and name == 'llama7b'):
+                sections & {'chunked', 'paged', 'score', 'continuous', 'beam', 'logits', 'logprobs'} and
+                name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
         if 'score' in sections and name == 'llama7b':
@@ -1239,6 +1307,16 @@ def main():
                 print(f'{name} decode B={B} P=512, 128 new: plain {r["plain_ms"]:.3f} ms/step ({r["plain_tok_s"]:.0f} '
                       f'tok/s), with processors {r["processed_ms"]:.3f} ms/step ({r["processed_tok_s"]:.0f} tok/s), '
                       f'{100 * r["slowdown"]:+.2f}%; trials {r["trials_ms"]}', flush=True)
+        if 'logprobs' in sections and name == 'llama7b':
+            rec['logprobs_decode'] = []
+            for proc in (False, True):
+                for B in (1, 8, 32):
+                    r = logprobs_decode(model, cfg, B, proc)
+                    rec['logprobs_decode'].append(r)
+                    print(f'{name} decode B={B} P=256 processors={proc}: off {r["off_ms"]:.3f} ms/step, n=0 '
+                          f'{r["n0_ms"]:.3f} ({100 * r["n0_overhead"]:+.2f}%), n=20 {r["n20_ms"]:.3f} '
+                          f'({100 * r["n20_overhead"]:+.2f}%); tokens identical {r["tokens_identical"]}; trials '
+                          f'{r["trials_ms"]}', flush=True)
         for B, P in ((1, 2048), (8, 512)) if 'prefill' in sections else ():
             r = prefill_rate(model, B, P)
             rec['prefill'].append(r)
