@@ -344,7 +344,7 @@ int quip_prefill_attention_ragged_fp8(const void* q, const void* k_pool, const v
  * order (u * S exactly), so a token depends only on (row, settings, seed, t) -- not on the batch, the row index or the
  * launch -- and is bit-identical from run to run.  A row with non-finite logits still gets an index in [0, V).  The
  * launch depends on (B, V) only: one captured graph serves every step and any settings written between replays.
- * No workspace.  B >= 0 (0: nothing to do), 1 <= V <= 2^24. */
+ * No workspace.  B >= 0 (0: nothing to do), 1 <= V <= 2^24 - 1 (V weights of at most 2^40 sum below 2^64). */
 int quip_sample(const void* logits, const float* temperature, const int32_t* top_k, const float* top_p,
                 const uint64_t* seed, const int64_t* step, int64_t* tokens, int32_t B, int32_t V, void* stream);
 /* The same rule over logits (B * T, V): row b * T + i takes the settings and seed of row b (each (B)) and

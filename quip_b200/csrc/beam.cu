@@ -51,6 +51,7 @@ __device__ __forceinline__ void lse_one(Lse& a, float v) {
     a.s = a.s * expf(a.m - v);
     a.m = v;
   }
+  if (a.m == -INFINITY) return;                           // only -inf so far: adds nothing
   a.s += expf(v - a.m);
 }
 
@@ -70,6 +71,7 @@ __device__ __forceinline__ void lse_eight(Lse& a, const float* v) {
     a.s = a.s * expf(a.m - gm);
     a.m = gm;
   }
+  if (a.m == -INFINITY) return;                           // a group of -inf before any finite value adds nothing
   float t = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) t += expf(v[j] - a.m);

@@ -17,7 +17,7 @@ constexpr int LP_THREADS = 512;
 constexpr int LP_WARPS = LP_THREADS / 32;
 
 struct RowStat {
-  float m, s;      // running max and sum of exp(x - m); (-inf, 0) before any value
+  float m, s;      // running max and sum of exp(x - m); (-inf, 0) before any finite value
   float bv;        // largest value seen, and its lowest index (INT_MAX before any value)
   int bi;
   bool nan;
@@ -40,6 +40,7 @@ __device__ __forceinline__ void add_one(RowStat& a, float v, int i) {
     a.s = a.s * expf(a.m - v);
     a.m = v;
   }
+  if (a.m == -INFINITY) return;                  // only -inf so far: adds nothing (expf(-inf - -inf) would be NaN)
   a.s += expf(v - a.m);
 }
 
@@ -70,6 +71,7 @@ __device__ __forceinline__ void add_eight(RowStat& a, const uint4& raw, int i0) 
     a.s = a.s * expf(a.m - gm);
     a.m = gm;
   }
+  if (a.m == -INFINITY) return;                  // a group of -inf before any finite value adds nothing
   float t = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) t += expf(v[j] - a.m);

@@ -15,7 +15,7 @@
 //   select        per-warp totals of the kept weight over contiguous index segments, a serial prefix over the 16 warps,
 //                 and one warp walking its segment with a warp scan for the first running sum > u * S.
 //
-// Weights are e = expf(z - zmax) in fixed point, floor(e * 2^40) as uint64 (sums < 2^64 for V <= 2^24; e < 2^-40
+// Weights are e = expf(z - zmax) in fixed point, floor(e * 2^40) as uint64 (sums <= V 2^40 < 2^64 for V < 2^24; e < 2^-40
 // counts 0): integer histograms and sums are exact in any order, so shared-memory atomics are deterministic and the
 // running sum of the walk reaches exactly the S it is compared against; u * S is taken exactly (floor(w24 * S / 2^24)).
 // The kept set always has the form {key > tau} + {the first m keys == tau in index order}.  Every pass recomputes z from
@@ -37,7 +37,7 @@ constexpr int SP_THREADS = 512;
 constexpr int SP_WARPS = SP_THREADS / 32;
 constexpr uint32_t SP_ALL = 0xFFFFFFFFu;      // m: every key == tau is kept
 constexpr float SP_FIX = 1099511627776.f;     // 2^40
-constexpr int SP_MAX_V = 1 << 24;             // V * 2^40 < 2^64: the fixed-point sums cannot overflow
+constexpr int SP_MAX_V = (1 << 24) - 1;       // V * 2^40 < 2^64: the fixed-point sums cannot overflow (2^24 * 2^40 wraps to 0)
 
 __device__ __forceinline__ uint32_t order_key(float z) {
   if (z != z) return 0xFFFFFFFFu;
@@ -348,7 +348,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const __half* __r
     const int64_t t = step[(int64_t)bs * step_stride] + b % per_set;
     const uint64_t sd = seed[bs];
     const uint32_t w24 = philox_word0((uint32_t)t, (uint32_t)((uint64_t)t >> 32), (uint32_t)sd, (uint32_t)(sd >> 32)) >> 8;
-    // thr = floor(u * S), u = w24 / 2^24, exactly (S < 2^57)
+    // thr = floor(u * S), u = w24 / 2^24, exactly (S < 2^64: the 128-bit product shifted right by 24)
     const unsigned long long lo64 = S * (unsigned long long)w24, hi64 = __umul64hi(S, (unsigned long long)w24);
     const unsigned long long thr = (hi64 << 40) | (lo64 >> 24);
     s.warp_sel = -1;

@@ -243,6 +243,9 @@ def kv_quantize(src, cache, scales):
                                                     max_len, hd, torch.cuda.current_stream(src.device).cuda_stream))
 
 
+SAMPLE_MAX_V = 2 ** 24 - 1
+
+
 def sample(logits, temperature, top_k, top_p, seed, step, out):
     """quip_sample on torch tensors: one token per row of logits (B, V) fp16 into out (B,) int64, by the rule of
     include/quip_b200.h (greedy rows T <= 0 or k == 1; else temperature, top-k, top-p and a Philox draw of (seed, step)).
@@ -259,6 +262,8 @@ def sample(logits, temperature, top_k, top_p, seed, step, out):
                              f'{tuple(t.shape)} {t.dtype}')
     if step.dtype != torch.int64 or step.numel() != 1:
         raise ValueError(f'sample: step must be one int64, got {tuple(step.shape)} {step.dtype}')
+    if not 1 <= logits.shape[1] <= SAMPLE_MAX_V:
+        raise ValueError(f'sample: need 1 <= V <= {SAMPLE_MAX_V} (the fixed-point sum of V weights), got V {logits.shape[1]}')
     _check_cuda('sample', (logits, temperature, top_k, top_p, seed, step, out), logits.device)
     with torch.cuda.device(logits.device):
         _lib.check(_lib.load().quip_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(),
@@ -646,6 +651,8 @@ def sample_at(logits, temperature, top_k, top_p, seed, steps, out):
         if t.dtype not in dts or tuple(t.shape) != shape:
             raise ValueError(f'sample_at: {name} must be {shape} {" or ".join(str(d) for d in dts)}, got '
                              f'{tuple(t.shape)} {t.dtype}')
+    if not 1 <= V <= SAMPLE_MAX_V:
+        raise ValueError(f'sample_at: need 1 <= V <= {SAMPLE_MAX_V} (the fixed-point sum of V weights), got V {V}')
     _check_cuda('sample_at', (logits, temperature, top_k, top_p, seed, steps, out), logits.device)
     with torch.cuda.device(logits.device):
         _lib.check(_lib.load().quip_sample_at(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(),

@@ -190,6 +190,7 @@ def test_quip_sample_argument_errors_surface_as_messages():
     assert call(B=-1) == 1 and b'bad sizes' in lib.quip_last_error()
     assert call(V=0) == 1 and b'bad sizes' in lib.quip_last_error()
     assert call(V=(1 << 24) + 1) == 1 and b'bad sizes' in lib.quip_last_error()
+    assert call(V=1 << 24) == 1 and b'bad sizes' in lib.quip_last_error()     # 2^24 weights of 2^40 wrap the sum
     for kw in (dict(logits=None), dict(seed=None), dict(step=None), dict(out=None)):
         assert call(**kw) == 1 and b'null' in lib.quip_last_error()
     with pytest.raises(_lib.QuipError, match='null pointer'):
@@ -209,3 +210,10 @@ def test_sample_wrapper_checks_and_refuses_cpu_tensors():
                       ('seed', torch.zeros(B + 1, dtype=torch.int64)), ('step', torch.zeros(2, dtype=torch.int64))):
         with pytest.raises(ValueError, match=name):
             fused.sample(**{**args, name: bad})
+    wide = torch.empty(B, 1 << 24, dtype=torch.float16)                # 2^24 weights of 2^40 would wrap the sum
+    with pytest.raises(ValueError, match=r'sample: need 1 <= V <= 16777215'):
+        fused.sample(**{**args, 'logits': wide})
+    steps = torch.zeros(B, dtype=torch.int64)
+    with pytest.raises(ValueError, match=r'sample_at: need 1 <= V <= 16777215'):
+        fused.sample_at(wide.view(B, 1, -1), *[args[k] for k in ('temperature', 'top_k', 'top_p', 'seed')], steps,
+                        args['out'].view(B, 1))
