@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define QUIP_ABI_VERSION 2
+#define QUIP_ABI_VERSION 3
 
 enum {
   QUIP_OK = 0,
@@ -135,57 +135,80 @@ int quip_silu_mul(const void* gate, const void* up, void* out, int64_t n, void* 
 int quip_silu_mul_gather(const void* gate, const void* up, const uint32_t* idx, void* out, int64_t rows, int32_t n,
                          void* stream);
 
-/* One decode-attention step for B sequences, each at its own position, on one layer of the static KV cache.
- *   q (B, nh, hd) fp16 with rotary applied; k_new / v_new (B, nkv, hd) fp16: this step's key / value;
- *   k_cache / v_cache (B, nkv, max_len, hd) fp16; positions (B) int64 on the device; out (B, nh, hd) fp16.
+/* The KV cache of one layer, as every cache operation below takes it (decode, extend and prefill attention, the
+ * appends and the beam fork).  The format is stated once here; the operations add only their own rules.
+ *
+ * Format.  QUIP_KV_FP16: k / v hold fp16 values and k_scale / v_scale are NULL.  QUIP_KV_E4M3: k / v hold e4m3fn
+ * bytes and k_scale / v_scale fp32, one scale per cached head vector x (hd values):
+ *   amax = max_i |x_i|;  s = amax / 448 (IEEE fp32 division; s = 1 when amax == 0);  q_i = e4m3fn(x_i / s), round to
+ *   nearest even, subnormals kept;  the vector's value is float(q_i) * s.
+ * New keys and values (fp16) are quantized so when they are appended, written with their scales, and attended over as
+ * quantized values like every other slot; no scale past the slots a launch reads is read.  Non-finite inputs may give
+ * NaN outputs.  The format is never inferred from the scales: they must be non-NULL exactly when it is QUIP_KV_E4M3, so
+ * a NULL scale pointer is an error, never e4m3 bytes read as fp16.
+ *
+ * Layout.  page_table NULL: the contiguous cache, k / v (B, nkv, max_len, hd) and scales (B, nkv, max_len);
+ * max_pages and n_pages are not read.  page_table non-NULL: the paged cache, k / v pools (n_pages, nkv, 64, hd) and
+ * scales (n_pages, nkv, 64); a page holds 64 slots of every kv head.  page_table (B, max_pages) int32 on the device,
+ * shared by all layers: slot j of row b lives at slot j % 64 of page page_table[b][j / 64].  Rows may map the same page
+ * (a shared prompt prefix).  A page id outside [0, n_pages) -- the -1 of an unmapped entry, say -- follows the rule of a
+ * position outside the cache: it is never dereferenced, nothing is written through it, and every output of a token that
+ * would read or write a slot on that page is NaN.  Pages past the slots a launch reads or writes are not looked up.
+ * max_len is not read: it is max_pages * 64 everywhere it matters (decode chunking, grids, the workspace sizes of
+ * quip_decode_attention_workspace_bytes / quip_extend_attention_workspace_bytes), so a paged launch runs the contiguous
+ * launch's blocks and arithmetic: its results are bit-identical to the contiguous launch over the same cached bytes.
+ *
+ * Every operation checks the descriptor before it launches: k and v non-NULL and 16-byte aligned, the scales 4-byte
+ * aligned, hd in {64, 128}; paged: page_table 4-byte aligned, 0 < max_pages <= 2^31 / 64, n_pages > 0.  B below is the
+ * number of rows of the contiguous cache or of page_table. */
+typedef struct {
+  void* k;                 /* keys: the cache or the page pool */
+  void* v;                 /* values, of the same shape */
+  float* k_scale;          /* QUIP_KV_E4M3 only, else NULL */
+  float* v_scale;
+  int32_t* page_table;     /* NULL: contiguous.  Only quip_kv_beam_fork writes through it */
+  int32_t format;          /* QUIP_KV_FP16 or QUIP_KV_E4M3 */
+  int32_t nkv, hd;         /* kv heads, head dim */
+  int32_t max_len;         /* contiguous only: slots per row */
+  int32_t max_pages;       /* paged only: columns of page_table */
+  int32_t n_pages;         /* paged only: pages in each pool */
+} QuipKvCache;
+
+#define QUIP_KV_FP16 1
+#define QUIP_KV_E4M3 2
+
+/* One decode-attention step for B sequences, each at its own position, on one layer's KV cache kv.
+ *   q (B, nh, hd) fp16 with rotary applied; k_new / v_new (B, nkv, hd) fp16: this step's key / value; positions (B)
+ *   int64 on the device; out (B, nh, hd) fp16.
  * Writes k_new / v_new at slot positions[b] and returns
  *   out[b][h] = softmax_j(scale * q[b][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b],  G = nh / nkv,
  * reading no slot past positions[b].  fp32 scores, softmax and P.V; one fp16 rounding of the output.  The launch grid
- * depends on (B, nkv, max_len) only, so one captured graph serves every position.  hd in {64, 128}, nh % nkv == 0,
- * nh / nkv <= 8; all pointers 16-byte aligned; fp32 scratch from quip_decode_attention_workspace_bytes.  A position
+ * depends on (B, nkv, max_len) only, so one captured graph serves every position.  nh % nkv == 0, nh / nkv <= 8; q,
+ * k_new, v_new, out and workspace 16-byte aligned; fp32 scratch from quip_decode_attention_workspace_bytes.  A position
  * outside [0, max_len) leaves the cache untouched and gives a NaN output row.  Deterministic: bit-identical results from
  * run to run and for every other content of the other rows. */
-int quip_decode_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                          const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
-                          int32_t max_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+int quip_decode_attention(const QuipKvCache* kv, const void* q, const void* k_new, const void* v_new,
+                          const int64_t* positions, void* out, int32_t B, int32_t nh, float scale, void* workspace,
+                          size_t workspace_bytes, void* stream);
 int quip_decode_attention_workspace_bytes(int32_t B, int32_t nh, int32_t hd, int32_t max_len, size_t* out_bytes);
 
-/* The same step on an e4m3 KV cache: k_cache / v_cache (B, nkv, max_len, hd) e4m3fn bytes, k_scale / v_scale
- * (B, nkv, max_len) fp32, one scale per cached head vector x (hd values):
- *   amax = max_i |x_i|;  s = amax / 448 (IEEE fp32 division; s = 1 when amax == 0);  q_i = e4m3fn(x_i / s), round to
- *   nearest even, subnormals kept;  the vector's value is float(q_i) * s.
- * k_new / v_new (fp16) are quantized so, written with their scales at slot positions[b], and attended over as quantized
- * values like every other slot 0 .. positions[b].  No slot or scale past positions[b] is read.  Same grid, workspace
- * (quip_decode_attention_workspace_bytes) and determinism as quip_decode_attention; the scale pointers 4-byte aligned.
- * Non-finite inputs may give a NaN output row. */
-int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                              float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
-                              int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
-                              size_t workspace_bytes, void* stream);
-/* One attention step with T new tokens per row (speculative verification), each row at its own position, on one layer
- * of the static KV cache.  q (B, T, nh, hd) fp16 token-major, rotary applied; k_new / v_new (B, T, nkv, hd) fp16;
- * caches (B, nkv, max_len, hd); positions (B) int64 on the device; out (B, T, nh, hd) fp16.  Token i of row b is written
- * at slot positions[b] + i, and
+/* One attention step with T new tokens per row (speculative verification), each row at its own position, on one layer's
+ * KV cache kv.  q (B, T, nh, hd) fp16 token-major, rotary applied; k_new / v_new (B, T, nkv, hd) fp16; positions (B)
+ * int64 on the device; out (B, T, nh, hd) fp16.  Token i of row b is written at slot positions[b] + i, and
  *   out[b][i][h] = softmax_j(scale * q[b][i][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b] + i,
  * causal inside the new tokens.  No slot past positions[b] + T - 1 is read.  Scores and softmax in fp32; Q.K^T and P.V
  * on tensor cores (fp16 operands, fp32 accumulation; p rounded once to fp16); one fp16 rounding of the output.  1 <= T
- * <= 8, hd in {64, 128}, nh % nkv == 0, nh / nkv <= 8; pointers 16-byte aligned; fp32 scratch from
+ * <= 8, nh % nkv == 0, nh / nkv <= 8; pointers 16-byte aligned; fp32 scratch from
  * quip_extend_attention_workspace_bytes.  The grid depends on (B, T, nkv, max_len) only.  A row with positions[b] < 0
  * or positions[b] + T > max_len writes nothing and gets NaN outputs.  Deterministic, and a row's result does not depend
- * on the other rows.  T = 1 computes what quip_decode_attention does, to within its rounding of p. */
-int quip_extend_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                          const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
-                          int32_t max_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+ * on the other rows.  T = 1 computes what quip_decode_attention does, to within its rounding of p.  e4m3: a slot's k
+ * scale multiplies its score column; its v scale multiplies p before p is rounded to fp16 (normalised by the chunk's
+ * largest v scale, which multiplies the chunk's P.V). */
+int quip_extend_attention(const QuipKvCache* kv, const void* q, const void* k_new, const void* v_new,
+                          const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, float scale,
+                          void* workspace, size_t workspace_bytes, void* stream);
 int quip_extend_attention_workspace_bytes(int32_t B, int32_t T, int32_t nh, int32_t hd, int32_t max_len,
                                           size_t* out_bytes);
-/* The same on an e4m3 cache with per-slot scales (the format of quip_decode_attention_fp8): the new keys and values are
- * quantized on append and attended over as quantized values.  A slot's k scale multiplies its score column; its v scale
- * multiplies p before p is rounded to fp16 (normalised by the chunk's largest v scale, which multiplies the chunk's
- * P.V). */
-int quip_extend_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                              float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t T,
-                              int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
-                              size_t workspace_bytes, void* stream);
 
 /* Prompt-lookup drafts.  hist (B, max_len) int64 holds each row's tokens by position; the current token is at
  * c = positions[b].  For e < c let L(e) be the length of the common suffix of hist[b, ..e] and hist[b, ..c], capped at
@@ -204,100 +227,43 @@ int quip_spec_accept(const int64_t* tokens, const int64_t* targets, int64_t* gen
                      int64_t* positions, int64_t* n_gen, int64_t* accepted, int32_t B, int32_t T, int32_t max_new,
                      int32_t gen_cols, int32_t max_len, void* stream);
 
-/* Prefill of an e4m3 cache: src (B, nkv, P, hd) fp16 quantized as above into slots 0 .. P-1 of cache
- * (B, nkv, max_len, hd) e4m3fn and scales (B, nkv, max_len) fp32; slots >= P are not touched.  hd in {64, 128},
+/* Prefill of an e4m3 cache: src (B, nkv, P, hd) fp16 quantized by the rule of QuipKvCache into slots 0 .. P-1 of
+ * cache (B, nkv, max_len, hd) e4m3fn and scales (B, nkv, max_len) fp32; slots >= P are not touched.  hd in {64, 128},
  * P <= max_len; src and cache 16-byte aligned, scales 4-byte aligned. */
 int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,
                          int32_t max_len, int32_t hd, void* stream);
 
-/* Chunked prefill, part 1: append a chunk of new keys and values to one layer of the static KV cache.  k_new / v_new
- * (B, T, nkv, hd) fp16 token-major; caches (B, nkv, max_len, hd) fp16; positions, counts (B) int64 on the device.  Token
- * i of row b goes to slot positions[b] + i for i < counts[b]; no other slot, and nothing of a row with counts[b] == 0, is
- * touched.  A row with positions[b] < 0, counts[b] outside [0, T] or positions[b] + counts[b] > max_len writes nothing.
- * 1 <= T <= max_len, hd in {64, 128}; pointers 16-byte aligned. */
-int quip_kv_append(const void* k_new, const void* v_new, void* k_cache, void* v_cache, const int64_t* positions,
-                   const int64_t* counts, int32_t B, int32_t T, int32_t nkv, int32_t hd, int32_t max_len, void* stream);
-/* The same into an e4m3 cache: each new head vector is quantized by the rule of quip_decode_attention_fp8 (amax / 448,
- * round to nearest even, subnormals kept) and stored with its fp32 scale in k_scale / v_scale (B, nkv, max_len). */
-int quip_kv_append_fp8(const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
-                       float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T,
-                       int32_t nkv, int32_t hd, int32_t max_len, void* stream);
+/* Chunked prefill, part 1: append a chunk of new keys and values to one layer's KV cache kv.  k_new / v_new
+ * (B, T, nkv, hd) fp16 token-major; positions, counts (B) int64 on the device.  Token i of row b goes to slot
+ * positions[b] + i for i < counts[b]; no other slot, and nothing of a row with counts[b] == 0, is touched.  A row with
+ * positions[b] < 0, counts[b] outside [0, T] or positions[b] + counts[b] > max_len writes nothing.  1 <= T <= max_len;
+ * pointers 16-byte aligned. */
+int quip_kv_append(const QuipKvCache* kv, const void* k_new, const void* v_new, const int64_t* positions,
+                   const int64_t* counts, int32_t B, int32_t T, void* stream);
 /* Chunked prefill, part 2: causal attention of a chunk of T query tokens per row over the cache that already holds the
  * chunk (quip_kv_append first).  q (B, T, nh, hd) fp16 token-major, rotary applied; out (B, T, nh, hd) fp16.  For
  * i < counts[b]
  *   out[b][i][h] = softmax_j(scale * q[b][i][h] . k[b][h / G][j]) v[b][h / G][j],  j = 0 .. positions[b] + i,
  * and out[b][i] = 0 for counts[b] <= i < T.  No slot past positions[b] + counts[b] - 1 is read.  Flash-attention style:
  * Q.K^T and P.V on tensor cores (fp16 operands, fp32 accumulation), online softmax in fp32, p rounded once to fp16 per
- * 64-slot block, one fp16 rounding of the output; no workspace.  1 <= T <= max_len, hd in {64, 128}, nh % nkv == 0,
- * nh / nkv <= 8; pointers 16-byte aligned.  A row with positions[b] < 0, counts[b] outside [0, T] or positions[b] +
- * counts[b] > max_len gets NaN outputs.  Deterministic, and a row's result does not depend on the other rows.  At T <= 8
- * it computes what quip_extend_attention does, to within the rounding of p. */
-int quip_prefill_attention(const void* q, const void* k_cache, const void* v_cache, const int64_t* positions,
-                           const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
-                           int32_t max_len, float scale, void* stream);
-/* The same over an e4m3 cache with per-slot scales (scale pointers 4-byte aligned).  A chunk attends over the quantized
- * values the cache holds, its own keys and values included (quip_kv_append_fp8 wrote them): the values every later
- * decode step reads back, the rule of quip_decode_attention_fp8 and quip_extend_attention_fp8.  (Filling the cache by
- * quip_kv_quantize_fp8 after an fp16 forward instead attends in fp16 and rounds afterwards.)  Per 64-slot block, a
- * slot's k scale multiplies its score column; its v scale multiplies p before p is rounded to fp16, normalised by the
- * largest v scale among the query row's visible slots of the block, which multiplies the block's P.V. */
-int quip_prefill_attention_fp8(const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
-                               const float* v_scale, const int64_t* positions, const int64_t* counts, void* out,
-                               int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale,
-                               void* stream);
+ * 64-slot block, one fp16 rounding of the output; no workspace.  1 <= T <= max_len, nh % nkv == 0, nh / nkv <= 8;
+ * pointers 16-byte aligned.  A row with positions[b] < 0, counts[b] outside [0, T] or positions[b] + counts[b] > max_len
+ * gets NaN outputs.  Deterministic, and a row's result does not depend on the other rows.  At T <= 8 it computes what
+ * quip_extend_attention does, to within the rounding of p.
+ * e4m3: a chunk attends over the quantized values the cache holds, its own keys and values included (quip_kv_append
+ * wrote them): the values every later decode step reads back, the rule of quip_decode_attention and
+ * quip_extend_attention.  (Filling the cache by quip_kv_quantize_fp8 after an fp16 forward instead attends in fp16 and
+ * rounds afterwards.)  Per 64-slot block, a slot's k scale multiplies its score column; its v scale multiplies p before
+ * p is rounded to fp16, normalised by the largest v scale among the query row's visible slots of the block, which
+ * multiplies the block's P.V. */
+int quip_prefill_attention(const QuipKvCache* kv, const void* q, const int64_t* positions, const int64_t* counts,
+                           void* out, int32_t B, int32_t T, int32_t nh, float scale, void* stream);
 
-/* Paged KV cache.  Per layer, k_pool / v_pool (n_pages, nkv, 64, hd) hold fp16 or e4m3fn values (e4m3: with k_scale /
- * v_scale (n_pages, nkv, 64) fp32, the format of quip_decode_attention_fp8); a page holds 64 slots of every kv head.
- * page_table (B, max_pages) int32 on the device, shared by all layers: slot j of row b lives at slot j % 64 of page
- * page_table[b][j / 64].  Rows may map the same page (a shared prompt prefix).  A page id outside [0, n_pages) -- the
- * -1 of an unmapped entry, say -- follows the rule of a position outside the cache: it is never dereferenced, nothing
- * is written through it, and every output of a token that would read or write a slot on that page is NaN.  Pages past
- * the slots a launch reads or writes are not looked up.
- *
- * Each entry point below takes the arguments of its contiguous twin with the caches replaced by the pools and max_len by
- * (page_table, max_pages, n_pages); max_len = max_pages * 64 everywhere it mattered (decode chunking, grids, the
- * workspace sizes of quip_decode_attention_workspace_bytes / quip_extend_attention_workspace_bytes), so a paged launch
- * runs the contiguous launch's blocks and arithmetic: its results are bit-identical to the contiguous launch over the
- * same cached bytes.  page_table 4-byte aligned, 0 < max_pages <= 2^31 / 64, n_pages > 0. */
-int quip_decode_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
-                                float scale, void* workspace, size_t workspace_bytes, const int32_t* page_table,
-                                int32_t max_pages, int32_t n_pages, void* stream);
-int quip_decode_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                    float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
-                                    int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
-                                    size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
-                                    int32_t n_pages, void* stream);
-int quip_extend_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
-                                int32_t hd, float scale, void* workspace, size_t workspace_bytes,
-                                const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
-int quip_extend_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                    float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B,
-                                    int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
-                                    size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
-                                    int32_t n_pages, void* stream);
-int quip_kv_append_paged(const void* k_new, const void* v_new, void* k_pool, void* v_pool, const int64_t* positions,
-                         const int64_t* counts, int32_t B, int32_t T, int32_t nkv, int32_t hd,
-                         const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
-int quip_kv_append_paged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool, float* k_scale,
-                             float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T,
-                             int32_t nkv, int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                             void* stream);
-int quip_prefill_attention_paged(const void* q, const void* k_pool, const void* v_pool, const int64_t* positions,
-                                 const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
-                                 int32_t hd, float scale, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                 void* stream);
-int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale,
-                                     const float* v_scale, const int64_t* positions, const int64_t* counts, void* out,
-                                     int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale,
-                                     const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
-
-/* Ragged (packed) chunks over a paged cache: S sequences of different lengths back to back in N token rows, so a step
- * that mixes decode rows (one token each) and prompt chunks feeds no padding.  seq_start (S + 1) int64 on the device
- * holds offsets 0 <= seq_start[0] <= ... <= seq_start[S] <= N: token i of sequence s is packed row seq_start[s] + i, at
- * slot positions[s] + i (positions (S) int64) of row s of page_table (S, max_pages) -- the table rows of the S
- * sequences.  k_new / v_new are (N, nkv, hd), q / out (N, nh, hd), fp16 token-major; the pools and scales as above.
+/* Ragged (packed) chunks over a paged cache (kv must have a page_table): S sequences of different lengths back to back
+ * in N token rows, so a step that mixes decode rows (one token each) and prompt chunks feeds no padding.  seq_start
+ * (S + 1) int64 on the device holds offsets 0 <= seq_start[0] <= ... <= seq_start[S] <= N: token i of sequence s is
+ * packed row seq_start[s] + i, at slot positions[s] + i (positions (S) int64) of row s of page_table (S, max_pages) --
+ * the table rows of the S sequences.  k_new / v_new are (N, nkv, hd), q / out (N, nh, hd), fp16 token-major.
  * max_count >= 1 bounds every sequence's length (the attention grid is (query tile, kv head, sequence) with
  * ceil(G * max_count / 64) tiles; a tile past its sequence's length exits at once).
  *
@@ -306,26 +272,15 @@ int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const vo
  * A sequence whose offsets break the order above or leave [0, N] is not looked at: nothing is read or written for it.
  * There are no padding rows: out rows outside every sequence are not written.
  *
- * The rule: per sequence s, the ragged launch is bit-identical to the paged launch (quip_kv_append_paged(_fp8),
- * quip_prefill_attention_paged(_fp8)) with B = S, T = max_count, counts[s] = seq_start[s + 1] - seq_start[s] and row s
- * of the padded q / k_new / v_new holding the sequence's tokens, over the same cached bytes: each sequence runs the same
- * query tiles, 64-slot blocks and arithmetic, and only the addressing of the packed rows differs. */
-int quip_kv_append_ragged(const void* k_new, const void* v_new, void* k_pool, void* v_pool, const int64_t* seq_start,
-                          const int64_t* positions, int32_t S, int32_t N, int32_t max_count, int32_t nkv, int32_t hd,
-                          const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream);
-int quip_kv_append_ragged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool, float* k_scale,
-                              float* v_scale, const int64_t* seq_start, const int64_t* positions, int32_t S, int32_t N,
-                              int32_t max_count, int32_t nkv, int32_t hd, const int32_t* page_table, int32_t max_pages,
-                              int32_t n_pages, void* stream);
-int quip_prefill_attention_ragged(const void* q, const void* k_pool, const void* v_pool, const int64_t* seq_start,
+ * The rule: per sequence s, the ragged launch is bit-identical to the padded launch (quip_kv_append,
+ * quip_prefill_attention) on the same paged cache with B = S, T = max_count, counts[s] = seq_start[s + 1] - seq_start[s]
+ * and row s of the padded q / k_new / v_new holding the sequence's tokens, over the same cached bytes: each sequence runs
+ * the same query tiles, 64-slot blocks and arithmetic, and only the addressing of the packed rows differs. */
+int quip_kv_append_ragged(const QuipKvCache* kv, const void* k_new, const void* v_new, const int64_t* seq_start,
+                          const int64_t* positions, int32_t S, int32_t N, int32_t max_count, void* stream);
+int quip_prefill_attention_ragged(const QuipKvCache* kv, const void* q, const int64_t* seq_start,
                                   const int64_t* positions, void* out, int32_t S, int32_t N, int32_t max_count,
-                                  int32_t nh, int32_t nkv, int32_t hd, float scale, const int32_t* page_table,
-                                  int32_t max_pages, int32_t n_pages, void* stream);
-int quip_prefill_attention_ragged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale,
-                                      const float* v_scale, const int64_t* seq_start, const int64_t* positions,
-                                      void* out, int32_t S, int32_t N, int32_t max_count, int32_t nh, int32_t nkv,
-                                      int32_t hd, float scale, const int32_t* page_table, int32_t max_pages,
-                                      int32_t n_pages, void* stream);
+                                  int32_t nh, float scale, void* stream);
 
 /* Token selection of one generation step: for each row b of logits (B, V) fp16 contiguous (rows need no alignment),
  * with T = temperature[b], k = top_k[b], p = top_p[b] and s = seed[b] (each (B), device) and t = *step (device; the
@@ -445,13 +400,14 @@ int quip_logits_process(void* logits, int64_t ld, int32_t R, int32_t T, int32_t 
  * early_stopping: 0 False, 1 True, 2 'never'.  Histories are (B, K, max_new) int64, fin_tmp / hist_tmp scratch of
  * that shape.  One CTA per prompt; everything is read from device memory, so one captured graph serves every step.
  *
- * quip_kv_beam_fork(_fp8): after a select, with len = lens[r] (the slots row r has filled, the last at pos = len - 1,
+ * quip_kv_beam_fork: after a select, with len = lens[r] (the slots row r has filled, the last at pos = len - 1,
  * cur = pos / 64) and p = parents[r] != r: table[r, :cur] = the old table[p, :cur] (read from table_tmp, a copy made by
  * the first phase, so rows may swap); slots 64 * cur .. pos of row p's current page are copied (every layer, k and v,
  * and on e4m3 pools their scales) into row r's current page, through scratch page scratch0 + r in two phases (gather
- * every parent, then scatter), so cycles and fan-out are safe.  Pools (L, n_pages, nkv, 64, hd) (scales
- * (L, n_pages, nkv, 64)), 16-byte aligned, hd * element size % 16 == 0; scratch0 + R <= n_pages.  A page id outside
- * [0, n_pages) is never dereferenced; rows with p == r or p outside [0, R) change nothing.  Two launches. */
+ * every parent, then scatter), so cycles and fan-out are safe.  kv describes layer 0 of L layers of paged pools
+ * (L, n_pages, nkv, 64, hd) (scales (L, n_pages, nkv, 64)); table is its page_table (R, max_pages), which the fork
+ * writes, and table_tmp scratch of that shape.  scratch0 + R <= n_pages.  A page id outside [0, n_pages) is never
+ * dereferenced; rows with p == r or p outside [0, R) change nothing.  Two launches. */
 int quip_beam_candidates(const void* logits, int64_t ld, const float* scores, float* cand_s, int32_t* cand_i,
                          int32_t R, int32_t V, int32_t K, int32_t C, void* stream);
 int quip_beam_select(const float* cand_s, const int32_t* cand_i, const int64_t* eos, int32_t n_eos,
@@ -460,12 +416,8 @@ int quip_beam_select(const float* cand_s, const int32_t* cand_i, const int64_t* 
                      uint8_t* fin_filled, uint8_t* heur, uint8_t* done, int64_t* tokens, int64_t* parents,
                      int64_t* adv, int32_t B, int32_t K, int32_t C, int32_t V, int32_t max_new,
                      int32_t early_stopping, int32_t never_long, void* stream);
-int quip_kv_beam_fork(void* k_pool, void* v_pool, int32_t* table, int32_t* table_tmp, const int64_t* parents,
-                      const int64_t* lens, int32_t R, int32_t L, int32_t n_pages, int32_t nkv, int32_t hd,
-                      int32_t max_pages, int32_t scratch0, void* stream);
-int quip_kv_beam_fork_fp8(void* k_pool, void* v_pool, float* k_scale, float* v_scale, int32_t* table,
-                          int32_t* table_tmp, const int64_t* parents, const int64_t* lens, int32_t R, int32_t L,
-                          int32_t n_pages, int32_t nkv, int32_t hd, int32_t max_pages, int32_t scratch0, void* stream);
+int quip_kv_beam_fork(const QuipKvCache* kv, int32_t L, int32_t* table_tmp, const int64_t* parents,
+                      const int64_t* lens, int32_t R, int32_t scratch0, void* stream);
 
 /* Signature-compatible replacement of the reference's own native call (quant_cuda.vecquant3matmul quant.py:229-230,
  * vecquant4matmul zeroShot/models/quant.py:207-208): ONE token, fp32, on the REFERENCE's packed layout

@@ -1,6 +1,6 @@
 """Exactly representable cases for the decode-attention kernels.  TEST INFRASTRUCTURE ONLY.
 
-The kernels are quip_decode_attention and quip_decode_attention_fp8 (csrc/attn_decode.cu).  Softmax is not exact in
+The kernels are quip_decode_attention's, on fp16 and e4m3 caches (csrc/attn_decode.cu).  Softmax is not exact in
 general, because expf is not correctly rounded.  It is exact when every score of a head either equals the head's maximum
 bit for bit or lies at least DELTA = 128 below it: expf(0) = 1, and e^-128 ~ 2.6e-56 is far below the smallest fp32
 subnormal 2^-149 ~ 1.4e-45, so expf(x <= -128) = 0.  Attention then returns exactly the mean of the V rows of the

@@ -1,7 +1,7 @@
 """Exactly representable multi-token cases for the extend- and prefill-attention kernels.  TEST INFRASTRUCTURE ONLY.
 
-The kernels are quip_extend_attention(_fp8) (csrc/attn_decode.cu: attn_extend_split_kernel and the multi-token
-combine) and quip_kv_append(_fp8) followed by quip_prefill_attention(_fp8) (csrc/attn_prefill.cu).  Token i of row b
+The kernels are quip_extend_attention's (csrc/attn_decode.cu: attn_extend_split_kernel and the multi-token
+combine) and quip_kv_append followed by quip_prefill_attention (csrc/attn_prefill.cu), on fp16 and e4m3 caches.  Token i of row b
 attends over slots 0 .. positions[b] + i.  The premise is the one of oracle/exact_attn.py, per (row, token): when
 every score a token sees either equals its maximum bit for bit or lies at least DELTA = 128 below it, expf gives
 exactly 1 or 0, and attention returns the mean of the V rows of the token's visible selected slots.  In detail:

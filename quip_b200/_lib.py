@@ -13,7 +13,7 @@ QUIP_FLAG_SYMMETRIC = 1
 WS_HEADER_BYTES = 16 * 1024
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class QuipPass(C.Structure):
@@ -30,6 +30,18 @@ class QuipLinearDesc(C.Structure):
     _fields_ = [('K', C.c_int32), ('N', C.c_int32), ('bits', C.c_int32), ('flags', C.c_int32),
                 ('qweight', C.c_void_p), ('scales', C.c_void_p), ('zeros', C.c_void_p), ('bias', C.c_void_p),
                 ('inv_scale', C.c_void_p), ('V', QuipSide), ('U', QuipSide)]
+
+
+QUIP_KV_FP16, QUIP_KV_E4M3 = 1, 2
+
+
+class QuipKvCache(C.Structure):
+    _fields_ = [('k', C.c_void_p), ('v', C.c_void_p), ('k_scale', C.c_void_p), ('v_scale', C.c_void_p),
+                ('page_table', C.c_void_p), ('format', C.c_int32), ('nkv', C.c_int32), ('hd', C.c_int32),
+                ('max_len', C.c_int32), ('max_pages', C.c_int32), ('n_pages', C.c_int32)]
+
+
+_KV = C.POINTER(QuipKvCache)
 
 
 # name -> (restype, argtypes); every symbol include/quip_b200.h declares
@@ -56,68 +68,25 @@ EXPORTS = {
     'quip_greedy_block': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     'quip_hessian_accumulate': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
     'quip_silu_mul_gather': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
-    'quip_decode_attention': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
-                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+    'quip_decode_attention': (C.c_int, [_KV] + [C.c_void_p] * 5 + [C.c_int32] * 2 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                   C.c_void_p]),
+    'quip_extend_attention': (C.c_int, [_KV] + [C.c_void_p] * 5 + [C.c_int32] * 3 + [C.c_float, C.c_void_p, C.c_size_t,
+                                                                                   C.c_void_p]),
+    'quip_kv_append': (C.c_int, [_KV] + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]),
+    'quip_prefill_attention': (C.c_int, [_KV] + [C.c_void_p] * 4 + [C.c_int32] * 3 + [C.c_float, C.c_void_p]),
+    'quip_kv_append_ragged': (C.c_int, [_KV] + [C.c_void_p] * 4 + [C.c_int32] * 3 + [C.c_void_p]),
+    'quip_prefill_attention_ragged': (C.c_int, [_KV] + [C.c_void_p] * 4 + [C.c_int32] * 4 + [C.c_float, C.c_void_p]),
+    'quip_kv_beam_fork': (C.c_int, [_KV, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 2 + [C.c_void_p]),
     'quip_decode_attention_workspace_bytes': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                         C.POINTER(C.c_size_t)]),
-    'quip_decode_attention_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                            C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     'quip_kv_quantize_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, C.c_void_p]),
     'quip_sample': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_int32, C.c_int32, C.c_void_p]),
     'quip_sample_at': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
-    'quip_extend_attention': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                        C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     'quip_extend_attention_workspace_bytes': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                         C.POINTER(C.c_size_t)]),
-    'quip_extend_attention_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                            C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_size_t,
-                                            C.c_void_p]),
-    'quip_kv_append': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                 C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
-    'quip_kv_append_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                     C.c_void_p]),
-    'quip_prefill_attention': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
-                                         C.c_void_p]),
-    'quip_prefill_attention_fp8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                             C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                             C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
-    'quip_decode_attention_paged': (C.c_int, [C.c_void_p] * 7 + [C.c_int32] * 4 + [C.c_float, C.c_void_p, C.c_size_t,
-                                                                                  C.c_void_p, C.c_int32, C.c_int32,
-                                                                                  C.c_void_p]),
-    'quip_decode_attention_paged_fp8': (C.c_int, [C.c_void_p] * 9 + [C.c_int32] * 4 + [C.c_float, C.c_void_p, C.c_size_t,
-                                                                                      C.c_void_p, C.c_int32, C.c_int32,
-                                                                                      C.c_void_p]),
-    'quip_extend_attention_paged': (C.c_int, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_size_t,
-                                                                                  C.c_void_p, C.c_int32, C.c_int32,
-                                                                                  C.c_void_p]),
-    'quip_extend_attention_paged_fp8': (C.c_int, [C.c_void_p] * 9 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_size_t,
-                                                                                      C.c_void_p, C.c_int32, C.c_int32,
-                                                                                      C.c_void_p]),
-    'quip_kv_append_paged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
-    'quip_kv_append_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_int32,
-                                                                               C.c_void_p]),
-    'quip_prefill_attention_paged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
-                                                                                   C.c_int32, C.c_void_p]),
-    'quip_prefill_attention_paged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32,
-                                                                                       C.c_int32, C.c_void_p]),
-    'quip_kv_append_ragged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.c_int32,
-                                                                            C.c_void_p]),
-    'quip_kv_append_ragged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.c_int32,
-                                                                                C.c_void_p]),
-    'quip_prefill_attention_ragged': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 6 + [C.c_float, C.c_void_p, C.c_int32,
-                                                                                    C.c_int32, C.c_void_p]),
-    'quip_prefill_attention_ragged_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 6 + [C.c_float, C.c_void_p,
-                                                                                        C.c_int32, C.c_int32,
-                                                                                        C.c_void_p]),
     'quip_token_logprobs': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_void_p]),
     'quip_token_topk_logprobs': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_int32] * 3 + [C.c_void_p] * 3 +
@@ -125,8 +94,6 @@ EXPORTS = {
     'quip_beam_candidates':(C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 4 +
                              [C.c_void_p]),
     'quip_beam_select': (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 16 + [C.c_int32] * 7 + [C.c_void_p]),
-    'quip_kv_beam_fork': (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 7 + [C.c_void_p]),
-    'quip_kv_beam_fork_fp8': (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 7 + [C.c_void_p]),
     'quip_logits_process': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_int32] * 3 + [C.c_void_p] * 9 + [C.c_int32] +
                             [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p]),
     'quip_ngram_draft':(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

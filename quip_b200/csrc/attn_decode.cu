@@ -657,36 +657,26 @@ void launch_split_g(int G, dim3 grid, cudaStream_t st, const void* q, const void
 #undef AD_LAUNCH
 }
 
-bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
 size_t ws_bytes(int64_t B, int64_t nh, int64_t hd, int64_t nsplit) {
   const size_t o = (size_t)(B * nh * nsplit * hd) * sizeof(float);
   return ((o + 255) & ~(size_t)255) + (size_t)(B * nh * nsplit * 2) * sizeof(float);
 }
 
-// Argument checks and launches of quip_decode_attention (FP8 false) and quip_decode_attention_fp8 (FP8 true), and of
-// their paged twins (PAGED true: k_cache / v_cache and the scales are page pools, max_len = max_pages * 64); fn names
-// the entry point in the messages.
-template <bool FP8, bool PAGED = false>
-int decode_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                     float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t nh,
-                     int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
-                     void* stream, KvPages pg = {}) {
-  QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
-                 "%s: null pointer", fn);
-  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
-  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
-                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
-                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
+// Argument checks and launches of quip_decode_attention on a cache kv_check accepted (FP8: e4m3; PAGED: the caches
+// and scales are page pools behind pg, max_len = max_pages * 64); fn names the entry point in the messages.
+template <bool FP8, bool PAGED>
+int decode_attention(const char* fn, const QuipKvCache& kv, KvPages pg, int32_t max_len, const void* q,
+                     const void* k_new, const void* v_new, const int64_t* positions, void* out, int32_t B, int32_t nh,
+                     float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  const int32_t nkv = kv.nkv, hd = kv.hd;
+  QUIP_CHECK_ARG(q && k_new && v_new && positions && out && workspace, "%s: null pointer", fn);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
   QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
                  "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head",
                  fn, nh, nkv, AD_MAXG);
-  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache) && al16(out) && al16(workspace),
+  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(out) && al16(workspace),
                  "%s: pointers must be 16-byte aligned", fn);
-  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
   const int chunk = (int64_t)B * nkv * ceil_div(max_len, AD_CHUNK) < AD_SMALL_GRID ? AD_SMALL_CHUNK : AD_CHUNK;
   const int nsplit = ceil_div(max_len, chunk);
   const size_t need = ws_bytes(B, nh, hd, nsplit);
@@ -697,8 +687,8 @@ int decode_attention(const char* fn, const void* q, const void* k_new, const voi
   const cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(nsplit, nkv, B);
   const int G = nh / nkv;
-  if (hd == 64) launch_split_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
-  else launch_split_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
+  if (hd == 64) launch_split_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
+  else launch_split_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, chunk, scale);
   QUIP_LAUNCHED("attn_decode_split_kernel");
   attn_decode_combine_kernel<<<(unsigned)(B * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd, max_len, nsplit, chunk, 1);
   QUIP_LAUNCHED("attn_decode_combine_kernel");
@@ -738,28 +728,21 @@ int launch_extend_g(int G, dim3 grid, cudaStream_t st, const void* q, const void
 #undef AX_LAUNCH
 }
 
-// Argument checks and launches of quip_extend_attention (FP8 false) and quip_extend_attention_fp8 (FP8 true), and of
-// their paged twins.
-template <bool FP8, bool PAGED = false>
-int extend_attention(const char* fn, const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                     float* k_scale, float* v_scale, const int64_t* positions, void* out, int32_t B, int32_t T,
-                     int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* workspace,
-                     size_t workspace_bytes, void* stream, KvPages pg = {}) {
-  QUIP_CHECK_ARG(q && k_new && v_new && k_cache && v_cache && positions && out && workspace && (!FP8 || (k_scale && v_scale)),
-                 "%s: null pointer", fn);
-  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
-  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
-                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
-                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
+// Argument checks and launches of quip_extend_attention on a cache kv_check accepted, as decode_attention.
+template <bool FP8, bool PAGED>
+int extend_attention(const char* fn, const QuipKvCache& kv, KvPages pg, int32_t max_len, const void* q,
+                     const void* k_new, const void* v_new, const int64_t* positions, void* out, int32_t B, int32_t T,
+                     int32_t nh, float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  const int32_t nkv = kv.nkv, hd = kv.hd;
+  QUIP_CHECK_ARG(q && k_new && v_new && positions && out && workspace, "%s: null pointer", fn);
   QUIP_CHECK_ARG(T >= 1 && T <= AX_MAXT, "%s: %d tokens per row: need 1 <= T <= %d", fn, T, AX_MAXT);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d)", fn, B, nh, nkv, max_len);
   QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= AD_MAXG,
                  "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head",
                  fn, nh, nkv, AD_MAXG);
-  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache) && al16(out) && al16(workspace),
+  QUIP_CHECK_ARG(al16(q) && al16(k_new) && al16(v_new) && al16(out) && al16(workspace),
                  "%s: pointers must be 16-byte aligned", fn);
-  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
   const int nsplit = ceil_div(max_len, AX_CHUNK);
   const size_t need = ws_bytes((int64_t)B * T, nh, hd, nsplit);
   QUIP_CHECK_ARG(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
@@ -770,8 +753,8 @@ int extend_attention(const char* fn, const void* q, const void* k_new, const voi
   const dim3 grid(nsplit, nkv, B);
   const int G = nh / nkv;
   const int e = hd == 64
-      ? launch_extend_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale)
-      : launch_extend_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale);
+      ? launch_extend_g<FP8, PAGED, 64>(G, grid, st, q, k_new, v_new, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale)
+      : launch_extend_g<FP8, PAGED, 128>(G, grid, st, q, k_new, v_new, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, po, pml, pg, nh, nkv, max_len, nsplit, T, scale);
   if (e != QUIP_OK) return e;
   attn_decode_combine_kernel<<<(unsigned)((int64_t)B * T * nh), hd, 0, st>>>(po, pml, positions, (__half*)out, nh, hd,
                                                                              max_len, nsplit, AX_CHUNK, T);
@@ -794,20 +777,18 @@ extern "C" int quip_decode_attention_workspace_bytes(int32_t B, int32_t nh, int3
   return QUIP_OK;
 }
 
-extern "C" int quip_decode_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                                     const int64_t* positions, void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd,
-                                     int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
-                                     void* stream) {
-  return decode_attention<false>("quip_decode_attention", q, k_new, v_new, k_cache, v_cache, nullptr, nullptr, positions,
-                                 out, B, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
-}
-
-extern "C" int quip_decode_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache,
-                                         void* v_cache, float* k_scale, float* v_scale, const int64_t* positions,
-                                         void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len,
-                                         float scale, void* workspace, size_t workspace_bytes, void* stream) {
-  return decode_attention<true>("quip_decode_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
-                                positions, out, B, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
+extern "C" int quip_decode_attention(const QuipKvCache* kv, const void* q, const void* k_new, const void* v_new,
+                                     const int64_t* positions, void* out, int32_t B, int32_t nh, float scale,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "quip_decode_attention";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  return kv_dispatch(*kv, [&](auto fp8, auto paged) {
+    return decode_attention<decltype(fp8)::value, decltype(paged)::value>(fn, *kv, pg, max_len, q, k_new, v_new,
+                                                                        positions, out, B, nh, scale, workspace,
+                                                                        workspace_bytes, stream);
+  });
 }
 
 extern "C" int quip_extend_attention_workspace_bytes(int32_t B, int32_t T, int32_t nh, int32_t hd, int32_t max_len,
@@ -820,63 +801,18 @@ extern "C" int quip_extend_attention_workspace_bytes(int32_t B, int32_t T, int32
   return QUIP_OK;
 }
 
-extern "C" int quip_extend_attention(const void* q, const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                                     const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
-                                     int32_t hd, int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
-                                     void* stream) {
-  return extend_attention<false>("quip_extend_attention", q, k_new, v_new, k_cache, v_cache, nullptr, nullptr, positions,
-                                 out, B, T, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
-}
-
-extern "C" int quip_extend_attention_fp8(const void* q, const void* k_new, const void* v_new, void* k_cache,
-                                         void* v_cache, float* k_scale, float* v_scale, const int64_t* positions,
-                                         void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
-                                         int32_t max_len, float scale, void* workspace, size_t workspace_bytes,
-                                         void* stream) {
-  return extend_attention<true>("quip_extend_attention_fp8", q, k_new, v_new, k_cache, v_cache, k_scale, v_scale,
-                                positions, out, B, T, nh, nkv, hd, max_len, scale, workspace, workspace_bytes, stream);
-}
-
-// Paged twins: max_len = max_pages * 64 everywhere (chunking, grid, workspace), so a paged launch runs the contiguous
-// launch's chunking on the same shape.
-extern "C" int quip_decode_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool,
-                                           void* v_pool, const int64_t* positions, void* out, int32_t B, int32_t nh,
-                                           int32_t nkv, int32_t hd, float scale, void* workspace, size_t workspace_bytes,
-                                           const int32_t* page_table, int32_t max_pages, int32_t n_pages, void* stream) {
-  return decode_attention<false, true>("quip_decode_attention_paged", q, k_new, v_new, k_pool, v_pool, nullptr, nullptr,
-                                       positions, out, B, nh, nkv, hd, paged_len(max_pages), scale, workspace,
-                                       workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_decode_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool,
-                                               void* v_pool, float* k_scale, float* v_scale, const int64_t* positions,
-                                               void* out, int32_t B, int32_t nh, int32_t nkv, int32_t hd, float scale,
-                                               void* workspace, size_t workspace_bytes, const int32_t* page_table,
-                                               int32_t max_pages, int32_t n_pages, void* stream) {
-  return decode_attention<true, true>("quip_decode_attention_paged_fp8", q, k_new, v_new, k_pool, v_pool, k_scale,
-                                      v_scale, positions, out, B, nh, nkv, hd, paged_len(max_pages), scale, workspace,
-                                      workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_extend_attention_paged(const void* q, const void* k_new, const void* v_new, void* k_pool,
-                                           void* v_pool, const int64_t* positions, void* out, int32_t B, int32_t T,
-                                           int32_t nh, int32_t nkv, int32_t hd, float scale, void* workspace,
-                                           size_t workspace_bytes, const int32_t* page_table, int32_t max_pages,
-                                           int32_t n_pages, void* stream) {
-  return extend_attention<false, true>("quip_extend_attention_paged", q, k_new, v_new, k_pool, v_pool, nullptr, nullptr,
-                                       positions, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, workspace,
-                                       workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_extend_attention_paged_fp8(const void* q, const void* k_new, const void* v_new, void* k_pool,
-                                               void* v_pool, float* k_scale, float* v_scale, const int64_t* positions,
-                                               void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
-                                               float scale, void* workspace, size_t workspace_bytes,
-                                               const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                               void* stream) {
-  return extend_attention<true, true>("quip_extend_attention_paged_fp8", q, k_new, v_new, k_pool, v_pool, k_scale,
-                                      v_scale, positions, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, workspace,
-                                      workspace_bytes, stream, KvPages{page_table, max_pages, n_pages});
+extern "C" int quip_extend_attention(const QuipKvCache* kv, const void* q, const void* k_new, const void* v_new,
+                                     const int64_t* positions, void* out, int32_t B, int32_t T, int32_t nh, float scale,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "quip_extend_attention";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  return kv_dispatch(*kv, [&](auto fp8, auto paged) {
+    return extend_attention<decltype(fp8)::value, decltype(paged)::value>(fn, *kv, pg, max_len, q, k_new, v_new,
+                                                                        positions, out, B, T, nh, scale, workspace,
+                                                                        workspace_bytes, stream);
+  });
 }
 
 extern "C" int quip_kv_quantize_fp8(const void* src, void* cache, float* scales, int32_t B, int32_t nkv, int32_t P,

@@ -2,9 +2,9 @@
 // position, attending causally over the cache itself (one layer: k_cache / v_cache (B, nkv, max_len, hd), fp16 or e4m3
 // with per-slot fp32 scales).  Two launches per layer:
 //
-//   quip_kv_append(_fp8)          token i < counts[b] of row b to slot positions[b] + i (e4m3: quantized on the way);
-//   quip_prefill_attention(_fp8)  out[b][i][h] = softmax_j(scale * q[b][i][h] . K[b][h/G][j]) V[b][h/G][j],
-//                                 j = 0 .. positions[b] + i, over the cache as the append left it.
+//   quip_kv_append          token i < counts[b] of row b to slot positions[b] + i (e4m3: quantized on the way);
+//   quip_prefill_attention  out[b][i][h] = softmax_j(scale * q[b][i][h] . K[b][h/G][j]) V[b][h/G][j],
+//                           j = 0 .. positions[b] + i, over the cache as the append left it.
 //
 // Appending first means no CTA of the attention writes what another one reads, and with an e4m3 cache the new tokens
 // attend over their own quantized keys and values, which is what every later decode step reads back.
@@ -444,9 +444,6 @@ attn_prefill_kernel(const __half* __restrict__ q, const void* __restrict__ kc, c
   }
 }
 
-bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
 template <bool FP8, bool PAGED, bool RAGGED, int HD, int G>
 int launch_prefill(dim3 grid, cudaStream_t st, const void* q, const void* kc, const void* vc, const float* ksc,
                    const float* vsc, const int64_t* pos, const int64_t* cnt, void* out, KvPages pg, int T, int nh,
@@ -480,58 +477,45 @@ int launch_prefill_g(int G, dim3 grid, cudaStream_t st, const void* q, const voi
 #undef PF_LAUNCH
 }
 
-// Argument checks and launches of quip_prefill_attention (FP8 false) and quip_prefill_attention_fp8 (FP8 true), of
-// their paged twins (PAGED true: the caches and scales are page pools, max_len = max_pages * 64) and of the ragged ones
-// (RAGGED true: B = S sequences, counts = seq_start (S + 1) over n_tok packed rows, T = max_count).
-template <bool FP8, bool PAGED = false, bool RAGGED = false>
-int prefill_attention(const char* fn, const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
-                      const float* v_scale, const int64_t* positions, const int64_t* counts, void* out, int32_t B,
-                      int32_t T, int32_t nh, int32_t nkv, int32_t hd, int32_t max_len, float scale, void* stream,
-                      KvPages pg = {}, int32_t n_tok = 0) {
-  QUIP_CHECK_ARG(q && k_cache && v_cache && positions && counts && out && (!FP8 || (k_scale && v_scale)),
-                 "%s: null pointer", fn);
-  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
-  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
-                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
-                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
+// Argument checks and launches of quip_prefill_attention on a cache kv_check accepted (FP8: e4m3; PAGED: the caches
+// and scales are page pools behind pg, max_len = max_pages * 64) and of quip_prefill_attention_ragged (RAGGED: B = S
+// sequences, counts = seq_start (S + 1) over n_tok packed rows, T = max_count); fn names the entry point.
+template <bool FP8, bool PAGED, bool RAGGED = false>
+int prefill_attention(const char* fn, const QuipKvCache& kv, KvPages pg, int32_t max_len, const void* q,
+                      const int64_t* positions, const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh,
+                      float scale, void* stream, int32_t n_tok = 0) {
+  const int32_t nkv = kv.nkv, hd = kv.hd;
+  QUIP_CHECK_ARG(q && positions && counts && out, "%s: null pointer", fn);
   QUIP_CHECK_ARG(B >= 0 && B <= 65535 && max_len > 0 && nkv > 0 && nkv <= 65535 && nh > 0 && n_tok >= 0,
                  "%s: bad sizes (B %d, nh %d, nkv %d, max_len %d, N %d)", fn, B, nh, nkv, max_len, n_tok);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
   QUIP_CHECK_ARG(nh % nkv == 0 && nh / nkv <= PF_MAXG,
                  "%s: %d query heads on %d kv heads: nh %% nkv must be 0 with at most %d per kv head", fn, nh, nkv,
                  PF_MAXG);
-  QUIP_CHECK_ARG(al16(q) && al16(k_cache) && al16(v_cache) && al16(out), "%s: pointers must be 16-byte aligned", fn);
-  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
+  QUIP_CHECK_ARG(al16(q) && al16(out), "%s: pointers must be 16-byte aligned", fn);
   if (B == 0) return QUIP_OK;
   const int G = nh / nkv;
   const dim3 grid(ceil_div((int64_t)G * T, PF_BM), nkv, B);
   const cudaStream_t st = (cudaStream_t)stream;
-  return hd == 64 ? launch_prefill_g<FP8, PAGED, RAGGED, 64>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale,
+  return hd == 64 ? launch_prefill_g<FP8, PAGED, RAGGED, 64>(G, grid, st, q, kv.k, kv.v, kv.k_scale, kv.v_scale,
                                                              positions, counts, out, pg, T, nh, nkv, max_len, n_tok,
                                                              scale)
-                  : launch_prefill_g<FP8, PAGED, RAGGED, 128>(G, grid, st, q, k_cache, v_cache, k_scale, v_scale,
+                  : launch_prefill_g<FP8, PAGED, RAGGED, 128>(G, grid, st, q, kv.k, kv.v, kv.k_scale, kv.v_scale,
                                                               positions, counts, out, pg, T, nh, nkv, max_len, n_tok,
                                                               scale);
 }
 
-// Argument checks and launches of quip_kv_append (FP8 false) and quip_kv_append_fp8 (FP8 true), and of their paged and
-// ragged twins (RAGGED: as prefill_attention; n_tok * nkv head vectors).
-template <bool FP8, bool PAGED = false, bool RAGGED = false>
-int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
-              float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
-              int32_t hd, int32_t max_len, void* stream, KvPages pg = {}, int32_t n_tok = 0) {
-  QUIP_CHECK_ARG(k_new && v_new && k_cache && v_cache && positions && counts && (!FP8 || (k_scale && v_scale)),
-                 "%s: null pointer", fn);
-  QUIP_CHECK_ARG(hd == 64 || hd == 128, "%s: head_dim %d is not 64 or 128", fn, hd);
-  QUIP_CHECK_ARG(!PAGED || pages_ok(pg),
-                 "%s: page_table must be non-null and 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)",
-                 fn, INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
+// Argument checks and launches of quip_kv_append and quip_kv_append_ragged, as prefill_attention (RAGGED: n_tok * nkv
+// head vectors).
+template <bool FP8, bool PAGED, bool RAGGED = false>
+int kv_append(const char* fn, const QuipKvCache& kv, KvPages pg, int32_t max_len, const void* k_new, const void* v_new,
+              const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, void* stream, int32_t n_tok = 0) {
+  const int32_t nkv = kv.nkv, hd = kv.hd;
+  QUIP_CHECK_ARG(k_new && v_new && positions && counts, "%s: null pointer", fn);
   QUIP_CHECK_ARG(B >= 0 && max_len > 0 && nkv > 0 && n_tok >= 0, "%s: bad sizes (B %d, nkv %d, max_len %d, N %d)", fn,
                  B, nkv, max_len, n_tok);
   QUIP_CHECK_ARG(T >= 1 && T <= max_len, "%s: %d tokens per row: need 1 <= T <= max_len %d", fn, T, max_len);
-  QUIP_CHECK_ARG(al16(k_new) && al16(v_new) && al16(k_cache) && al16(v_cache), "%s: pointers must be 16-byte aligned",
-                 fn);
-  QUIP_CHECK_ARG(!FP8 || (al4(k_scale) && al4(v_scale)), "%s: scale pointers must be 4-byte aligned", fn);
+  QUIP_CHECK_ARG(al16(k_new) && al16(v_new), "%s: pointers must be 16-byte aligned", fn);
   const int64_t nvec = (RAGGED ? (B ? (int64_t)n_tok : 0) : (int64_t)B * T) * nkv;
   if (nvec == 0) return QUIP_OK;
   const unsigned blocks = (unsigned)((nvec + KA_WARPS - 1) / KA_WARPS);
@@ -540,10 +524,10 @@ int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cach
   const __half* vn = (const __half*)v_new;
   if (hd == 64)
     kv_append_kernel<FP8, PAGED, RAGGED, 64><<<blocks, KA_WARPS * 32, 0, st>>>(
-        kn, vn, k_cache, v_cache, k_scale, v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
+        kn, vn, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
   else
     kv_append_kernel<FP8, PAGED, RAGGED, 128><<<blocks, KA_WARPS * 32, 0, st>>>(
-        kn, vn, k_cache, v_cache, k_scale, v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
+        kn, vn, kv.k, kv.v, kv.k_scale, kv.v_scale, positions, counts, pg, nvec, B, T, nkv, max_len);
   QUIP_LAUNCHED("kv_append_kernel");
   return QUIP_OK;
 }
@@ -554,114 +538,57 @@ int kv_append(const char* fn, const void* k_new, const void* v_new, void* k_cach
 
 using namespace quip;
 
-extern "C" int quip_kv_append(const void* k_new, const void* v_new, void* k_cache, void* v_cache,
-                              const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
-                              int32_t hd, int32_t max_len, void* stream) {
-  return kv_append<false>("quip_kv_append", k_new, v_new, k_cache, v_cache, nullptr, nullptr, positions, counts, B, T,
-                          nkv, hd, max_len, stream);
+extern "C" int quip_kv_append(const QuipKvCache* kv, const void* k_new, const void* v_new, const int64_t* positions,
+                              const int64_t* counts, int32_t B, int32_t T, void* stream) {
+  const char* fn = "quip_kv_append";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  return kv_dispatch(*kv, [&](auto fp8, auto paged) {
+    return kv_append<decltype(fp8)::value, decltype(paged)::value>(fn, *kv, pg, max_len, k_new, v_new, positions,
+                                                                 counts, B, T, stream);
+  });
 }
 
-extern "C" int quip_kv_append_fp8(const void* k_new, const void* v_new, void* k_cache, void* v_cache, float* k_scale,
-                                  float* v_scale, const int64_t* positions, const int64_t* counts, int32_t B, int32_t T,
-                                  int32_t nkv, int32_t hd, int32_t max_len, void* stream) {
-  return kv_append<true>("quip_kv_append_fp8", k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, counts, B,
-                         T, nkv, hd, max_len, stream);
+extern "C" int quip_prefill_attention(const QuipKvCache* kv, const void* q, const int64_t* positions,
+                                      const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, float scale,
+                                      void* stream) {
+  const char* fn = "quip_prefill_attention";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  return kv_dispatch(*kv, [&](auto fp8, auto paged) {
+    return prefill_attention<decltype(fp8)::value, decltype(paged)::value>(fn, *kv, pg, max_len, q, positions, counts,
+                                                                         out, B, T, nh, scale, stream);
+  });
 }
 
-extern "C" int quip_prefill_attention(const void* q, const void* k_cache, const void* v_cache, const int64_t* positions,
-                                      const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv,
-                                      int32_t hd, int32_t max_len, float scale, void* stream) {
-  return prefill_attention<false>("quip_prefill_attention", q, k_cache, v_cache, nullptr, nullptr, positions, counts,
-                                  out, B, T, nh, nkv, hd, max_len, scale, stream);
-}
-
-extern "C" int quip_prefill_attention_fp8(const void* q, const void* k_cache, const void* v_cache, const float* k_scale,
-                                          const float* v_scale, const int64_t* positions, const int64_t* counts,
-                                          void* out, int32_t B, int32_t T, int32_t nh, int32_t nkv, int32_t hd,
-                                          int32_t max_len, float scale, void* stream) {
-  return prefill_attention<true>("quip_prefill_attention_fp8", q, k_cache, v_cache, k_scale, v_scale, positions,
-                                 counts, out, B, T, nh, nkv, hd, max_len, scale, stream);
-}
-
-// Paged twins: max_len = max_pages * 64.
-extern "C" int quip_kv_append_paged(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                    const int64_t* positions, const int64_t* counts, int32_t B, int32_t T, int32_t nkv,
-                                    int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                    void* stream) {
-  return kv_append<false, true>("quip_kv_append_paged", k_new, v_new, k_pool, v_pool, nullptr, nullptr, positions,
-                                counts, B, T, nkv, hd, paged_len(max_pages), stream,
-                                KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_kv_append_paged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                        float* k_scale, float* v_scale, const int64_t* positions, const int64_t* counts,
-                                        int32_t B, int32_t T, int32_t nkv, int32_t hd, const int32_t* page_table,
-                                        int32_t max_pages, int32_t n_pages, void* stream) {
-  return kv_append<true, true>("quip_kv_append_paged_fp8", k_new, v_new, k_pool, v_pool, k_scale, v_scale, positions,
-                               counts, B, T, nkv, hd, paged_len(max_pages), stream,
-                               KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_prefill_attention_paged(const void* q, const void* k_pool, const void* v_pool,
-                                            const int64_t* positions, const int64_t* counts, void* out, int32_t B,
-                                            int32_t T, int32_t nh, int32_t nkv, int32_t hd, float scale,
-                                            const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                            void* stream) {
-  return prefill_attention<false, true>("quip_prefill_attention_paged", q, k_pool, v_pool, nullptr, nullptr, positions,
-                                        counts, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, stream,
-                                        KvPages{page_table, max_pages, n_pages});
-}
-
-extern "C" int quip_prefill_attention_paged_fp8(const void* q, const void* k_pool, const void* v_pool,
-                                                const float* k_scale, const float* v_scale, const int64_t* positions,
-                                                const int64_t* counts, void* out, int32_t B, int32_t T, int32_t nh,
-                                                int32_t nkv, int32_t hd, float scale, const int32_t* page_table,
-                                                int32_t max_pages, int32_t n_pages, void* stream) {
-  return prefill_attention<true, true>("quip_prefill_attention_paged_fp8", q, k_pool, v_pool, k_scale, v_scale,
-                                       positions, counts, out, B, T, nh, nkv, hd, paged_len(max_pages), scale, stream,
-                                       KvPages{page_table, max_pages, n_pages});
-}
-
-// Ragged twins: S packed sequences (seq_start (S + 1), positions (S), page_table (S, max_pages)) over N token rows; T is
-// max_count.
-extern "C" int quip_kv_append_ragged(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
+// Ragged launches: S packed sequences (seq_start (S + 1), positions (S), page_table (S, max_pages)) over N token rows;
+// T is max_count.  Paged only, so only the format selects the instantiation.
+extern "C" int quip_kv_append_ragged(const QuipKvCache* kv, const void* k_new, const void* v_new,
                                      const int64_t* seq_start, const int64_t* positions, int32_t S, int32_t N,
-                                     int32_t max_count, int32_t nkv, int32_t hd, const int32_t* page_table,
-                                     int32_t max_pages, int32_t n_pages, void* stream) {
-  return kv_append<false, true, true>("quip_kv_append_ragged", k_new, v_new, k_pool, v_pool, nullptr, nullptr,
-                                      positions, seq_start, S, max_count, nkv, hd, paged_len(max_pages), stream,
-                                      KvPages{page_table, max_pages, n_pages}, N);
+                                     int32_t max_count, void* stream) {
+  const char* fn = "quip_kv_append_ragged";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  QUIP_CHECK_ARG(kv->page_table, "%s: page_table is null: ragged launches are paged only", fn);
+  return kv->format == QUIP_KV_E4M3
+      ? kv_append<true, true, true>(fn, *kv, pg, max_len, k_new, v_new, positions, seq_start, S, max_count, stream, N)
+      : kv_append<false, true, true>(fn, *kv, pg, max_len, k_new, v_new, positions, seq_start, S, max_count, stream, N);
 }
 
-extern "C" int quip_kv_append_ragged_fp8(const void* k_new, const void* v_new, void* k_pool, void* v_pool,
-                                         float* k_scale, float* v_scale, const int64_t* seq_start,
-                                         const int64_t* positions, int32_t S, int32_t N, int32_t max_count, int32_t nkv,
-                                         int32_t hd, const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                         void* stream) {
-  return kv_append<true, true, true>("quip_kv_append_ragged_fp8", k_new, v_new, k_pool, v_pool, k_scale, v_scale,
-                                     positions, seq_start, S, max_count, nkv, hd, paged_len(max_pages), stream,
-                                     KvPages{page_table, max_pages, n_pages}, N);
-}
-
-extern "C" int quip_prefill_attention_ragged(const void* q, const void* k_pool, const void* v_pool,
-                                             const int64_t* seq_start, const int64_t* positions, void* out, int32_t S,
-                                             int32_t N, int32_t max_count, int32_t nh, int32_t nkv, int32_t hd,
-                                             float scale, const int32_t* page_table, int32_t max_pages,
-                                             int32_t n_pages, void* stream) {
-  return prefill_attention<false, true, true>("quip_prefill_attention_ragged", q, k_pool, v_pool, nullptr, nullptr,
-                                              positions, seq_start, out, S, max_count, nh, nkv, hd,
-                                              paged_len(max_pages), scale, stream,
-                                              KvPages{page_table, max_pages, n_pages}, N);
-}
-
-extern "C" int quip_prefill_attention_ragged_fp8(const void* q, const void* k_pool, const void* v_pool,
-                                                 const float* k_scale, const float* v_scale, const int64_t* seq_start,
-                                                 const int64_t* positions, void* out, int32_t S, int32_t N,
-                                                 int32_t max_count, int32_t nh, int32_t nkv, int32_t hd, float scale,
-                                                 const int32_t* page_table, int32_t max_pages, int32_t n_pages,
-                                                 void* stream) {
-  return prefill_attention<true, true, true>("quip_prefill_attention_ragged_fp8", q, k_pool, v_pool, k_scale, v_scale,
-                                             positions, seq_start, out, S, max_count, nh, nkv, hd,
-                                             paged_len(max_pages), scale, stream,
-                                             KvPages{page_table, max_pages, n_pages}, N);
+extern "C" int quip_prefill_attention_ragged(const QuipKvCache* kv, const void* q, const int64_t* seq_start,
+                                             const int64_t* positions, void* out, int32_t S, int32_t N,
+                                             int32_t max_count, int32_t nh, float scale, void* stream) {
+  const char* fn = "quip_prefill_attention_ragged";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  QUIP_CHECK_ARG(kv->page_table, "%s: page_table is null: ragged launches are paged only", fn);
+  return kv->format == QUIP_KV_E4M3
+      ? prefill_attention<true, true, true>(fn, *kv, pg, max_len, q, positions, seq_start, out, S, max_count, nh,
+                                            scale, stream, N)
+      : prefill_attention<false, true, true>(fn, *kv, pg, max_len, q, positions, seq_start, out, S, max_count, nh,
+                                             scale, stream, N);
 }

@@ -523,25 +523,23 @@ __global__ void __launch_bounds__(128) beam_fork_kernel(int phase, T* __restrict
   }
 }
 
+// Checks and the two launches of quip_kv_beam_fork on pools of T (SCALES: e4m3 with scales); kv describes layer 0.
 template <typename T, bool SCALES>
-int launch_fork(void* k_pool, void* v_pool, float* k_scale, float* v_scale, int32_t* table, int32_t* table_tmp,
-                const int64_t* parents, const int64_t* lens, int32_t R, int32_t L, int32_t n_pages, int32_t nkv,
-                int32_t hd, int32_t max_pages, int32_t scratch0, void* stream) {
-  QUIP_CHECK_ARG(R >= 0 && L >= 1 && L <= 65535 && nkv >= 1 && nkv <= 32767 && hd >= 1 &&
-                     (hd * (int)sizeof(T)) % 16 == 0 && max_pages >= 1 && max_pages <= INT32_MAX / KV_PAGE &&
-                     n_pages >= 1 && scratch0 >= 0 && (int64_t)scratch0 + R <= n_pages,
+int launch_fork(const QuipKvCache& kv, KvPages pg, int32_t L, int32_t* table_tmp, const int64_t* parents,
+                const int64_t* lens, int32_t R, int32_t scratch0, void* stream) {
+  const int32_t nkv = kv.nkv, hd = kv.hd, max_pages = pg.max_pages, n_pages = pg.n_pages;
+  QUIP_CHECK_ARG(R >= 0 && L >= 1 && L <= 65535 && nkv >= 1 && nkv <= 32767 && scratch0 >= 0 &&
+                     (int64_t)scratch0 + R <= n_pages,
                  "quip_kv_beam_fork: bad sizes (R %d, L %d, n_pages %d, nkv %d, hd %d, max_pages %d, scratch0 %d)", R,
                  L, n_pages, nkv, hd, max_pages, scratch0);
-  QUIP_CHECK_ARG(k_pool && v_pool && table && table_tmp && parents && lens && (!SCALES || (k_scale && v_scale)),
-                 "quip_kv_beam_fork: null pointer");
-  QUIP_CHECK_ARG(((uintptr_t)k_pool & 15) == 0 && ((uintptr_t)v_pool & 15) == 0,
-                 "quip_kv_beam_fork: the pools must be 16-byte aligned");
+  QUIP_CHECK_ARG(table_tmp && parents && lens, "quip_kv_beam_fork: null pointer");
   if (R == 0) return QUIP_OK;
   const dim3 grid((unsigned)R, (unsigned)L, 2u * (unsigned)nkv);
   for (int phase = 0; phase < 2; ++phase) {
-    beam_fork_kernel<T, SCALES><<<grid, 128, 0, (cudaStream_t)stream>>>(phase, (T*)k_pool, (T*)v_pool, k_scale,
-                                                                         v_scale, table, table_tmp, parents, lens, R,
-                                                                         n_pages, nkv, hd, max_pages, scratch0);
+    beam_fork_kernel<T, SCALES><<<grid, 128, 0, (cudaStream_t)stream>>>(phase, (T*)kv.k, (T*)kv.v, kv.k_scale,
+                                                                         kv.v_scale, kv.page_table, table_tmp, parents,
+                                                                         lens, R, n_pages, nkv, hd, max_pages,
+                                                                         scratch0);
     QUIP_LAUNCHED("beam_fork_kernel");
   }
   return QUIP_OK;
@@ -589,17 +587,14 @@ extern "C" int quip_beam_select(const float* cand_s, const int32_t* cand_i, cons
   return QUIP_OK;
 }
 
-extern "C" int quip_kv_beam_fork(void* k_pool, void* v_pool, int32_t* table, int32_t* table_tmp,
-                                 const int64_t* parents, const int64_t* lens, int32_t R, int32_t L, int32_t n_pages,
-                                 int32_t nkv, int32_t hd, int32_t max_pages, int32_t scratch0, void* stream) {
-  return launch_fork<__half, false>(k_pool, v_pool, nullptr, nullptr, table, table_tmp, parents, lens, R, L, n_pages,
-                                    nkv, hd, max_pages, scratch0, stream);
-}
-
-extern "C" int quip_kv_beam_fork_fp8(void* k_pool, void* v_pool, float* k_scale, float* v_scale, int32_t* table,
-                                     int32_t* table_tmp, const int64_t* parents, const int64_t* lens, int32_t R,
-                                     int32_t L, int32_t n_pages, int32_t nkv, int32_t hd, int32_t max_pages,
-                                     int32_t scratch0, void* stream) {
-  return launch_fork<uint8_t, true>(k_pool, v_pool, k_scale, v_scale, table, table_tmp, parents, lens, R, L, n_pages,
-                                    nkv, hd, max_pages, scratch0, stream);
+extern "C" int quip_kv_beam_fork(const QuipKvCache* kv, int32_t L, int32_t* table_tmp, const int64_t* parents,
+                                 const int64_t* lens, int32_t R, int32_t scratch0, void* stream) {
+  const char* fn = "quip_kv_beam_fork";
+  KvPages pg;
+  int32_t max_len;
+  if (const int e = kv_check(fn, kv, pg, max_len)) return e;
+  QUIP_CHECK_ARG(kv->page_table, "%s: page_table is null: the fork is paged only", fn);
+  return kv->format == QUIP_KV_E4M3
+      ? launch_fork<uint8_t, true>(*kv, pg, L, table_tmp, parents, lens, R, scratch0, stream)
+      : launch_fork<__half, false>(*kv, pg, L, table_tmp, parents, lens, R, scratch0, stream);
 }

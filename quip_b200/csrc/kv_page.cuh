@@ -1,9 +1,14 @@
 // Where a cached slot lives: the contiguous KV cache (B, nkv, max_len, hd) or the paged one (include/quip_b200.h: a
 // (n_pages, nkv, 64, hd) pool per layer behind page_table (B, max_pages) int32).  Every attention kernel walks the cache
 // in 64-slot blocks aligned to 64, so a block lies in one page and a kernel looks up each page once per block.  One
-// helper serves both layouts; the contiguous instantiation is the index arithmetic the kernels always had.
+// helper serves both layouts; the contiguous instantiation is the index arithmetic the kernels always had.  The entry
+// points take a layer's cache as one QuipKvCache, which kv_check validates and resolves for the kernels.
 #pragma once
 #include <stdint.h>
+
+#include <type_traits>
+
+#include "common.cuh"
 
 namespace quip {
 
@@ -28,14 +33,43 @@ __device__ __forceinline__ int64_t kv_vec(const KvPages& pg, int64_t b, int h, i
   }
 }
 
-// The checks of a paged launch's table: 4-byte aligned, max_len = max_pages * 64 an int32, a non-empty pool.
-inline bool pages_ok(const KvPages& pg) {
-  return pg.table && (reinterpret_cast<uintptr_t>(pg.table) & 3) == 0 && pg.max_pages > 0 &&
-         pg.max_pages <= INT32_MAX / KV_PAGE && pg.n_pages > 0;
+inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+inline bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+// The host check of a cache descriptor, shared by every entry point that takes one (fn names it in the messages).  On
+// success pg is the page table (empty when contiguous) and max_len the slots per row the kernels take: the
+// descriptor's max_len, or max_pages * 64 when paged.
+inline int kv_check(const char* fn, const QuipKvCache* kv, KvPages& pg, int32_t& max_len) {
+  QUIP_CHECK_ARG(kv, "%s: null cache descriptor", fn);
+  QUIP_CHECK_ARG(kv->format == QUIP_KV_FP16 || kv->format == QUIP_KV_E4M3,
+                 "%s: format %d is neither QUIP_KV_FP16 nor QUIP_KV_E4M3", fn, kv->format);
+  const bool fp8 = kv->format == QUIP_KV_E4M3;
+  QUIP_CHECK_ARG(kv->k && kv->v, "%s: null pointer (k / v)", fn);
+  QUIP_CHECK_ARG(!fp8 || (kv->k_scale && kv->v_scale), "%s: null pointer (k_scale / v_scale of an e4m3 cache)", fn);
+  QUIP_CHECK_ARG(fp8 || (!kv->k_scale && !kv->v_scale), "%s: k_scale / v_scale given for an fp16 cache", fn);
+  QUIP_CHECK_ARG(al16(kv->k) && al16(kv->v), "%s: k and v must be 16-byte aligned", fn);
+  QUIP_CHECK_ARG(!fp8 || (al4(kv->k_scale) && al4(kv->v_scale)), "%s: k_scale and v_scale must be 4-byte aligned", fn);
+  QUIP_CHECK_ARG(kv->hd == 64 || kv->hd == 128, "%s: head_dim %d is not 64 or 128", fn, kv->hd);
+  if (!kv->page_table) {
+    pg = KvPages{};
+    max_len = kv->max_len;
+    return QUIP_OK;
+  }
+  pg = KvPages{kv->page_table, kv->max_pages, kv->n_pages};
+  QUIP_CHECK_ARG(al4(pg.table) && pg.max_pages > 0 && pg.max_pages <= INT32_MAX / KV_PAGE && pg.n_pages > 0,
+                 "%s: page_table must be 4-byte aligned, 0 < max_pages <= %d, n_pages > 0 (got %d, %d)", fn,
+                 INT32_MAX / KV_PAGE, pg.max_pages, pg.n_pages);
+  max_len = pg.max_pages * KV_PAGE;
+  return QUIP_OK;
 }
-// max_len of a paged launch; 1 for a max_pages that pages_ok refuses (the launch then fails on the table)
-inline int32_t paged_len(int32_t max_pages) {
-  return max_pages > 0 && max_pages <= INT32_MAX / KV_PAGE ? max_pages * KV_PAGE : 1;
+
+// Calls f(fp8, paged), two std::bool_constant tags, for the format and layout of a checked descriptor, so an entry
+// point instantiates its host template once per cache kind.
+template <class F>
+int kv_dispatch(const QuipKvCache& kv, F&& f) {
+  if (kv.format == QUIP_KV_E4M3)
+    return kv.page_table ? f(std::true_type{}, std::true_type{}) : f(std::true_type{}, std::false_type{});
+  return kv.page_table ? f(std::false_type{}, std::true_type{}) : f(std::false_type{}, std::false_type{});
 }
 
 }  // namespace quip

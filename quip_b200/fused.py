@@ -91,89 +91,67 @@ class CudaGlue:
 KV_PAGE = 64
 
 
-def _kv_layout(fn, k_cache, B, page_table):
-    """(rows, slots, max_len) of one layer's cache k_cache (rows, nkv, slots, hd): the contiguous cache (B, nkv, max_len,
-    hd) without a page table; with page_table (B, max_pages) int32, pools (n_pages, nkv, 64, hd) and max_len =
-    max_pages * 64 (include/quip_b200.h has the rule).  Checks the table's dtype, shape, device and alignment and the
-    pools' alignment; the callers check the rest of the shapes against these."""
+def _kv_format(fn, k_cache, v_cache, k_scale, v_scale):
+    """Whether one layer's caches are e4m3: fp16 caches take no scales, float8_e4m3fn caches fp32 k_scale / v_scale."""
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn caches only')
+    if fp8 and (k_scale is None or v_scale is None):
+        raise ValueError(f'{fn}: float8_e4m3fn caches need k_scale and v_scale')
+    cdt = torch.float8_e4m3fn if fp8 else torch.float16
+    if (k_cache.dtype != cdt or v_cache.dtype != cdt or
+            (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
+        raise ValueError(f'{fn} takes fp16 or float8_e4m3fn caches (fp32 scales), got {k_cache.dtype} / '
+                         f'{v_cache.dtype}')
+    return fp8
+
+
+def _kv_cache(fn, k_cache, v_cache, k_scale, v_scale, page_table, rows):
+    """The checked QuipKvCache of one layer's cache (include/quip_b200.h has the rule): fp16 caches, or float8_e4m3fn
+    caches with fp32 k_scale / v_scale, one per slot.  Without a page table the caches are (rows, nkv, max_len, hd);
+    with page_table (rows, max_pages) int32 they are pools (n_pages, nkv, 64, hd) and max_len = max_pages * 64, which
+    the descriptor's max_len holds in both layouts.  Checks the table's dtype, shape, device and alignment and the
+    pools' alignment; the callers check that the caches and scales are contiguous CUDA tensors with their operands."""
+    fp8 = _kv_format(fn, k_cache, v_cache, k_scale, v_scale)
+    if k_cache.dim() != 4:
+        raise ValueError(f'{fn}: the caches must be (B, nkv, max_len, hd), got {tuple(k_cache.shape)}')
+    n, nkv, slots, hd = k_cache.shape
+    kv = _lib.QuipKvCache(k=k_cache.data_ptr(), v=v_cache.data_ptr(), nkv=nkv, hd=hd,
+                          format=_lib.QUIP_KV_E4M3 if fp8 else _lib.QUIP_KV_FP16)
     if page_table is None:
-        return B, k_cache.shape[2], k_cache.shape[2]
-    if page_table.dtype != torch.int32 or page_table.dim() != 2 or page_table.shape[0] != B or page_table.shape[1] < 1:
-        raise ValueError(f'{fn}: page_table must be (B={B}, max_pages >= 1) int32, got {tuple(page_table.shape)} '
-                         f'{page_table.dtype}')
-    if k_cache.dim() != 4 or k_cache.shape[2] != KV_PAGE or k_cache.shape[0] < 1:
-        raise ValueError(f'{fn}: with a page table the caches are pools (n_pages, nkv, {KV_PAGE}, hd), got '
-                         f'{tuple(k_cache.shape)}')
-    if page_table.shape[1] > (2 ** 31 - 1) // KV_PAGE:
-        raise ValueError(f'{fn}: {page_table.shape[1]} pages per row: max_pages * {KV_PAGE} must fit int32')
-    if not page_table.is_cuda or page_table.device != k_cache.device or not page_table.is_contiguous():
-        raise ValueError(f'{fn}: page_table must be a contiguous CUDA tensor on the caches\' device')
-    if page_table.data_ptr() % 4 or k_cache.data_ptr() % 16:
-        raise ValueError(f'{fn}: page_table must be 4-byte aligned and the pools 16-byte aligned')
-    return k_cache.shape[0], KV_PAGE, page_table.shape[1] * KV_PAGE
-
-
-def _paged_args(page_table, n_pages):
-    return (page_table.data_ptr(), page_table.shape[1], n_pages)
-
-
-def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
-    """quip_decode_attention on torch tensors: append k_new / v_new (B, nkv, hd) at slot positions[b] of one layer's
-    k_cache / v_cache (B, nkv, max_len, hd) and attend q (B, nh, hd) over slots 0 .. positions[b].  fp16, CUDA,
-    contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream.
-
-    Caches of dtype torch.float8_e4m3fn take quip_decode_attention_fp8 and need their per-slot fp32 scales k_scale /
-    v_scale (B, nkv, max_len): k_new / v_new are quantized on append (include/quip_b200.h has the format).
-
-    page_table (B, max_pages) int32: the caches are page pools (n_pages, nkv, 64, hd), scales (n_pages, nkv, 64), and
-    slot j of row b lives at slot j % 64 of page page_table[b, j // 64] (quip_decode_attention_paged(_fp8)); a row that
-    would touch a page id outside [0, n_pages) writes nothing there and gets NaN."""
-    if k_cache.dtype == torch.float8_e4m3fn:
-        return _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale, page_table)
-    if k_scale is not None or v_scale is not None:
-        raise ValueError('decode_attention: k_scale / v_scale go with float8_e4m3fn caches only')
-    ts = (q, k_new, v_new, k_cache, v_cache)
-    for t in ts + (positions,):
-        if not t.is_cuda:
-            raise RuntimeError('decode_attention runs on a CUDA device only (there is no CPU fallback)')
-        if t.device != q.device:
-            raise ValueError('decode_attention: all tensors must be on one device')
-        if not t.is_contiguous():
-            raise ValueError('decode_attention takes contiguous tensors')
-    if any(t.dtype != torch.float16 for t in ts) or positions.dtype != torch.int64:
-        raise ValueError('decode_attention takes fp16 q / k / v / caches and int64 positions')
-    if q.dim() != 3 or k_cache.dim() != 4:
-        raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
-                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
-    B, nh, hd = q.shape
-    nkv = k_cache.shape[1]
-    rows, slots, max_len = _kv_layout('decode_attention', k_cache, B, page_table)
-    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
-            tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,)):
-        raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
-                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
-                         f'{tuple(positions.shape)} do not agree')
-    lib = _lib.load()
-    need = C.c_size_t(0)
-    _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
-    ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
-    out = torch.empty_like(q)
-    st = torch.cuda.current_stream(q.device).cuda_stream
-    with torch.cuda.device(q.device):
-        if page_table is not None:
-            _lib.check(lib.quip_decode_attention_paged(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                                                       k_cache.data_ptr(), v_cache.data_ptr(), positions.data_ptr(),
-                                                       out.data_ptr(), B, nh, nkv, hd, C.c_float(scale), ws.data_ptr(),
-                                                       ws.numel(), *_paged_args(page_table, rows), st))
-        else:
-            _lib.check(lib.quip_decode_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                 v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh, nkv,
-                                                 hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
-    return out
+        kv.max_len = slots
+        if n != rows:
+            raise ValueError(f'{fn}: caches {tuple(k_cache.shape)} do not agree with {rows} rows')
+    else:
+        if (page_table.dtype != torch.int32 or page_table.dim() != 2 or page_table.shape[0] != rows or
+                page_table.shape[1] < 1):
+            raise ValueError(f'{fn}: page_table must be (B={rows}, max_pages >= 1) int32, got '
+                             f'{tuple(page_table.shape)} {page_table.dtype}')
+        if slots != KV_PAGE or n < 1:
+            raise ValueError(f'{fn}: with a page table the caches are pools (n_pages, nkv, {KV_PAGE}, hd), got '
+                             f'{tuple(k_cache.shape)}')
+        if page_table.shape[1] > (2 ** 31 - 1) // KV_PAGE:
+            raise ValueError(f'{fn}: {page_table.shape[1]} pages per row: max_pages * {KV_PAGE} must fit int32')
+        if not page_table.is_cuda or page_table.device != k_cache.device or not page_table.is_contiguous():
+            raise ValueError(f'{fn}: page_table must be a contiguous CUDA tensor on the caches\' device')
+        if page_table.data_ptr() % 4 or k_cache.data_ptr() % 16 or v_cache.data_ptr() % 16:
+            raise ValueError(f'{fn}: page_table must be 4-byte aligned and the pools 16-byte aligned')
+        kv.page_table, kv.max_pages, kv.n_pages = page_table.data_ptr(), page_table.shape[1], n
+        kv.max_len = page_table.shape[1] * KV_PAGE
+    if v_cache.shape != k_cache.shape or (fp8 and (tuple(k_scale.shape) != (n, nkv, slots) or
+                                                    v_scale.shape != k_scale.shape)):
+        raise ValueError(f'{fn}: shapes caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, scales '
+                         f'{None if k_scale is None else tuple(k_scale.shape)} / '
+                         f'{None if v_scale is None else tuple(v_scale.shape)} do not agree')
+    if fp8:
+        kv.k_scale, kv.v_scale = k_scale.data_ptr(), v_scale.data_ptr()
+    return kv
 
 
 def _check_cuda(fn, ts, dev):
     for t in ts:
+        if t is None:
+            continue
         if not t.is_cuda:
             raise RuntimeError(f'{fn} runs on a CUDA device only (there is no CPU fallback)')
         if t.device != dev:
@@ -182,44 +160,39 @@ def _check_cuda(fn, ts, dev):
             raise ValueError(f'{fn} takes contiguous tensors')
 
 
-def _decode_attention_fp8(q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, scale, page_table):
-    if k_scale is None or v_scale is None:
-        raise ValueError('decode_attention: float8_e4m3fn caches need k_scale and v_scale')
-    if (any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or v_cache.dtype != torch.float8_e4m3fn or
-            k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32 or positions.dtype != torch.int64):
-        raise ValueError('decode_attention: an e4m3 step takes fp16 q / k / v, float8_e4m3fn caches, fp32 scales and '
-                         'int64 positions')
-    if q.dim() != 3 or k_cache.dim() != 4:
-        raise ValueError(f'decode_attention: q must be (B, nh, hd) and the caches (B, nkv, max_len, hd), got '
-                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
+def decode_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
+    """quip_decode_attention on torch tensors: append k_new / v_new (B, nkv, hd) at slot positions[b] of one layer's
+    k_cache / v_cache (B, nkv, max_len, hd) and attend q (B, nh, hd) over slots 0 .. positions[b].  fp16, CUDA,
+    contiguous; positions (B,) int64 on the same device.  Returns (B, nh, hd) fp16, on the current stream.
+
+    Caches of dtype torch.float8_e4m3fn need their per-slot fp32 scales k_scale / v_scale (B, nkv, max_len): k_new /
+    v_new are quantized on append (include/quip_b200.h has the format).
+
+    page_table (B, max_pages) int32: the caches are page pools (n_pages, nkv, 64, hd), scales (n_pages, nkv, 64), and
+    slot j of row b lives at slot j % 64 of page page_table[b, j // 64]; a row that would touch a page id outside
+    [0, n_pages) writes nothing there and gets NaN."""
+    if q.dim() != 3:
+        raise ValueError(f'decode_attention: q must be (B, nh, hd), got {tuple(q.shape)}')
     B, nh, hd = q.shape
-    nkv = k_cache.shape[1]
-    rows, slots, max_len = _kv_layout('decode_attention', k_cache, B, page_table)
-    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
-            tuple(k_new.shape) != (B, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
-            tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape):
+    kv = _kv_cache('decode_attention', k_cache, v_cache, k_scale, v_scale, page_table, B)
+    if any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or positions.dtype != torch.int64:
+        raise ValueError('decode_attention takes fp16 q / k / v and int64 positions')
+    if (kv.hd != hd or tuple(k_new.shape) != (B, kv.nkv, hd) or v_new.shape != k_new.shape or
+            tuple(positions.shape) != (B,)):
         raise ValueError(f'decode_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
-                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, scales '
-                         f'{tuple(k_scale.shape)} / {tuple(v_scale.shape)}, positions {tuple(positions.shape)} do not agree')
+                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)}, positions {tuple(positions.shape)} do '
+                         'not agree')
     _check_cuda('decode_attention', (q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions), q.device)
     lib = _lib.load()
     need = C.c_size_t(0)
-    _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, max_len, C.byref(need)))
+    _lib.check(lib.quip_decode_attention_workspace_bytes(B, nh, hd, kv.max_len, C.byref(need)))
     ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
     out = torch.empty_like(q)
     st = torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        if page_table is not None:
-            _lib.check(lib.quip_decode_attention_paged_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                                                           k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
-                                                           v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B,
-                                                           nh, nkv, hd, C.c_float(scale), ws.data_ptr(), ws.numel(),
-                                                           *_paged_args(page_table, rows), st))
-        else:
-            _lib.check(lib.quip_decode_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                                                     k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
-                                                     v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B, nh,
-                                                     nkv, hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
+        _lib.check(lib.quip_decode_attention(C.byref(kv), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                             positions.data_ptr(), out.data_ptr(), B, nh, C.c_float(scale),
+                                             ws.data_ptr(), ws.numel(), st))
     return out
 
 
@@ -362,163 +335,85 @@ def token_topk_logprobs(logits, tokens, cols, lp, top_ids=None, top_lp=None, T=1
 
 
 def extend_attention(q, k_new, v_new, k_cache, v_cache, positions, scale, k_scale=None, v_scale=None, page_table=None):
-    """quip_extend_attention(_fp8) on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot
-    positions[b] + i of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots
-    0 .. positions[b] + i.  fp16 q / k / v; fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale
-    (B, nkv, max_len).  CUDA, one device, contiguous; positions (B,) int64.  Returns (B, T, nh, hd) fp16.
-    page_table: page pools as in decode_attention (quip_extend_attention_paged(_fp8))."""
-    fp8 = k_cache.dtype == torch.float8_e4m3fn
-    if not fp8 and (k_scale is not None or v_scale is not None):
-        raise ValueError('extend_attention: k_scale / v_scale go with float8_e4m3fn caches only')
-    if fp8 and (k_scale is None or v_scale is None):
-        raise ValueError('extend_attention: float8_e4m3fn caches need k_scale and v_scale')
-    cdt = torch.float8_e4m3fn if fp8 else torch.float16
-    if (any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or k_cache.dtype != cdt or v_cache.dtype != cdt or
-            positions.dtype != torch.int64 or (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
-        raise ValueError('extend_attention takes fp16 q / k / v, fp16 or float8_e4m3fn caches (fp32 scales) and int64 '
-                         'positions')
-    if q.dim() != 4 or k_cache.dim() != 4:
-        raise ValueError(f'extend_attention: q must be (B, T, nh, hd) and the caches (B, nkv, max_len, hd), got '
-                         f'{tuple(q.shape)} and {tuple(k_cache.shape)}')
+    """quip_extend_attention on torch tensors: append token i of k_new / v_new (B, T, nkv, hd) at slot positions[b] + i
+    of one layer's caches (B, nkv, max_len, hd) and attend q (B, T, nh, hd) causally over slots 0 .. positions[b] + i.
+    fp16 q / k / v; fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale (B, nkv, max_len).  CUDA, one
+    device, contiguous; positions (B,) int64.  Returns (B, T, nh, hd) fp16.  page_table: page pools as in
+    decode_attention."""
+    if q.dim() != 4:
+        raise ValueError(f'extend_attention: q must be (B, T, nh, hd), got {tuple(q.shape)}')
     B, T, nh, hd = q.shape
-    nkv = k_cache.shape[1]
-    rows, slots, max_len = _kv_layout('extend_attention', k_cache, B, page_table)
-    if (tuple(k_cache.shape) != (rows, nkv, slots, hd) or v_cache.shape != k_cache.shape or
-            tuple(k_new.shape) != (B, T, nkv, hd) or v_new.shape != k_new.shape or tuple(positions.shape) != (B,) or
-            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
+    kv = _kv_cache('extend_attention', k_cache, v_cache, k_scale, v_scale, page_table, B)
+    if any(t.dtype != torch.float16 for t in (q, k_new, v_new)) or positions.dtype != torch.int64:
+        raise ValueError('extend_attention takes fp16 q / k / v and int64 positions')
+    if (kv.hd != hd or tuple(k_new.shape) != (B, T, kv.nkv, hd) or v_new.shape != k_new.shape or
+            tuple(positions.shape) != (B,)):
         raise ValueError(f'extend_attention: shapes q {tuple(q.shape)}, k_new {tuple(k_new.shape)}, v_new '
-                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
-                         f'{tuple(positions.shape)} do not agree')
-    ts = (q, k_new, v_new, k_cache, v_cache, positions) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('extend_attention', ts, q.device)
+                         f'{tuple(v_new.shape)}, caches {tuple(k_cache.shape)}, positions {tuple(positions.shape)} do '
+                         'not agree')
+    _check_cuda('extend_attention', (q, k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions), q.device)
     lib = _lib.load()
     need = C.c_size_t(0)
-    _lib.check(lib.quip_extend_attention_workspace_bytes(B, T, nh, hd, max_len, C.byref(need)))
+    _lib.check(lib.quip_extend_attention_workspace_bytes(B, T, nh, hd, kv.max_len, C.byref(need)))
     ws = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=q.device)
     out = torch.empty_like(q)
     st = torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        if page_table is not None and fp8:
-            _lib.check(lib.quip_extend_attention_paged_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                                                           k_cache.data_ptr(), v_cache.data_ptr(), k_scale.data_ptr(),
-                                                           v_scale.data_ptr(), positions.data_ptr(), out.data_ptr(), B, T,
-                                                           nh, nkv, hd, C.c_float(scale), ws.data_ptr(), ws.numel(),
-                                                           *_paged_args(page_table, rows), st))
-        elif page_table is not None:
-            _lib.check(lib.quip_extend_attention_paged(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                                                       k_cache.data_ptr(), v_cache.data_ptr(), positions.data_ptr(),
-                                                       out.data_ptr(), B, T, nh, nkv, hd, C.c_float(scale),
-                                                       ws.data_ptr(), ws.numel(), *_paged_args(page_table, rows), st))
-        elif fp8:
-            _lib.check(lib.quip_extend_attention_fp8(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                     v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
-                                                     positions.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,
-                                                     C.c_float(scale), ws.data_ptr(), ws.numel(), st))
-        else:
-            _lib.check(lib.quip_extend_attention(q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                 v_cache.data_ptr(), positions.data_ptr(), out.data_ptr(), B, T, nh, nkv,
-                                                 hd, max_len, C.c_float(scale), ws.data_ptr(), ws.numel(), st))
+        _lib.check(lib.quip_extend_attention(C.byref(kv), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                                             positions.data_ptr(), out.data_ptr(), B, T, nh, C.c_float(scale),
+                                             ws.data_ptr(), ws.numel(), st))
     return out
 
 
-def _check_chunk(fn, k_cache, v_cache, positions, counts, k_scale, v_scale, page_table=None):
-    """The checks kv_append and prefill_attention share: cache and scale dtypes, positions / counts (B,) int64, and the
-    page table with its pools.  Returns (whether the caches are e4m3, B, rows, max_len) (_kv_layout)."""
-    fp8 = k_cache.dtype == torch.float8_e4m3fn
-    if not fp8 and (k_scale is not None or v_scale is not None):
-        raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn caches only')
-    if fp8 and (k_scale is None or v_scale is None):
-        raise ValueError(f'{fn}: float8_e4m3fn caches need k_scale and v_scale')
-    cdt = torch.float8_e4m3fn if fp8 else torch.float16
-    if (k_cache.dtype != cdt or v_cache.dtype != cdt or positions.dtype != torch.int64 or counts.dtype != torch.int64 or
-            (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
-        raise ValueError(f'{fn} takes fp16 or float8_e4m3fn caches (fp32 scales) and int64 positions and counts')
-    if k_cache.dim() != 4:
-        raise ValueError(f'{fn}: the caches must be (B, nkv, max_len, hd), got {tuple(k_cache.shape)}')
-    B = k_cache.shape[0] if page_table is None else (positions.shape[0] if positions.dim() == 1 else -1)
-    nkv = k_cache.shape[1]
-    rows, slots, max_len = _kv_layout(fn, k_cache, B, page_table)
-    if (v_cache.shape != k_cache.shape or tuple(positions.shape) != (B,) or tuple(counts.shape) != (B,) or
-            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
-        raise ValueError(f'{fn}: shapes caches {tuple(k_cache.shape)} / {tuple(v_cache.shape)}, positions '
-                         f'{tuple(positions.shape)}, counts {tuple(counts.shape)} do not agree')
-    return fp8, B, rows, max_len
+def _check_chunk(fn, positions, counts):
+    """The operand checks kv_append and prefill_attention share: positions and counts (B,) int64.  Returns B."""
+    if positions.dtype != torch.int64 or counts.dtype != torch.int64:
+        raise ValueError(f'{fn} takes int64 positions and counts')
+    if positions.dim() != 1 or counts.shape != positions.shape:
+        raise ValueError(f'{fn}: shapes positions {tuple(positions.shape)}, counts {tuple(counts.shape)} do not agree')
+    return positions.shape[0]
 
 
 def kv_append(k_new, v_new, k_cache, v_cache, positions, counts, k_scale=None, v_scale=None, page_table=None):
-    """quip_kv_append(_fp8) on torch tensors: token i of k_new / v_new (B, T, nkv, hd) fp16 to slot positions[b] + i of
-    one layer's caches (B, nkv, max_len, hd) for i < counts[b]; nothing else is written.  fp16 caches, or
-    float8_e4m3fn caches with fp32 k_scale / v_scale (B, nkv, max_len), quantized on the way.  CUDA, one device,
-    contiguous; positions / counts (B,) int64.  On the current stream.  page_table: page pools as in decode_attention
-    (quip_kv_append_paged(_fp8)); a slot whose page id lies outside the pool is not written."""
-    fp8, B, rows, max_len = _check_chunk('kv_append', k_cache, v_cache, positions, counts, k_scale, v_scale, page_table)
+    """quip_kv_append on torch tensors: token i of k_new / v_new (B, T, nkv, hd) fp16 to slot positions[b] + i of one
+    layer's caches (B, nkv, max_len, hd) for i < counts[b]; nothing else is written.  fp16 caches, or float8_e4m3fn
+    caches with fp32 k_scale / v_scale (B, nkv, max_len), quantized on the way.  CUDA, one device, contiguous;
+    positions / counts (B,) int64.  On the current stream.  page_table: page pools as in decode_attention; a slot whose
+    page id lies outside the pool is not written."""
+    B = _check_chunk('kv_append', positions, counts)
+    kv = _kv_cache('kv_append', k_cache, v_cache, k_scale, v_scale, page_table, B)
     if k_new.dtype != torch.float16 or v_new.dtype != torch.float16:
         raise ValueError('kv_append takes fp16 k_new / v_new')
-    nkv, hd = k_cache.shape[1], k_cache.shape[3]
-    if k_new.dim() != 4 or k_new.shape[0] != B or tuple(k_new.shape[2:]) != (nkv, hd) or v_new.shape != k_new.shape:
+    if (k_new.dim() != 4 or k_new.shape[0] != B or tuple(k_new.shape[2:]) != (kv.nkv, kv.hd) or
+            v_new.shape != k_new.shape):
         raise ValueError(f'kv_append: k_new {tuple(k_new.shape)} / v_new {tuple(v_new.shape)} must be (B, T, nkv, hd) '
                          f'for caches {tuple(k_cache.shape)}')
-    T = k_new.shape[1]
-    ts = (k_new, v_new, k_cache, v_cache, positions, counts) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('kv_append', ts, k_new.device)
-    lib, st = _lib.load(), torch.cuda.current_stream(k_new.device).cuda_stream
+    _check_cuda('kv_append', (k_new, v_new, k_cache, v_cache, k_scale, v_scale, positions, counts), k_new.device)
     with torch.cuda.device(k_new.device):
-        if page_table is not None and fp8:
-            _lib.check(lib.quip_kv_append_paged_fp8(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                    v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
-                                                    positions.data_ptr(), counts.data_ptr(), B, T, nkv, hd,
-                                                    *_paged_args(page_table, rows), st))
-        elif page_table is not None:
-            _lib.check(lib.quip_kv_append_paged(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(),
-                                                v_cache.data_ptr(), positions.data_ptr(), counts.data_ptr(), B, T, nkv,
-                                                hd, *_paged_args(page_table, rows), st))
-        elif fp8:
-            _lib.check(lib.quip_kv_append_fp8(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                              k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
-                                              counts.data_ptr(), B, T, nkv, hd, max_len, st))
-        else:
-            _lib.check(lib.quip_kv_append(k_new.data_ptr(), v_new.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                          positions.data_ptr(), counts.data_ptr(), B, T, nkv, hd, max_len, st))
+        _lib.check(_lib.load().quip_kv_append(C.byref(kv), k_new.data_ptr(), v_new.data_ptr(), positions.data_ptr(),
+                                              counts.data_ptr(), B, k_new.shape[1],
+                                              torch.cuda.current_stream(k_new.device).cuda_stream))
 
 
 def prefill_attention(q, k_cache, v_cache, positions, counts, scale, k_scale=None, v_scale=None, page_table=None):
-    """quip_prefill_attention(_fp8) on torch tensors: q (B, T, nh, hd) fp16 attends causally over one layer's caches
+    """quip_prefill_attention on torch tensors: q (B, T, nh, hd) fp16 attends causally over one layer's caches
     (B, nkv, max_len, hd), which already hold the chunk (kv_append): token i of row b over slots 0 .. positions[b] + i
     for i < counts[b]; rows i >= counts[b] are zero.  fp16 caches, or float8_e4m3fn caches with fp32 k_scale / v_scale.
     CUDA, one device, contiguous; positions / counts (B,) int64.  Returns (B, T, nh, hd) fp16, on the current stream.
-    page_table: page pools as in decode_attention (quip_prefill_attention_paged(_fp8))."""
-    fp8, B, rows, max_len = _check_chunk('prefill_attention', k_cache, v_cache, positions, counts, k_scale, v_scale,
-                                         page_table)
+    page_table: page pools as in decode_attention."""
+    B = _check_chunk('prefill_attention', positions, counts)
+    kv = _kv_cache('prefill_attention', k_cache, v_cache, k_scale, v_scale, page_table, B)
     if q.dtype != torch.float16 or q.dim() != 4:
         raise ValueError(f'prefill_attention: q must be (B, T, nh, hd) fp16, got {tuple(q.shape)} {q.dtype}')
     T, nh, hd = q.shape[1:]
-    nkv = k_cache.shape[1]
-    if q.shape[0] != B or k_cache.shape[3] != hd:
+    if q.shape[0] != B or kv.hd != hd:
         raise ValueError(f'prefill_attention: q {tuple(q.shape)} and caches {tuple(k_cache.shape)} do not agree')
-    ts = (q, k_cache, v_cache, positions, counts) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('prefill_attention', ts, q.device)
+    _check_cuda('prefill_attention', (q, k_cache, v_cache, k_scale, v_scale, positions, counts), q.device)
     out = torch.empty_like(q)
-    lib, st = _lib.load(), torch.cuda.current_stream(q.device).cuda_stream
     with torch.cuda.device(q.device):
-        if page_table is not None and fp8:
-            _lib.check(lib.quip_prefill_attention_paged_fp8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                            k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
-                                                            counts.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd,
-                                                            C.c_float(scale), *_paged_args(page_table, rows), st))
-        elif page_table is not None:
-            _lib.check(lib.quip_prefill_attention_paged(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                        positions.data_ptr(), counts.data_ptr(), out.data_ptr(), B, T,
-                                                        nh, nkv, hd, C.c_float(scale), *_paged_args(page_table, rows),
-                                                        st))
-        elif fp8:
-            _lib.check(lib.quip_prefill_attention_fp8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                      k_scale.data_ptr(), v_scale.data_ptr(), positions.data_ptr(),
-                                                      counts.data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len,
-                                                      C.c_float(scale), st))
-        else:
-            _lib.check(lib.quip_prefill_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                  positions.data_ptr(), counts.data_ptr(), out.data_ptr(), B, T, nh, nkv,
-                                                  hd, max_len, C.c_float(scale), st))
+        _lib.check(_lib.load().quip_prefill_attention(C.byref(kv), q.data_ptr(), positions.data_ptr(),
+                                                      counts.data_ptr(), out.data_ptr(), B, T, nh, C.c_float(scale),
+                                                      torch.cuda.current_stream(q.device).cuda_stream))
     return out
 
 
@@ -544,97 +439,61 @@ class RaggedChunk:
         self.seq_start = torch.tensor(offs, dtype=torch.int64).to(device)
 
 
-def _check_ragged(fn, k_pool, v_pool, seqs, positions, page_table, k_scale, v_scale):
-    """The checks kv_append_ragged and prefill_attention_ragged share: the chunk, pool and scale dtypes and shapes,
-    positions (S,) int64 and the page table (S, max_pages).  Returns (whether the pools are e4m3, n_pages)."""
+def _check_ragged(fn, seqs, positions, page_table, dev):
+    """The operand checks kv_append_ragged and prefill_attention_ragged share: the chunk, on the pools' device dev,
+    positions (S,) int64 and a page table."""
     if not isinstance(seqs, RaggedChunk):
         raise ValueError(f'{fn}: seqs must be a RaggedChunk (its offsets are checked when it is made)')
     if page_table is None:
         raise ValueError(f'{fn}: a ragged chunk is paged only: pass the page_table')
-    fp8 = k_pool.dtype == torch.float8_e4m3fn
-    if not fp8 and (k_scale is not None or v_scale is not None):
-        raise ValueError(f'{fn}: k_scale / v_scale go with float8_e4m3fn pools only')
-    if fp8 and (k_scale is None or v_scale is None):
-        raise ValueError(f'{fn}: float8_e4m3fn pools need k_scale and v_scale')
-    cdt = torch.float8_e4m3fn if fp8 else torch.float16
-    if (k_pool.dtype != cdt or v_pool.dtype != cdt or positions.dtype != torch.int64 or
-            (fp8 and (k_scale.dtype != torch.float32 or v_scale.dtype != torch.float32))):
-        raise ValueError(f'{fn} takes fp16 or float8_e4m3fn pools (fp32 scales) and int64 positions')
-    if k_pool.dim() != 4:
-        raise ValueError(f'{fn}: the pools must be (n_pages, nkv, {KV_PAGE}, hd), got {tuple(k_pool.shape)}')
-    if tuple(positions.shape) != (seqs.S,):
-        raise ValueError(f'{fn}: positions must be ({seqs.S},) for {seqs.S} sequences, got {tuple(positions.shape)}')
-    rows, slots, _ = _kv_layout(fn, k_pool, seqs.S, page_table)
-    nkv = k_pool.shape[1]
-    if (v_pool.shape != k_pool.shape or
-            (fp8 and (tuple(k_scale.shape) != (rows, nkv, slots) or v_scale.shape != k_scale.shape))):
-        raise ValueError(f'{fn}: shapes pools {tuple(k_pool.shape)} / {tuple(v_pool.shape)}, positions '
-                         f'{tuple(positions.shape)} do not agree with {seqs.S} sequences')
-    if seqs.seq_start.device != k_pool.device:
-        raise ValueError(f'{fn}: the chunk\'s offsets live on {seqs.seq_start.device}, the pools on {k_pool.device}')
-    return fp8, rows
+    if positions.dtype != torch.int64 or tuple(positions.shape) != (seqs.S,):
+        raise ValueError(f'{fn}: positions must be ({seqs.S},) int64 for {seqs.S} sequences, got '
+                         f'{tuple(positions.shape)} {positions.dtype}')
+    if seqs.seq_start.device != dev:
+        raise ValueError(f'{fn}: the chunk\'s offsets live on {seqs.seq_start.device}, the pools on {dev}')
 
 
 def kv_append_ragged(k_new, v_new, k_pool, v_pool, seqs, positions, page_table, k_scale=None, v_scale=None):
-    """quip_kv_append_ragged(_fp8) on torch tensors: packed row seq_start[s] + i of k_new / v_new (N, nkv, hd) fp16 --
-    token i of sequence s (seqs: a RaggedChunk) -- to slot positions[s] + i of row s of page_table (S, max_pages) int32,
-    in one layer's pools (n_pages, nkv, 64, hd): fp16, or float8_e4m3fn with fp32 k_scale / v_scale (n_pages, nkv, 64),
+    """quip_kv_append_ragged on torch tensors: packed row seq_start[s] + i of k_new / v_new (N, nkv, hd) fp16 -- token
+    i of sequence s (seqs: a RaggedChunk) -- to slot positions[s] + i of row s of page_table (S, max_pages) int32, in
+    one layer's pools (n_pages, nkv, 64, hd): fp16, or float8_e4m3fn with fp32 k_scale / v_scale (n_pages, nkv, 64),
     quantized on the way.  A sequence whose slots leave the cache, or a slot whose page id lies outside the pool, writes
     nothing.  CUDA, one device, contiguous; positions (S,) int64.  Everything is checked before the launch, which runs on
     the current stream."""
-    fp8, n_pages = _check_ragged('kv_append_ragged', k_pool, v_pool, seqs, positions, page_table, k_scale, v_scale)
+    _check_ragged('kv_append_ragged', seqs, positions, page_table, k_pool.device)
+    kv = _kv_cache('kv_append_ragged', k_pool, v_pool, k_scale, v_scale, page_table, seqs.S)
     if k_new.dtype != torch.float16 or v_new.dtype != torch.float16:
         raise ValueError('kv_append_ragged takes fp16 k_new / v_new')
-    nkv, hd = k_pool.shape[1], k_pool.shape[3]
-    if tuple(k_new.shape) != (seqs.N, nkv, hd) or v_new.shape != k_new.shape:
+    if tuple(k_new.shape) != (seqs.N, kv.nkv, kv.hd) or v_new.shape != k_new.shape:
         raise ValueError(f'kv_append_ragged: k_new {tuple(k_new.shape)} / v_new {tuple(v_new.shape)} must be '
-                         f'(N={seqs.N}, nkv={nkv}, hd={hd})')
-    ts = (k_new, v_new, k_pool, v_pool, positions) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('kv_append_ragged', ts, k_new.device)
-    lib, st = _lib.load(), torch.cuda.current_stream(k_new.device).cuda_stream
-    sizes = (seqs.S, seqs.N, seqs.max_count, nkv, hd)
+                         f'(N={seqs.N}, nkv={kv.nkv}, hd={kv.hd})')
+    _check_cuda('kv_append_ragged', (k_new, v_new, k_pool, v_pool, k_scale, v_scale, positions), k_new.device)
     with torch.cuda.device(k_new.device):
-        if fp8:
-            _lib.check(lib.quip_kv_append_ragged_fp8(k_new.data_ptr(), v_new.data_ptr(), k_pool.data_ptr(),
-                                                     v_pool.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
-                                                     seqs.seq_start.data_ptr(), positions.data_ptr(), *sizes,
-                                                     *_paged_args(page_table, n_pages), st))
-        else:
-            _lib.check(lib.quip_kv_append_ragged(k_new.data_ptr(), v_new.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
-                                                 seqs.seq_start.data_ptr(), positions.data_ptr(), *sizes,
-                                                 *_paged_args(page_table, n_pages), st))
+        _lib.check(_lib.load().quip_kv_append_ragged(C.byref(kv), k_new.data_ptr(), v_new.data_ptr(),
+                                                     seqs.seq_start.data_ptr(), positions.data_ptr(), seqs.S, seqs.N,
+                                                     seqs.max_count,
+                                                     torch.cuda.current_stream(k_new.device).cuda_stream))
 
 
 def prefill_attention_ragged(q, k_pool, v_pool, seqs, positions, page_table, scale, k_scale=None, v_scale=None):
-    """quip_prefill_attention_ragged(_fp8) on torch tensors: packed row seq_start[s] + i of q (N, nh, hd) fp16 -- token
-    i of sequence s (seqs: a RaggedChunk) -- attends causally over slots 0 .. positions[s] + i of row s of page_table
+    """quip_prefill_attention_ragged on torch tensors: packed row seq_start[s] + i of q (N, nh, hd) fp16 -- token i of
+    sequence s (seqs: a RaggedChunk) -- attends causally over slots 0 .. positions[s] + i of row s of page_table
     (S, max_pages), in one layer's pools that already hold the chunk (kv_append_ragged).  Returns (N, nh, hd) fp16, on
     the current stream.  Per sequence the result is bit-identical to prefill_attention with page_table, B = S,
     T = seqs.max_count and counts = the sequence lengths (include/quip_b200.h); a sequence that would read a slot
     outside the cache or a page outside the pool gets NaN.  Pools, scales and checks as kv_append_ragged."""
-    fp8, n_pages = _check_ragged('prefill_attention_ragged', k_pool, v_pool, seqs, positions, page_table, k_scale,
-                                 v_scale)
-    nkv, hd = k_pool.shape[1], k_pool.shape[3]
-    if q.dtype != torch.float16 or q.dim() != 3 or q.shape[0] != seqs.N or q.shape[2] != hd:
-        raise ValueError(f'prefill_attention_ragged: q must be (N={seqs.N}, nh, hd={hd}) fp16, got {tuple(q.shape)} '
-                         f'{q.dtype}')
-    nh = q.shape[1]
-    ts = (q, k_pool, v_pool, positions) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('prefill_attention_ragged', ts, q.device)
+    _check_ragged('prefill_attention_ragged', seqs, positions, page_table, k_pool.device)
+    kv = _kv_cache('prefill_attention_ragged', k_pool, v_pool, k_scale, v_scale, page_table, seqs.S)
+    if q.dtype != torch.float16 or q.dim() != 3 or q.shape[0] != seqs.N or q.shape[2] != kv.hd:
+        raise ValueError(f'prefill_attention_ragged: q must be (N={seqs.N}, nh, hd={kv.hd}) fp16, got '
+                         f'{tuple(q.shape)} {q.dtype}')
+    _check_cuda('prefill_attention_ragged', (q, k_pool, v_pool, k_scale, v_scale, positions), q.device)
     out = torch.empty_like(q)
-    lib, st = _lib.load(), torch.cuda.current_stream(q.device).cuda_stream
-    sizes = (seqs.S, seqs.N, seqs.max_count, nh, nkv, hd, C.c_float(scale))
     with torch.cuda.device(q.device):
-        if fp8:
-            _lib.check(lib.quip_prefill_attention_ragged_fp8(q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
-                                                             k_scale.data_ptr(), v_scale.data_ptr(),
-                                                             seqs.seq_start.data_ptr(), positions.data_ptr(),
-                                                             out.data_ptr(), *sizes, *_paged_args(page_table, n_pages),
-                                                             st))
-        else:
-            _lib.check(lib.quip_prefill_attention_ragged(q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
-                                                         seqs.seq_start.data_ptr(), positions.data_ptr(), out.data_ptr(),
-                                                         *sizes, *_paged_args(page_table, n_pages), st))
+        _lib.check(_lib.load().quip_prefill_attention_ragged(C.byref(kv), q.data_ptr(), seqs.seq_start.data_ptr(),
+                                                             positions.data_ptr(), out.data_ptr(), seqs.S, seqs.N,
+                                                             seqs.max_count, q.shape[1], C.c_float(scale),
+                                                             torch.cuda.current_stream(q.device).cuda_stream))
     return out
 
 
@@ -897,50 +756,36 @@ def beam_select(cand_s, cand_i, eos, budget, step, pen, st, K, V, early_stopping
 
 
 def kv_beam_fork(k_pool, v_pool, table, table_tmp, parents, lens, scratch0, k_scale=None, v_scale=None):
-    """quip_kv_beam_fork(_fp8): after a beam select, row r with parents[r] != r takes its parent's table entries for
-    the spans before its current one and a copy of its parent's slots 64 * cur .. lens[r] - 1 of the current span, in
-    every layer of the pools k_pool / v_pool (L, n_pages, nkv, 64, hd) (fp16, or float8_e4m3fn with fp32 k_scale /
-    v_scale (L, n_pages, nkv, 64)), through scratch pages scratch0 .. scratch0 + R - 1 (include/quip_b200.h).  table /
+    """quip_kv_beam_fork: after a beam select, row r with parents[r] != r takes its parent's table entries for the
+    spans before its current one and a copy of its parent's slots 64 * cur .. lens[r] - 1 of the current span, in every
+    layer of the pools k_pool / v_pool (L, n_pages, nkv, 64, hd) (fp16, or float8_e4m3fn with fp32 k_scale / v_scale
+    (L, n_pages, nkv, 64)), through scratch pages scratch0 .. scratch0 + R - 1 (include/quip_b200.h).  table /
     table_tmp (R, max_pages) int32, parents / lens (R,) int64.  CUDA, one device, contiguous; checked before the
     launches (two, on the current stream)."""
-    fp8 = k_pool.dtype == torch.float8_e4m3fn
-    if fp8 != (k_scale is not None) or (k_scale is None) != (v_scale is None):
-        raise ValueError('kv_beam_fork: float8_e4m3fn pools need k_scale and v_scale, fp16 pools take none')
-    if k_pool.dtype not in (torch.float16, torch.float8_e4m3fn) or v_pool.dtype != k_pool.dtype:
-        raise ValueError(f'kv_beam_fork: fp16 or float8_e4m3fn pools, got {k_pool.dtype} / {v_pool.dtype}')
-    if k_pool.dim() != 5 or k_pool.shape[3] != KV_PAGE or v_pool.shape != k_pool.shape:
+    fp8 = _kv_format('kv_beam_fork', k_pool, v_pool, k_scale, v_scale)
+    if k_pool.dim() != 5 or k_pool.shape[0] < 1 or k_pool.shape[3] != KV_PAGE or v_pool.shape != k_pool.shape:
         raise ValueError(f'kv_beam_fork: pools must be (L, n_pages, nkv, {KV_PAGE}, hd), got {tuple(k_pool.shape)} / '
                          f'{tuple(v_pool.shape)}')
     L, n_pages, nkv, _, hd = k_pool.shape
     if (hd * k_pool.element_size()) % 16:
         raise ValueError(f'kv_beam_fork: a head vector must be a multiple of 16 bytes, got hd {hd}')
-    if fp8 and (k_scale.dtype != torch.float32 or tuple(k_scale.shape) != (L, n_pages, nkv, KV_PAGE) or
-                v_scale.shape != k_scale.shape or v_scale.dtype != torch.float32):
+    if fp8 and (tuple(k_scale.shape) != (L, n_pages, nkv, KV_PAGE) or v_scale.shape != k_scale.shape):
         raise ValueError(f'kv_beam_fork: scales must be {(L, n_pages, nkv, KV_PAGE)} fp32')
     if table.dtype != torch.int32 or table.dim() != 2 or table_tmp.shape != table.shape or table_tmp.dtype != torch.int32:
         raise ValueError(f'kv_beam_fork: table and table_tmp must be (R, max_pages) int32, got {tuple(table.shape)} / '
                          f'{tuple(table_tmp.shape)}')
-    R, max_pages = table.shape
-    if max_pages < 1 or max_pages > (2 ** 31 - 1) // KV_PAGE:
-        raise ValueError(f'kv_beam_fork: {max_pages} pages per row')
+    R = table.shape[0]
     _check_i64('kv_beam_fork', parents=(parents, (R,)), lens=(lens, (R,)))
     if isinstance(scratch0, bool) or int(scratch0) != scratch0 or not 0 <= scratch0 <= n_pages - R:
         raise ValueError(f'kv_beam_fork: scratch pages {scratch0} .. {scratch0} + {R} - 1 lie outside the pool of '
                          f'{n_pages}')
-    ts = (k_pool, v_pool, table, table_tmp, parents, lens) + ((k_scale, v_scale) if fp8 else ())
-    _check_cuda('kv_beam_fork', ts, k_pool.device)
-    if k_pool.data_ptr() % 16 or v_pool.data_ptr() % 16:
-        raise ValueError('kv_beam_fork: the pools must be 16-byte aligned')
-    lib, stream = _lib.load(), torch.cuda.current_stream(k_pool.device).cuda_stream
-    sizes = (R, L, n_pages, nkv, hd, max_pages, int(scratch0), stream)
+    _check_cuda('kv_beam_fork', (k_pool, v_pool, k_scale, v_scale, table, table_tmp, parents, lens), k_pool.device)
+    kv = _kv_cache('kv_beam_fork', k_pool[0], v_pool[0], k_scale[0] if fp8 else None, v_scale[0] if fp8 else None,
+                   table, R)                                         # layer 0; the kernels step n_pages per layer
     with torch.cuda.device(k_pool.device):
-        if fp8:
-            _lib.check(lib.quip_kv_beam_fork_fp8(k_pool.data_ptr(), v_pool.data_ptr(), k_scale.data_ptr(),
-                                                 v_scale.data_ptr(), table.data_ptr(), table_tmp.data_ptr(),
-                                                 parents.data_ptr(), lens.data_ptr(), *sizes))
-        else:
-            _lib.check(lib.quip_kv_beam_fork(k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr(),
-                                             table_tmp.data_ptr(), parents.data_ptr(), lens.data_ptr(), *sizes))
+        _lib.check(_lib.load().quip_kv_beam_fork(C.byref(kv), L, table_tmp.data_ptr(), parents.data_ptr(),
+                                                 lens.data_ptr(), R, int(scratch0),
+                                                 torch.cuda.current_stream(k_pool.device).cuda_stream))
 
 
 PROC_MAX_V, PROC_MAX_EOS, PROC_MAX_BAD, PROC_BAD_LEN = 2 ** 18, 8, 256, 16

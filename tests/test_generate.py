@@ -125,12 +125,13 @@ def test_generate_rejects_bad_requests_before_any_work():
         dec.step()
 
 
-def test_decode_attention_argument_errors_surface_as_messages():
+def test_decode_attention_descriptor_argument_errors_surface_as_messages():
     lib = _lib.load()
     buf, ws = 64, 1 << 20
 
     def call(B=2, nh=8, nkv=2, hd=128, max_len=256, q=buf, pos=buf, wsb=ws, out=buf):
-        return lib.quip_decode_attention(q, buf, buf, buf, buf, pos, out, B, nh, nkv, hd, max_len, 1.0, buf, wsb, None)
+        kv = _lib.QuipKvCache(k=buf, v=buf, format=_lib.QUIP_KV_FP16, nkv=nkv, hd=hd, max_len=max_len)
+        return lib.quip_decode_attention(kv, q, buf, buf, pos, out, B, nh, 1.0, buf, wsb, None)
     assert call(hd=96) == 1 and b'head_dim 96' in lib.quip_last_error()
     assert call(nh=6, nkv=4) == 1 and b'nh % nkv' in lib.quip_last_error()
     assert call(nh=32, nkv=2) == 1 and b'at most 8' in lib.quip_last_error()

@@ -1,5 +1,5 @@
 """Beam search on the GPU: quip_beam_candidates against oracle/beam.py, quip_beam_select bit for bit against its torch
-restatement, quip_kv_beam_fork(_fp8) bit for bit against the torch fork on shuffled NaN-poisoned pools, the captured
+restatement, quip_kv_beam_fork (fp16 and e4m3) bit for bit against the torch fork on shuffled NaN-poisoned pools, the captured
 step against the eager one, and generate(num_beams=K) against the torch restatement on the tiny packed models, away
 from near ties."""
 import pytest

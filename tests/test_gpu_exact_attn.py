@@ -1,4 +1,4 @@
-"""The decode-attention kernels (quip_decode_attention and quip_decode_attention_fp8, csrc/attn_decode.cu) on exact
+"""The decode-attention kernels (quip_decode_attention on fp16 and e4m3 caches, csrc/attn_decode.cu) on exact
 cases (oracle/exact_attn.py), compared bit for bit with fp16_rn(fp32(O) / fp32(L)): every (cache dtype, head_dim, heads
 per kv head) instantiation at both chunk sizes, the cache after the append, a wide grid, the grid.z limit, positions
 out of range, and a stale workspace.  The cases are deterministic; tests/test_exact_attn_cases.py proves each one's
@@ -107,13 +107,13 @@ def run(c, ws=None):
         B, nh, nkv, hd, max_len = c.shape
         lib = _lib.load()
         out = torch.empty_like(d['q'])
-        p = [d[k].data_ptr() for k in ('q', 'kn', 'vn', 'kc', 'vc')]
-        tail = [d['pos'].data_ptr(), out.data_ptr(), B, nh, nkv, hd, max_len, C.c_float(c.scale), ws.data_ptr(),
-                ws.numel(), torch.cuda.current_stream().cuda_stream]
+        kv = _lib.QuipKvCache(k=d['kc'].data_ptr(), v=d['vc'].data_ptr(), nkv=nkv, hd=hd, max_len=max_len,
+                              format=_lib.QUIP_KV_E4M3 if c.fp8 else _lib.QUIP_KV_FP16)
         if c.fp8:
-            _lib.check(lib.quip_decode_attention_fp8(*p, d['ks'].data_ptr(), d['vs'].data_ptr(), *tail))
-        else:
-            _lib.check(lib.quip_decode_attention(*p, *tail))
+            kv.k_scale, kv.v_scale = d['ks'].data_ptr(), d['vs'].data_ptr()
+        _lib.check(lib.quip_decode_attention(C.byref(kv), *[d[k].data_ptr() for k in ('q', 'kn', 'vn', 'pos')],
+                                             out.data_ptr(), B, nh, C.c_float(c.scale), ws.data_ptr(), ws.numel(),
+                                             torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
     return out.cpu().numpy(), d
 
@@ -230,7 +230,7 @@ def stale_case(fp8):
 
 
 @pytest.mark.parametrize('fp8', [False, True], ids=['fp16', 'e4m3'])
-def test_combine_reads_only_partials_of_its_own_launch(fp8):
+def test_descriptor_launch_combine_reads_only_its_own_partials(fp8):
     """A workspace of NaN bytes (0xFF), then one left by a call with every row at max_len - 1 (all chunks written):
     both give the clean result bit for bit."""
     c = stale_case(fp8)

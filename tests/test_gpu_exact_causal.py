@@ -1,5 +1,5 @@
-"""The extend-attention kernel (quip_extend_attention(_fp8), csrc/attn_decode.cu) and kv_append + prefill attention
-(quip_kv_append(_fp8), quip_prefill_attention(_fp8), csrc/attn_prefill.cu) on exact multi-token cases
+"""The extend-attention kernel (quip_extend_attention, csrc/attn_decode.cu) and kv_append + prefill attention
+(quip_kv_append, quip_prefill_attention, csrc/attn_prefill.cu) on exact multi-token cases
 (oracle/exact_causal.py), compared bit for bit with fp16_rn(fp32(O) / fp32(L)): every (cache dtype, head_dim, heads per
 kv head) instantiation at tokens per row and positions that straddle 64-slot chunks, blocks and query tiles, wide and
 long grids, rows out of range, a stale workspace, and the kernels against each other.  The cases are deterministic;
@@ -179,13 +179,13 @@ def run(c, ws=None):
         B, T, nh, nkv, hd, max_len = c.shape
         lib = _lib.load()
         out = torch.empty_like(d['q'])
-        p = [d[k].data_ptr() for k in ('q', 'kn', 'vn', 'kc', 'vc')]
-        tail = [d['pos'].data_ptr(), out.data_ptr(), B, T, nh, nkv, hd, max_len, C.c_float(c.scale), ws.data_ptr(),
-                ws.numel(), torch.cuda.current_stream().cuda_stream]
+        kv = _lib.QuipKvCache(k=d['kc'].data_ptr(), v=d['vc'].data_ptr(), nkv=nkv, hd=hd, max_len=max_len,
+                              format=_lib.QUIP_KV_E4M3 if c.fp8 else _lib.QUIP_KV_FP16)
         if c.fp8:
-            _lib.check(lib.quip_extend_attention_fp8(*p, d['ks'].data_ptr(), d['vs'].data_ptr(), *tail))
-        else:
-            _lib.check(lib.quip_extend_attention(*p, *tail))
+            kv.k_scale, kv.v_scale = d['ks'].data_ptr(), d['vs'].data_ptr()
+        _lib.check(lib.quip_extend_attention(C.byref(kv), *[d[k].data_ptr() for k in ('q', 'kn', 'vn', 'pos')],
+                                             out.data_ptr(), B, T, nh, C.c_float(c.scale), ws.data_ptr(), ws.numel(),
+                                             torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
     return out.cpu().numpy(), d
 
@@ -306,7 +306,7 @@ def test_prefill_invalid_rows_give_nan_and_write_nothing(fp8, hd, G):
 
 # ---- stale workspace ----
 @pytest.mark.parametrize('fp8', [False, True], ids=['fp16', 'e4m3'])
-def test_extend_combine_reads_only_partials_of_its_own_launch(fp8):
+def test_extend_descriptor_launch_combine_reads_only_its_own_partials(fp8):
     """A workspace of NaN bytes (0xFF), then one left by a call with every row at max_len - T (all chunks written):
     both give the clean result bit for bit."""
     c = stale_case(fp8)

@@ -1,4 +1,4 @@
-"""The e4m3 KV cache on the GPU: quip_kv_quantize_fp8 and quip_decode_attention_fp8 (csrc/attn_decode.cu) against
+"""The e4m3 KV cache on the GPU: quip_kv_quantize_fp8 and quip_decode_attention on e4m3 caches (csrc/attn_decode.cu) against
 oracle/kvfp8.py, and PromptDecoder / generate with kv_dtype=torch.float8_e4m3fn on synthetic packed models."""
 import math
 

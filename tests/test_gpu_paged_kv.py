@@ -1,5 +1,5 @@
-"""Paged KV cache on the GPU: every paged kernel (quip_decode_attention_paged, quip_extend_attention_paged,
-quip_kv_append_paged, quip_prefill_attention_paged, each fp16 and e4m3) against its contiguous twin over the same cached
+"""Paged KV cache on the GPU: every paged kernel (quip_decode_attention, quip_extend_attention, quip_kv_append,
+quip_prefill_attention with a page table, each fp16 and e4m3) against its contiguous twin over the same cached
 bytes -- bit for bit, outputs and appended bytes and scales -- with pools built by scattering the contiguous cache into
 shuffled pages, unused pages NaN-poisoned and table entries past each row's slots unmapped; shared pages; the guard
 on page ids outside the pool; and the decoder and generate() end to end."""

@@ -16,7 +16,7 @@ from quip_b200 import quant as Q
 from quip_b200.incoherence import plan_side
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_of_abi_v3():
     header = open(os.path.join(ROOT, 'include', 'quip_b200.h')).read()
     declared = set(re.findall(r'\b(quip_[a-z_0-9]+)\s*\(', header))
     assert declared, 'no declarations parsed'
@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f'{name} declared in include/quip_b200.h but not exported'
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
-    assert lib.quip_abi_version() == _lib.ABI_VERSION == 2
+    assert lib.quip_abi_version() == _lib.ABI_VERSION == 3
     assert lib.quip_packed_words(16, 128, 2) == 128
     assert lib.quip_packed_words(16, 128, 3) == 192
     assert lib.quip_packed_words(16, 100, 2) == 0          # bad shape -> 0
@@ -187,14 +187,14 @@ def test_fragment_order_matches_the_header_formula():
             assert frag[word, 0] == F_[blk, row, k0] and frag[word, 1] == F_[blk, row, k0 + 1]
 
 
-def test_abi_v2_structs_carry_the_optional_pointers():
+def test_abi_v3_keeps_the_optional_pointers_of_v2():
     from quip_b200 import _lib
     assert 'factors_frag' in [n for n, _ in _lib.QuipPass._fields_]
     assert 'inv_idx' in [n for n, _ in _lib.QuipSide._fields_]
     s = _lib.QuipSide()
     assert not s.inv_idx and not s.passes[0].factors_frag          # NULL by default: the C side takes the unfused routes
     hdr = open(os.path.join(ROOT, 'include', 'quip_b200.h')).read()
-    assert 'QUIP_ABI_VERSION 2' in hdr and 'factors_frag' in hdr and 'inv_idx' in hdr
+    assert 'QUIP_ABI_VERSION 3' in hdr and 'factors_frag' in hdr and 'inv_idx' in hdr
 
 
 def test_committed_bench_line_has_the_contract_keys():

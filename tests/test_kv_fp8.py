@@ -1,6 +1,6 @@
 """The e4m3 KV cache of generation (PromptDecoder / generate with kv_dtype=torch.float8_e4m3fn) on tiny fp32 HF models on
-the CPU, where the step is the torch restatement of quip_decode_attention_fp8, against oracle/kvfp8.py and an fp32-cache
-decoder; and the argument checks of the two fp8 entry points of the C ABI."""
+the CPU, where the step is the torch restatement of quip_decode_attention on an e4m3 cache, against oracle/kvfp8.py and an
+fp32-cache decoder; and the argument checks of the C ABI on e4m3 caches."""
 import ctypes as C
 
 import pytest
@@ -148,14 +148,15 @@ def test_kv_dtype_choices():
         generate(m, _prompts()[:1], 2, kv_dtype=torch.int8)
 
 
-def test_fp8_entry_points_argument_errors_surface_as_messages():
+def test_e4m3_cache_descriptor_argument_errors_surface_as_messages():
     lib = _lib.load()
     buf, ws = 64, 1 << 20
 
     def call(B=2, nh=8, nkv=2, hd=128, max_len=256, q=buf, ks=buf, vs=buf, pos=buf, wsb=ws, out=buf, kc=buf):
-        return lib.quip_decode_attention_fp8(q, buf, buf, kc, buf, ks, vs, pos, out, B, nh, nkv, hd, max_len, 1.0, buf,
-                                             wsb, None)
-    assert call(hd=96) == 1 and b'quip_decode_attention_fp8: head_dim 96' in lib.quip_last_error()
+        kv = _lib.QuipKvCache(k=kc, v=buf, k_scale=ks, v_scale=vs, format=_lib.QUIP_KV_E4M3, nkv=nkv, hd=hd,
+                              max_len=max_len)
+        return lib.quip_decode_attention(kv, q, buf, buf, pos, out, B, nh, 1.0, buf, wsb, None)
+    assert call(hd=96) == 1 and b'quip_decode_attention: head_dim 96' in lib.quip_last_error()
     assert call(nh=6, nkv=4) == 1 and b'nh % nkv' in lib.quip_last_error()
     assert call(nh=32, nkv=2) == 1 and b'at most 8' in lib.quip_last_error()
     assert call(q=None) == 1 and b'null' in lib.quip_last_error()
@@ -170,6 +171,15 @@ def test_fp8_entry_points_argument_errors_surface_as_messages():
     assert call(B=0, wsb=0) == 0
     with pytest.raises(_lib.QuipError, match='head_dim'):
         _lib.check(call(hd=32))
+    # the format is stated, never inferred from the scales
+    fp16 = _lib.QuipKvCache(k=buf, v=buf, k_scale=buf, v_scale=buf, format=_lib.QUIP_KV_FP16, nkv=2, hd=128, max_len=256)
+    assert lib.quip_decode_attention(fp16, buf, buf, buf, buf, buf, 2, 8, 1.0, buf, ws, None) == 1
+    assert b'given for an fp16 cache' in lib.quip_last_error()
+    fp16.format = 0
+    assert lib.quip_decode_attention(fp16, buf, buf, buf, buf, buf, 2, 8, 1.0, buf, ws, None) == 1
+    assert b'format 0' in lib.quip_last_error()
+    assert lib.quip_decode_attention(None, buf, buf, buf, buf, buf, 2, 8, 1.0, buf, ws, None) == 1
+    assert b'null cache descriptor' in lib.quip_last_error()
 
     def quant(src=buf, cache=buf, scales=buf, B=2, nkv=4, P=10, max_len=16, hd=64):
         return lib.quip_kv_quantize_fp8(src, cache, scales, B, nkv, P, max_len, hd, None)

@@ -265,19 +265,31 @@ def test_argument_errors_are_raised_before_any_work(monkeypatch):
         PromptDecoder(m, max_len=8, batch=1, page_table=[[0]])
 
 
-def test_paged_entry_points_check_their_table_before_any_launch():
+def test_cache_descriptors_check_their_page_table_before_any_launch():
     lib = _lib.load()
     buf, ws = 64, 1 << 20
     B, nh, nkv, hd = 2, 8, 2, 128
     for table, mp, n, what in ((None, 4, 8, 'page_table'), (buf + 2, 4, 8, 'page_table'), (buf, 0, 8, 'max_pages'),
                                (buf, 1 << 26, 8, 'max_pages'), (buf, 4, 0, 'n_pages')):
-        calls = [lib.quip_decode_attention_paged(buf, buf, buf, buf, buf, buf, buf, B, nh, nkv, hd, 1.0, buf, ws, table,
-                                                 mp, n, None),
-                 lib.quip_extend_attention_paged_fp8(buf, buf, buf, buf, buf, buf, buf, buf, buf, B, 2, nh, nkv, hd, 1.0,
-                                                     buf, ws, table, mp, n, None),
-                 lib.quip_kv_append_paged(buf, buf, buf, buf, buf, buf, B, 2, nkv, hd, table, mp, n, None),
-                 lib.quip_prefill_attention_paged_fp8(buf, buf, buf, buf, buf, buf, buf, buf, B, 2, nh, nkv, hd, 1.0,
-                                                      table, mp, n, None)]
-        for code in calls:
-            assert code != 0
-            assert 'page_table' in lib.quip_last_error().decode(), what
+        def kv(fp8):
+            return _lib.QuipKvCache(k=buf, v=buf, k_scale=buf if fp8 else None, v_scale=buf if fp8 else None,
+                                    format=_lib.QUIP_KV_E4M3 if fp8 else _lib.QUIP_KV_FP16, nkv=nkv, hd=hd,
+                                    page_table=table, max_pages=mp, n_pages=n)
+        # ragged launches and the fork are paged only: a null table is refused; elsewhere it means contiguous
+        calls = {'quip_kv_append_ragged': lambda: lib.quip_kv_append_ragged(kv(False), buf, buf, buf, buf, B, 4, 2, None),
+                 'quip_prefill_attention_ragged':
+                     lambda: lib.quip_prefill_attention_ragged(kv(True), buf, buf, buf, buf, B, 4, 2, nh, 1.0, None),
+                 'quip_kv_beam_fork': lambda: lib.quip_kv_beam_fork(kv(True), 1, buf, buf, buf, B, 0, None)}
+        if table is not None:
+            calls.update({
+                'quip_decode_attention':
+                    lambda: lib.quip_decode_attention(kv(False), buf, buf, buf, buf, buf, B, nh, 1.0, buf, ws, None),
+                'quip_extend_attention':
+                    lambda: lib.quip_extend_attention(kv(True), buf, buf, buf, buf, buf, B, 2, nh, 1.0, buf, ws, None),
+                'quip_kv_append': lambda: lib.quip_kv_append(kv(False), buf, buf, buf, buf, B, 2, None),
+                'quip_prefill_attention':
+                    lambda: lib.quip_prefill_attention(kv(True), buf, buf, buf, buf, B, 2, nh, 1.0, None)})
+        for fn, call in calls.items():
+            assert call() != 0
+            msg = lib.quip_last_error().decode()
+            assert msg.startswith(fn + ':') and 'page_table' in msg, (what, msg)

@@ -130,22 +130,23 @@ def test_chunk_size_is_checked_before_any_work():
             PromptDecoder(m, max_len=8, batch=1).prefill([p], chunk=bad)
 
 
-def test_prefill_attention_and_append_argument_errors_surface_as_messages():
+def test_prefill_attention_and_append_descriptor_argument_errors_surface_as_messages():
     lib = _lib.load()
     buf = 64
 
-    def attn(fp8=False, B=2, T=4, nh=8, nkv=2, hd=128, max_len=256, q=buf, cnt=buf, ks=buf):
+    def cache(fp8, nkv, hd, max_len, ks=buf, vs=buf):
         if fp8:
-            return lib.quip_prefill_attention_fp8(q, buf, buf, ks, buf, buf, cnt, buf, B, T, nh, nkv, hd, max_len, 1.0,
-                                                  None)
-        return lib.quip_prefill_attention(q, buf, buf, buf, cnt, buf, B, T, nh, nkv, hd, max_len, 1.0, None)
+            return _lib.QuipKvCache(k=buf, v=buf, k_scale=ks, v_scale=vs, format=_lib.QUIP_KV_E4M3, nkv=nkv, hd=hd,
+                                    max_len=max_len)
+        return _lib.QuipKvCache(k=buf, v=buf, format=_lib.QUIP_KV_FP16, nkv=nkv, hd=hd, max_len=max_len)
+
+    def attn(fp8=False, B=2, T=4, nh=8, nkv=2, hd=128, max_len=256, q=buf, cnt=buf, ks=buf):
+        return lib.quip_prefill_attention(cache(fp8, nkv, hd, max_len, ks=ks), q, buf, cnt, buf, B, T, nh, 1.0, None)
 
     def append(fp8=False, B=2, T=4, nkv=2, hd=128, max_len=256, kn=buf, cnt=buf, vs=buf):
-        if fp8:
-            return lib.quip_kv_append_fp8(kn, buf, buf, buf, buf, vs, buf, cnt, B, T, nkv, hd, max_len, None)
-        return lib.quip_kv_append(kn, buf, buf, buf, buf, cnt, B, T, nkv, hd, max_len, None)
+        return lib.quip_kv_append(cache(fp8, nkv, hd, max_len, vs=vs), kn, buf, buf, cnt, B, T, None)
     for fp8 in (False, True):
-        name = b'quip_prefill_attention' + (b'_fp8' if fp8 else b'')
+        name = b'quip_prefill_attention: '
         assert attn(fp8, hd=96) == 1 and b'head_dim 96' in lib.quip_last_error()
         assert name in lib.quip_last_error()
         assert attn(fp8, nh=32, nkv=2) == 1 and b'at most 8' in lib.quip_last_error()
@@ -156,7 +157,7 @@ def test_prefill_attention_and_append_argument_errors_surface_as_messages():
         assert attn(fp8, cnt=None) == 1 and b'null' in lib.quip_last_error()
         assert attn(fp8, q=68) == 1 and b'aligned' in lib.quip_last_error()
         assert attn(fp8, B=0) == 0                                    # no rows: nothing to launch
-        name = b'quip_kv_append' + (b'_fp8' if fp8 else b'')
+        name = b'quip_kv_append: '
         assert append(fp8, hd=96) == 1 and b'head_dim 96' in lib.quip_last_error()
         assert name in lib.quip_last_error()
         assert append(fp8, T=0) == 1 and b'tokens per row' in lib.quip_last_error()

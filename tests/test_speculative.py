@@ -196,13 +196,15 @@ def test_generate_rejects_bad_speculation_settings():
     generate(_model('opt_pre_ln'), [p], 32, prompt_lookup_num_tokens=3)       # exactly the table
 
 
-def test_new_abi_argument_errors_surface_as_messages():
+def test_spec_abi_argument_errors_surface_as_messages():
     import ctypes as C
     lib = _lib.load()
     buf, ws = 64, 1 << 20
 
-    def ext(B=2, T=4, nh=8, nkv=2, hd=128, max_len=256, q=buf, wsb=ws, out=buf):
-        return lib.quip_extend_attention(q, buf, buf, buf, buf, buf, out, B, T, nh, nkv, hd, max_len, 1.0, buf, wsb, None)
+    def ext(B=2, T=4, nh=8, nkv=2, hd=128, max_len=256, q=buf, wsb=ws, out=buf, fmt=_lib.QUIP_KV_FP16, ks=None):
+        kv = _lib.QuipKvCache(k=buf, v=buf, k_scale=ks, v_scale=buf if ks else None, format=fmt, nkv=nkv, hd=hd,
+                              max_len=max_len)
+        return lib.quip_extend_attention(kv, q, buf, buf, buf, out, B, T, nh, 1.0, buf, wsb, None)
     assert ext(hd=96) == 1 and b'head_dim 96' in lib.quip_last_error()
     assert ext(T=9) == 1 and b'1 <= T <= 8' in lib.quip_last_error()
     assert ext(T=0) == 1 and b'1 <= T <= 8' in lib.quip_last_error()
@@ -214,8 +216,7 @@ def test_new_abi_argument_errors_surface_as_messages():
     assert ext(wsb=need.value - 1) == 1 and b'workspace' in lib.quip_last_error()
     assert lib.quip_extend_attention_workspace_bytes(2, 9, 8, 128, 256, C.byref(need)) == 1
     assert ext(B=0, wsb=0) == 0
-    assert lib.quip_extend_attention_fp8(buf, buf, buf, buf, buf, None, buf, buf, buf, 2, 4, 8, 2, 128, 256, 1.0, buf, ws,
-                                         None) == 1 and b'null' in lib.quip_last_error()
+    assert ext(fmt=_lib.QUIP_KV_E4M3) == 1 and b'null' in lib.quip_last_error()
     assert lib.quip_ngram_draft(buf, buf, buf, 2, 16, 3, 0, 3, None) == 1 and b'n_min' in lib.quip_last_error()
     assert lib.quip_ngram_draft(None, buf, buf, 2, 16, 3, 1, 3, None) == 1 and b'null' in lib.quip_last_error()
     assert lib.quip_spec_accept(buf, buf, buf, buf, buf, buf, buf, 2, 4, 9, 8, 32, None) == 1

@@ -19,7 +19,7 @@ T = 0.7, k = 50, p = 0.9 and at k = 0, p = 0.9, next to torch.argmax and the tor
 softmax, cumsum, top-p mask, multinomial) on the same rows, and a 7B PromptDecoder step at B = 32, context 2048, greedy
 against sampling, alternated over three trials.
 
-Section spec measures speculative generation: quip_extend_attention(_fp8) alone next to quip_decode_attention(_fp8)
+Section spec measures speculative generation: quip_extend_attention alone next to quip_decode_attention (fp16 and e4m3)
 (B in {1, 8}, T in {1, 4, 8}, contexts 2048 / 4096, every row's new slots ending at the context); the captured
 SpecDecoder step at T in {2, 4, 5, 6, 8} against the PromptDecoder step on the 7B shape at B in {1, 4}, context 2048
 (t_T / t_1 is the break-even number of tokens a step must yield); and generate() end to end, plain against
@@ -115,7 +115,7 @@ def attn_bytes(positions, nkv, hd, fp8=False):
 
 
 def kernel_alone_fp8(nh, nkv, hd, B, ctx, reps):
-    """quip_decode_attention_fp8 at every row's position ctx-1 of an e4m3 cache of ctx slots; rel err against the fp16
+    """quip_decode_attention on an e4m3 cache at every row's position ctx-1 of an e4m3 cache of ctx slots; rel err against the fp16
     kernel on the unquantized cache."""
     from quip_b200 import fused
     g = torch.Generator(device='cuda').manual_seed(0)
@@ -303,7 +303,7 @@ def decode_steps_fp8(model, B, ctx, steps, trials=2, kinds=('fp16', 'fp8')):
 
 
 def extend_alone(nh, nkv, hd, B, T, ctx, fp8, reps):
-    """quip_extend_attention(_fp8) with every row's T new slots ending at slot ctx - 1, and quip_decode_attention(_fp8)
+    """quip_extend_attention with every row's T new slots ending at slot ctx - 1, and quip_decode_attention
     at position ctx - 1 on the same cache."""
     from quip_b200 import fused
     g = torch.Generator(device='cuda').manual_seed(0)
@@ -481,7 +481,7 @@ def causal_flops(nh, hd, B, pos, T):
 
 
 def prefill_kernel_alone(nh, nkv, hd, B, T, fp8, reps):
-    """quip_prefill_attention(_fp8) of T tokens per row at position 0 (the cache already appended), in causal TFLOP/s,
+    """quip_prefill_attention of T tokens per row at position 0 (the cache already appended), in causal TFLOP/s,
     next to F.scaled_dot_product_attention(is_causal=True) on the same fp16 q / k / v (GQA expanded outside the
     timing)."""
     from quip_b200 import fused
