@@ -368,6 +368,41 @@ int quip_logits_process(void* logits, int64_t ld, int32_t R, int32_t T, int32_t 
                         int32_t n_eos, const int64_t* bad, const int32_t* bad_len, int32_t n_bad, int32_t B,
                         int32_t max_len, void* stream);
 
+/* Constrained generation (HF's PrefixConstrainedLogitsProcessor, which runs right after the processors above) by a
+ * token automaton on the device.  The table packs S states: offsets (S + 1) int32, ids (nnz) int32 and next (nnz)
+ * int32; state s allows ids[k] and leads to next[k] for k in [lo_s, hi_s), lo_s = clamp(offsets[s], 0, nnz),
+ * hi_s = clamp(offsets[s + 1], lo_s, nnz).  Several automata (one per prompt) share one table with disjoint state
+ * ranges.  The host validates the table (offsets[0] = 0 and non-decreasing, ids strictly increasing within a state,
+ * next in [0, S), every state non-empty); the kernels never read outside it whatever it holds.
+ *   delta(s, v) = next[k] if ids[k] == v for some k in [lo_s, hi_s), else s: a token without a transition (possible
+ *   only when the masked row had no finite allowed entry, e.g. min_new_tokens banning an EOS-only state) leaves the
+ *   state unchanged.  For s outside [0, S), delta(s, v) = s.
+ *
+ * quip_constrain_mask, in place on fp16 logits (R, V) with row stride ld (elements; rows need only 2-byte alignment):
+ * logits row r is offset i = r % T of decoder row b = rows[r / T] (rows (R / T) int64; null: b = r / T), with
+ * s_0 = state[b] (state (B) int32; -1 marks an unconstrained row) and s_j = delta(s_{j-1}, tokens[b, j]) for
+ * j = 1 .. i (tokens (B, T) int64, the speculative step's current token and drafts; may be null when T = 1).  A row
+ * with b outside [0, B) or s_i outside [0, S) is not touched, bit for bit.  Otherwise every x_v, v in [0, V), becomes
+ * x_v + (v allowed in s_i ? +0 : -inf) in fp16: HF's scores + mask, so an allowed -0 becomes +0 and a disallowed +inf or
+ * NaN becomes NaN (each sum is exact).  Table ids outside [0, V) allow nothing.
+ *
+ * quip_constrain_advance moves the state over the tokens a step commits: for n in [0, N), b = rows[n] (rows (N) int64,
+ * distinct; null: b = n), skipped when outside [0, B); c = counts[n] (counts (N) int64; null: T) clamped to [0, T];
+ * state[b] <- delta(... delta(state[b], tok[n * ld + 0]) ..., tok[n * ld + c - 1]) (tok int64, row stride ld >= T).
+ * A plain step passes its selected tokens (T = 1), a speculative step the targets (B, T) with counts = the tokens
+ * quip_spec_accept appended, a continuous step its rows with counts = 1 for live rows and 0 otherwise.
+ *
+ * Both launches depend on (R, T, V, B, S, nnz) and (N, T, B, S, nnz) only, so one captured graph serves every step.
+ * Mask: one CTA per logits row, a V-bit shared-memory bitmap of the allowed ids, no workspace.  Advance: one thread
+ * per entry.  Bounds: 1 <= V <= 2^18, 1 <= T <= 8 dividing R, ld >= V, S >= 0, nnz >= 0; int64 arrays 8-byte and int32
+ * arrays 4-byte aligned. */
+int quip_constrain_mask(void* logits, int64_t ld, int32_t R, int32_t T, int32_t V, const int64_t* rows,
+                        const int64_t* tokens, const int32_t* state, int32_t B, const int32_t* offsets,
+                        const int32_t* ids, const int32_t* next, int32_t S, int32_t nnz, void* stream);
+int quip_constrain_advance(int32_t* state, int32_t B, const int64_t* tok, int64_t ld, int32_t N, int32_t T,
+                           const int64_t* rows, const int64_t* counts, const int32_t* offsets, const int32_t* ids,
+                           const int32_t* next, int32_t S, int32_t nnz, void* stream);
+
 /* Beam search (HF's GenerationMixin._beam_search, prompt by prompt).  B prompts of K beams each are the rows
  * r = b * K + j (2 <= K <= 16 in generate).  C = max(2, 1 + n_eos) * K <= 64 candidates per prompt.
  *

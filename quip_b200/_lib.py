@@ -96,6 +96,10 @@ EXPORTS = {
     'quip_beam_select': (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 16 + [C.c_int32] * 7 + [C.c_void_p]),
     'quip_logits_process': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_int32] * 3 + [C.c_void_p] * 9 + [C.c_int32] +
                             [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p]),
+    'quip_constrain_mask': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int32] +
+                            [C.c_void_p] * 3 + [C.c_int32] * 2 + [C.c_void_p]),
+    'quip_constrain_advance': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32] +
+                               [C.c_void_p] * 5 + [C.c_int32] * 2 + [C.c_void_p]),
     'quip_ngram_draft':(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p]),
     'quip_spec_accept': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -27,6 +27,7 @@ acceptance by csrc/spec.cu.  `ContinuousDecoder` (generate(..., max_batch_size=n
 holds a decode row and its own pages only while it runs, and queued prompts join through ragged mixed steps
 (csrc/attn_prefill.cu's ragged kernels), scheduled by `ContinuousSchedule`.
 """
+import bisect
 import collections
 import heapq
 import math
@@ -34,6 +35,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .constrain import pack_automata
 from .fused import PROC_BAD_LEN, PROC_MAX_BAD, PROC_MAX_EOS, TOPK_MAX_N
 
 KV_PAGE = 64                                           # slots per page of a paged KV cache (include/quip_b200.h)
@@ -426,12 +428,19 @@ class PromptDecoder(GraphDecoder):
         processors in place, from device buffers filled by set_processing, over the row's history `hist` (B, max_len):
         the prompt by position (written by prefill) and each selected token (written inside the step).  On the CPU the
         same rule in torch (_process_torch).  Needs max_new >= 1;
+      * constraint=True: after the processors, quip_constrain_mask (csrc/constrain.cu; the rule is in
+        include/quip_b200.h) masks each row to the tokens its token-automaton state `cstate` (B,) int32 allows (-1:
+        unconstrained), and after the selection quip_constrain_advance moves the state over the committed token.  The
+        table and each row's start state come from set_constraint; a row restarts at its start state at its first
+        generated token.  On the CPU the same rule in torch (_constrain_torch, _constrain_advance_torch).  Needs
+        max_new >= 1;
       * logprobs=n (0 .. 20; default None: off, nothing allocated or launched): after the selection,
         quip_token_topk_logprobs (csrc/topk_logprobs.cu; the rule is in include/quip_b200.h) writes the raw logprob of
         each selected token, and with n >= 1 the n most likely ids and their logprobs, into lp (B, max_new), top_ids and
         top_lp (B, max_new, n) at the token's column of generated.  Raw: log_softmax of the head's fp16 logits before
         any processor or temperature; with processing=True the step first copies the rows the processors change in
-        place.  On the CPU the same rule in torch (_token_topk_logprobs_torch).  Needs max_new >= 1;
+        place (with constraint=True, that the mask changes).  On the CPU the same rule in torch
+        (_token_topk_logprobs_torch).  Needs max_new >= 1;
       * kv_dtype=torch.float8_e4m3fn: k_cache / v_cache e4m3 with k_scale / v_scale (L, B, nkv, max_len) fp32, one scale
         per cached head vector.  prefill quantizes the model's keys and values into slots 0 .. P-1
         (quip_kv_quantize_fp8); the step quantizes k / v on append (quip_decode_attention_fp8) and attends over the
@@ -447,7 +456,7 @@ class PromptDecoder(GraphDecoder):
     The whole model, no layer pipeline."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=0, ops=None, kv_dtype=None, sampling=False,
-                 page_table=None, n_pages=None, processing=False, logprobs=None):
+                 page_table=None, n_pages=None, processing=False, logprobs=None, constraint=False):
         if n_pages is None and page_table is not None:
             raise ValueError('a page_table needs n_pages, the size of the page pool')
         self.n_pages = None if n_pages is None else int(n_pages)
@@ -485,6 +494,13 @@ class PromptDecoder(GraphDecoder):
             self.penalty = torch.ones(B, dtype=torch.float32, device=self.dev)
             self.ngram, self.min_new = z(B, dt=torch.int32), z(B, dt=torch.int32)
             self.proc_eos, self.bad, self.bad_len = z(0), z(0, PROC_BAD_LEN), z(0, dt=torch.int32)
+        self.constrained = bool(constraint)
+        if self.constrained:
+            if self.max_new < 1:
+                raise ValueError('constraint=True acts between the head and the selection: max_new must be at least 1')
+            i32 = lambda *shape, v=0: torch.full(shape, v, dtype=torch.int32, device=self.dev)
+            self.cstate, self.cstart = i32(B, v=-1), i32(B, v=-1)
+            self.c_offsets, self.c_ids, self.c_next = i32(1), i32(0), i32(0)
         self.lp = self.top_ids = self.top_lp = None
         if logprobs is not None:
             if isinstance(logprobs, bool) or int(logprobs) != logprobs or not 0 <= logprobs <= TOPK_MAX_N:
@@ -538,6 +554,54 @@ class PromptDecoder(GraphDecoder):
         else:
             _process_torch(*args, tokens=tokens, rows=rows)
 
+    def set_constraint(self, offsets, ids, next, starts=None):
+        """Write a packed token-automaton table (constrain.pack_automata: offsets (S + 1,), ids and next (nnz,) int32)
+        into the device buffers a captured step reads and, given starts (one table state per row, -1: unconstrained),
+        each row's start state.  Once a step is captured, S and nnz are fixed."""
+        if not self.constrained:
+            raise ValueError('set_constraint needs a PromptDecoder made with constraint=True')
+        table = (offsets, ids, next)
+        if self.graph is None:
+            self.c_offsets, self.c_ids, self.c_next = (t.to(torch.int32).to(self.dev) for t in table)
+        elif offsets.numel() != self.c_offsets.numel() or ids.numel() != self.c_ids.numel():
+            raise ValueError(f'the captured step reads a table of {self.c_offsets.numel() - 1} states and '
+                             f'{self.c_ids.numel()} transitions; got {offsets.numel() - 1} and {ids.numel()}')
+        else:
+            for dst, t in zip((self.c_offsets, self.c_ids, self.c_next), table):
+                dst.copy_(t)
+        if starts is not None:
+            if len(starts) != self.batch:
+                raise ValueError(f'{len(starts)} start states for a decoder of batch {self.batch}')
+            self.cstart.copy_(torch.tensor(starts, dtype=torch.int32))
+            self.cstate.copy_(self.cstart)
+
+    def _constrain(self, logits, rows=None, tokens=None):
+        """With constraint=True, the token-automaton mask in place on logits (R, vocab) or (B, T, vocab): each logits
+        row at its decoder row's state cstate[b] (rows: the decoder row of each logits row), walked over the drafts
+        tokens[b, 1 ..] when T > 1."""
+        if not self.constrained:
+            return
+        x = logits.reshape(-1, logits.shape[-1])
+        T = 1 if tokens is None else tokens.shape[1]
+        args = (x, T, self.cstate, self.c_offsets, self.c_ids, self.c_next)
+        if self._kernel:
+            from . import fused
+            fused.constrain_mask(*args, tokens=tokens, rows=rows)
+        else:
+            _constrain_torch(*args, tokens=tokens, rows=rows)
+
+    def _constrain_advance(self, tokens, counts=None, rows=None):
+        """With constraint=True, each row's state moved over the first counts[n] (default all) of the committed tokens
+        (N, T) of entry n, the decoder row rows[n] (default n)."""
+        if not self.constrained:
+            return
+        args = (self.cstate, tokens, self.c_offsets, self.c_ids, self.c_next)
+        if self._kernel:
+            from . import fused
+            fused.constrain_advance(*args, counts=counts, rows=rows)
+        else:
+            _constrain_advance_torch(*args, counts=counts, rows=rows)
+
     def _hist_append(self, rows, tok, live=None):
         """hist[rows, positions[rows]] = tok (where live), at positions below max_len."""
         pos = self.positions[rows]
@@ -546,8 +610,8 @@ class PromptDecoder(GraphDecoder):
         self.hist[rows, col] = torch.where(ok, tok, self.hist[rows, col])
 
     def _raw(self, logits):
-        """The logits the logprobs read: a copy when the processors are about to change them in place."""
-        return logits.clone() if self.lp is not None and self.processing else logits
+        """The logits the logprobs read: a copy when the processors or the mask are about to change them in place."""
+        return logits.clone() if self.lp is not None and (self.processing or self.constrained) else logits
 
     def _logprobs(self, logits, tokens, cols, rows=None):
         """With logprobs on: the raw logprob of tokens (R,) or (B, T) and the top n of logits (R, vocab) or
@@ -773,6 +837,7 @@ class PromptDecoder(GraphDecoder):
         raw = self._raw(self.logits)
         if self.processing:
             self._process(self.logits, self.positions)                 # the token just fed is hist[b, positions[b]]
+        self._constrain(self.logits)
         self.positions.add_(1)
         if self.max_new:
             self._select(self.logits)
@@ -780,6 +845,7 @@ class PromptDecoder(GraphDecoder):
             self.generated.index_copy_(1, self._t, self.tokens[:, None])
             if self.processing:
                 self._hist_append(self._rows, self.tokens)
+            self._constrain_advance(self.tokens[:, None])
             self._t.add_(1)
 
     def _capture_state(self):
@@ -789,7 +855,7 @@ class PromptDecoder(GraphDecoder):
         # unmapped table and write nothing -- with a page shared by several rows, a warm-up write to slot 0 would
         # corrupt another row's prefix.
         return ([self.positions, self.tokens, self._t, self.generated] + ([self.hist] if self.processing else []) +
-                self._logprob_buffers())
+                ([self.cstate] if self.constrained else []) + self._logprob_buffers())
 
     def _counters_in_range(self):
         self.positions.clamp_(max=self.max_len - 1)
@@ -811,6 +877,8 @@ class PromptDecoder(GraphDecoder):
         if self.processing:
             self.hist.zero_()
             self.prompt_len.zero_()
+        if self.constrained:
+            self.cstate.copy_(self.cstart)
         for t in self._logprob_buffers():
             t.fill_(-1 if t.dtype == torch.long else float('nan'))
 
@@ -1016,16 +1084,20 @@ class PromptDecoder(GraphDecoder):
 
     def _first_token(self, logits):
         """Select the first generated token from the prefill's logits (B, vocab), at t = 0 (processed with the prompt
-        as the history)."""
+        as the history, masked at each row's start state)."""
         self._t.zero_()
         raw = self._raw(logits)
         if self.processing:
             self._process(logits, self.positions - 1)
+        if self.constrained:
+            self.cstate.copy_(self.cstart)
+        self._constrain(logits)
         self._select(logits)
         self._logprobs(raw, self.tokens, self._t)
         self.generated[:, 0].copy_(self.tokens)
         if self.processing:
             self._hist_append(self._rows, self.tokens)
+        self._constrain_advance(self.tokens[:, None])
         self._t.fill_(1)
         self._t_host = 1
 
@@ -1080,7 +1152,7 @@ class SpecDecoder(PromptDecoder):
     prompt + max_new + draft_tokens (a finished row's step still writes its T slots)."""
 
     def __init__(self, model, max_len=256, batch=1, max_new=1, draft_tokens=4, max_ngram=3, ops=None, kv_dtype=None,
-                 sampling=False, page_table=None, n_pages=None, processing=False, logprobs=None):
+                 sampling=False, page_table=None, n_pages=None, processing=False, logprobs=None, constraint=False):
         k, n_max = int(draft_tokens), int(max_ngram)
         if not 1 <= k <= 7:
             raise ValueError(f'draft_tokens must lie in [1, 7], got {draft_tokens}')
@@ -1092,7 +1164,7 @@ class SpecDecoder(PromptDecoder):
             raise ValueError(f'max_len {max_len} leaves no room for a step of {k + 1} tokens')
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
                          sampling=sampling, page_table=page_table, n_pages=n_pages, processing=processing,
-                         logprobs=logprobs)
+                         logprobs=logprobs, constraint=constraint)
         B, dev = self.batch, self.dev
         self.k, self.n_min, self.n_max = k, 1, n_max
         self.T = k + 1
@@ -1121,6 +1193,7 @@ class SpecDecoder(PromptDecoder):
         raw = self._raw(logits)
         if self.processing:                  # row i's history: hist[b, :positions[b] + 1], then drafts 1 .. i
             self._process(logits, self.positions, tokens=self.tokens)
+        self._constrain(logits, tokens=self.tokens)                  # row i's state: walked over drafts 1 .. i
         if not self.sampling:
             self.targets.copy_(logits.argmax(-1))
         elif self._kernel:
@@ -1129,6 +1202,7 @@ class SpecDecoder(PromptDecoder):
         else:
             self.targets.copy_(_sample_torch_at(logits, self.temperature, self.top_k, self.top_p, self.seed, self.n_gen))
         self._logprobs(raw, self.targets, self.n_gen)              # accepted targets: columns n_gen .. n_gen + e - 1
+        n0 = self.n_gen.clone() if self.constrained else None
         if self._kernel:
             from . import fused
             fused.spec_accept(self.tokens, self.targets, self.generated, self.hist, self.positions, self.n_gen,
@@ -1136,6 +1210,8 @@ class SpecDecoder(PromptDecoder):
         else:
             _spec_accept_torch(self.tokens, self.targets, self.generated, self.hist, self.positions, self.n_gen,
                                self.accepted, self.max_new)
+        if self.constrained:                                       # the targets the accept appended
+            self._constrain_advance(self.targets, counts=self.n_gen - n0)
 
     def _capture_state(self):
         return super()._capture_state() + [self.targets, self.hist, self.n_gen, self.accepted]
@@ -1168,7 +1244,11 @@ class SpecDecoder(PromptDecoder):
         raw = self._raw(logits)
         if self.processing:
             self._process(logits, self.positions - 1)
+        if self.constrained:
+            self.cstate.copy_(self.cstart)
+        self._constrain(logits)
         self._select(logits, out=self._first)
+        self._constrain_advance(self._first[:, None])
         self._logprobs(raw, self._first, self._t)
         self.generated[:, 0].copy_(self._first)
         self.hist[self._rows, self.positions] = self._first
@@ -1225,10 +1305,11 @@ class ContinuousDecoder(PromptDecoder):
     through the table, SDPA under each sequence's causal mask)."""
 
     def __init__(self, model, max_len, batch, n_pages, max_new, ops=None, kv_dtype=None, sampling=False, eos=(),
-                 processing=False, logprobs=None):
+                 processing=False, logprobs=None, constraint=False):
         max_pages = -(-int(max_len) // KV_PAGE)
         super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, ops=ops, kv_dtype=kv_dtype,
                          sampling=sampling, n_pages=n_pages, processing=processing, logprobs=logprobs,
+                         constraint=constraint,
                          page_table=torch.full((int(batch), max_pages), -1, dtype=torch.int32))
         B, dev = self.batch, self.dev
         self.n_gen = torch.zeros(B, dtype=torch.long, device=dev)
@@ -1240,10 +1321,11 @@ class ContinuousDecoder(PromptDecoder):
 
     # ---- per-row requests
 
-    def admit(self, row, pages, budget, settings=None, prompt=None, proc=None):
+    def admit(self, row, pages, budget, settings=None, prompt=None, proc=None, cstart=-1):
         """Give row `row` a new request: its pages (host ids, mapped from slot 0 on), its budget of new tokens, when
-        sampling its (temperature, top_k, top_p, seed) and, with processing, its prompt (the start of its history) and
-        (repetition_penalty, no_repeat_ngram_size, min_new_tokens).  Its prompt is then fed by mixed steps."""
+        sampling its (temperature, top_k, top_p, seed), with processing its prompt (the start of its history) and
+        (repetition_penalty, no_repeat_ngram_size, min_new_tokens), and with constraint=True its start state in the
+        table of set_constraint (-1: unconstrained).  Its prompt is then fed by mixed steps."""
         tbl = torch.full((self.max_pages,), -1, dtype=torch.int32)
         tbl[:len(pages)] = torch.tensor(pages, dtype=torch.int32)
         self.page_table[row].copy_(tbl)
@@ -1263,6 +1345,8 @@ class ContinuousDecoder(PromptDecoder):
             self.hist[row, :prompt.numel()] = prompt.to(self.dev)
             self.prompt_len[row] = prompt.numel()
             self.penalty[row], self.ngram[row], self.min_new[row] = float(proc[0]), int(proc[1]), int(proc[2])
+        if self.constrained:
+            self.cstate[row] = int(cstart)
 
     def retire(self, row):
         """Unmap row `row`'s pages and make it idle."""
@@ -1293,6 +1377,7 @@ class ContinuousDecoder(PromptDecoder):
         self.positions[rows] = self.positions[rows] + live.long()
         if self.processing:
             self._hist_append(rows, tok, live)
+        self._constrain_advance(tok[:, None], counts=live.long(), rows=rows)
         stop = (tok[:, None] == self.eos[None]).any(1) | (n >= self.budget[rows])
         self.done[rows] = self.done[rows] | (live & stop)
 
@@ -1300,6 +1385,7 @@ class ContinuousDecoder(PromptDecoder):
         raw = self._raw(self.logits)
         if self.processing:
             self._process(self.logits, self.positions)
+        self._constrain(self.logits)
         tok = self._choose(self.logits, self._rows)
         self._logprobs(raw, tok, self.n_gen)                   # a done row's column n_gen lies past its own tokens
         self._commit(self._rows, tok)
@@ -1362,6 +1448,7 @@ class ContinuousDecoder(PromptDecoder):
             raw = self._raw(logits)
             if self.processing:
                 self._process(logits, self.positions, rows=out_t)
+            self._constrain(logits, rows=out_t)
             tok = self._choose(logits, out_t)
             self._logprobs(raw, tok, self.n_gen, rows=out_t)
             self._commit(out_t, tok)
@@ -1759,18 +1846,21 @@ class ContinuousSchedule:
 
 
 def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len,
-                         proc=None, logprobs=None, top_logprobs=0):
+                         proc=None, logprobs=None, top_logprobs=0, constraint=None):
     """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages;
     proc: the per-prompt (penalties, ngram sizes, min_new_tokens) and the bad words of the logits processors, or None;
+    constraint: the packed token automata and each prompt's start state (constrain.pack_automata), or None;
     logprobs: generate()'s dict, or None.  A request's logprob entries are read with its tokens, before its row takes
     the next prompt (admission resets n_gen, and the next request writes the same columns)."""
     lens = [p.numel() for p in prompts]
     sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk)
     dec = ContinuousDecoder(model, max_len, rows, kv_pages, max(max_new), kv_dtype=kv_dtype,
                             sampling=settings is not None, eos=eos, processing=proc is not None,
-                            logprobs=None if logprobs is None else top_logprobs)
+                            logprobs=None if logprobs is None else top_logprobs, constraint=constraint is not None)
     if proc is not None:
         dec.set_processing(bad_words_ids=proc[3] or None, eos=eos)
+    if constraint is not None:
+        dec.set_constraint(*constraint[:3])
     if dec.dev.type == 'cuda':
         dec.capture()                                # before any row is mapped: the warm-up steps write nothing
     out = [None] * len(prompts)
@@ -1798,7 +1888,8 @@ def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows,
                     dec.retire(r)
             for r, i, pages in sched.admit():
                 dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings],
-                          prompts[i], None if proc is None else [s[i] for s in proc[:3]])
+                          prompts[i], None if proc is None else [s[i] for s in proc[:3]],
+                          -1 if constraint is None else constraint[3][i])
         if sched.finished:
             break
         decoding, pieces = sched.plan()
@@ -1903,6 +1994,56 @@ def _process_torch(logits, T, hist, last, prompt_len, penalty, ngram, min_new, e
         ids = torch.tensor(sorted(v for v in hard if 0 <= v < V), dtype=torch.long, device=logits.device)
         x[ids] = float('-inf')
     return logits
+
+
+def _table_walk(offsets, ids, next, s, tokens):
+    """delta of include/quip_b200.h (quip_constrain_mask) over tokens from state s, on the host lists of a table."""
+    for v in tokens:
+        if not 0 <= s < len(offsets) - 1:
+            return s
+        lo = min(max(offsets[s], 0), len(ids))
+        hi = min(max(offsets[s + 1], lo), len(ids))
+        k = bisect.bisect_left(ids, v, lo, hi)
+        s = next[k] if k < hi and ids[k] == v else s
+    return s
+
+
+def _constrain_torch(logits, T, state, offsets, ids, next, tokens=None, rows=None):
+    """The rule of quip_constrain_mask (include/quip_b200.h) in torch, in place on logits (R, V) (fp32 on the CPU,
+    fp16 on the GPU): x + (allowed ? +0 : -inf), HF's scores + mask; arguments as fused.constrain_mask."""
+    R, V = logits.shape
+    st, off, idl, nxl = state.tolist(), offsets.tolist(), ids.tolist(), next.tolist()
+    rows_l = None if rows is None else rows.tolist()
+    drafts = None if tokens is None else tokens.tolist()
+    for r in range(R):
+        b, i = (r // T if rows_l is None else rows_l[r // T]), r % T
+        if not 0 <= b < len(st):
+            continue
+        s = _table_walk(off, idl, nxl, st[b], drafts[b][1:i + 1] if i else [])
+        if not 0 <= s < len(off) - 1:
+            continue
+        lo = min(max(off[s], 0), len(idl))
+        hi = min(max(off[s + 1], lo), len(idl))
+        mask = torch.full((V,), float('-inf'), dtype=logits.dtype, device=logits.device)
+        mask[torch.tensor([v for v in idl[lo:hi] if 0 <= v < V], dtype=torch.long, device=logits.device)] = 0
+        logits[r] += mask
+    return logits
+
+
+def _constrain_advance_torch(state, tokens, offsets, ids, next, counts=None, rows=None):
+    """The rule of quip_constrain_advance (include/quip_b200.h) in torch, in place on state; arguments as
+    fused.constrain_advance."""
+    N, T = tokens.shape
+    st, off, idl, nxl, tok = state.tolist(), offsets.tolist(), ids.tolist(), next.tolist(), tokens.tolist()
+    rows_l = None if rows is None else rows.tolist()
+    cnt = None if counts is None else counts.tolist()
+    for n in range(N):
+        b = n if rows_l is None else rows_l[n]
+        if 0 <= b < len(st):
+            c = T if cnt is None else min(max(cnt[n], 0), T)
+            st[b] = _table_walk(off, idl, nxl, st[b], tok[n][:c])
+    state.copy_(torch.tensor(st, dtype=torch.int32))
+    return state
 
 
 def _processing_settings(n, V, repetition_penalty, no_repeat_ngram_size, min_new_tokens, bad_words_ids, eos):
@@ -2125,7 +2266,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
              max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
              beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
-             logprobs=None, top_logprobs=0):
+             logprobs=None, top_logprobs=0, token_constraint=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -2213,7 +2354,21 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     top_logprobs=n (1 .. 20) logprobs['top_ids'][i] (int64) and logprobs['top'][i] (fp32) are (len_i, n): the n most
     likely ids at each position, by logit descending and then lower id, and their logprobs.  They are the same for
     greedy, sampled and speculative runs and combine with every path but num_beams > 1 (beam_stats has the beams'
-    scores).  With logprobs=None nothing is allocated or launched; the returned tokens never change."""
+    scores).  With logprobs=None nothing is allocated or launched; the returned tokens never change.
+
+    token_constraint: a constrain.TokenAutomaton for every output row, or a list with one TokenAutomaton or None per
+    prompt (per output row with num_return_sequences, as the sampling settings); None rows are unconstrained.  Each
+    row starts at its automaton's start state at its first generated token (the prompt is not walked); inside the
+    captured step, after the logits processors and before temperature, top-k and top-p, quip_constrain_mask adds -inf
+    to every token its state does not allow (HF's PrefixConstrainedLogitsProcessor: scores + mask), and
+    quip_constrain_advance moves the state over the tokens the step commits (the rule is in include/quip_b200.h).  For
+    each prompt p the greedy result is what HF's model.generate(p[None], prefix_allowed_tokens_fn=
+    a.hf_prefix_allowed_tokens_fn(len(p)), ...the same settings...) returns with the prompt alone, in any batch, up to
+    ties and the fp16 rounding the processors document; a sampled row is what quip_sample picks from the masked row.
+    It combines with sampling, the logits processors, prompt_lookup_num_tokens (the tokens stay those of plain
+    constrained generation; drafts are not pruned), max_batch_size, share_prompt_prefixes, num_return_sequences,
+    prefill_chunk_size, kv_dtype and logprobs (which stay raw).  num_beams > 1, a token id outside the vocabulary, or a
+    list of the wrong length raises ValueError before any work.  With None, nothing of this is allocated or launched."""
     if logprobs is not None and not isinstance(logprobs, dict):
         raise ValueError(f'logprobs must be None or a dict that receives the results, got {type(logprobs).__name__}')
     if isinstance(top_logprobs, bool) or not isinstance(top_logprobs, int) or not 0 <= top_logprobs <= TOPK_MAX_N:
@@ -2306,6 +2461,14 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError('min_new_tokens bans the EOS ids: it needs eos_token_id')
         if len(eos) > PROC_MAX_EOS:
             raise ValueError(f'the logits processors take at most {PROC_MAX_EOS} eos ids, got {len(eos)}')
+    constraint = None
+    if token_constraint is not None:
+        automata = _per_prompt('token_constraint', token_constraint, len(prompts))
+        constraint = pack_automata(automata, model.lm_head.out_features)
+        if all(s < 0 for s in constraint[3]):
+            constraint = None
+        elif nb > 1:
+            raise ValueError('token_constraint does not combine with num_beams > 1 (beam search)')
     if nb > 1:
         return _beam_generate(model, prompts, budgets, nb, eos, kv_dtype, prefill_chunk_size, max_len,
                               float(length_penalty), early_stopping, n_ret, beam_stats)
@@ -2317,7 +2480,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError(f'kv_pages must be an integer >= 1, got {kv_pages!r}')
         return _generate_continuous(model, prompts, budgets, eos, kv_dtype, settings if do_sample else None, rows,
                                     int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len,
-                                    proc, logprobs, int(top_logprobs))
+                                    proc, logprobs, int(top_logprobs), constraint)
     pages, starts = {}, None
     if share:
         table, n_pages, starts = plan_prefix_pages(prompts, [n + m + k for n, m in zip(lens, budgets)],
@@ -2327,6 +2490,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         pages['processing'] = True
     if n_lp is not None:
         pages['logprobs'] = n_lp
+    if constraint is not None:
+        pages['constraint'] = True
     if spec:
         dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
                           max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
@@ -2337,6 +2502,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         dec.set_sampling(*settings)
     if proc is not None:
         dec.set_processing(*proc[:3], proc[3] or None, eos)
+    if constraint is not None:
+        dec.set_constraint(*constraint)
     if dec.dev.type == 'cuda' and max_new_tokens > 1:                # one token comes from the prefill alone
         dec.capture()                                                # before prefill maps a paged table
     dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)

@@ -843,3 +843,85 @@ def logits_process(logits, T, hist, last, prompt_len, penalty, ngram, min_new, e
                                                    n_eos, p(bad), p(bad_len), n_bad, B, max_len,
                                                    torch.cuda.current_stream(logits.device).cuda_stream))
     return logits
+
+
+CONSTRAIN_MAX_V, CONSTRAIN_MAX_T = 2 ** 18, 8
+
+
+def _constraint_table(fn, offsets, ids, next):
+    """(S, nnz) of a packed token-automaton table after checking its shapes and dtypes (its contents are checked where
+    it is packed: constrain.pack_automata)."""
+    if offsets.dtype != torch.int32 or offsets.dim() != 1 or offsets.numel() < 1:
+        raise ValueError(f'{fn}: offsets must be (S + 1,) int32, got {tuple(offsets.shape)} {offsets.dtype}')
+    nnz = ids.numel()
+    for name, t in (('ids', ids), ('next', next)):
+        if t.dtype != torch.int32 or tuple(t.shape) != (nnz,):
+            raise ValueError(f'{fn}: {name} must be (nnz = {nnz},) int32, got {tuple(t.shape)} {t.dtype}')
+    return offsets.numel() - 1, nnz
+
+
+def constrain_mask(logits, T, state, offsets, ids, next, tokens=None, rows=None):
+    """quip_constrain_mask: the token-automaton mask rule of include/quip_b200.h, in place on logits (R, V) fp16
+    (stride(1) == 1, any stride(0) >= V).  Row r is offset r % T of decoder row rows[r // T] (rows (R // T,) int64;
+    default r // T), whose state state[b] (state (B,) int32, -1: unconstrained) is walked over the drafts
+    tokens[b, 1 .. r % T] (tokens (B, T) int64, needed when T > 1) through the table offsets (S + 1,), ids and next
+    (nnz,) int32.  CUDA, one device; everything is checked before the launch, which runs on the current stream.
+    Returns logits."""
+    if logits.dim() != 2 or logits.dtype != torch.float16:
+        raise ValueError(f'constrain_mask: logits must be (R, V) fp16, got {tuple(logits.shape)} {logits.dtype}')
+    R, V = logits.shape
+    if not 1 <= V <= CONSTRAIN_MAX_V or (R > 1 and logits.stride(0) < V) or (V > 1 and logits.stride(1) != 1):
+        raise ValueError(f'constrain_mask: logits rows must be unit-stride, not overlap and hold 1 .. '
+                         f'{CONSTRAIN_MAX_V} values, got shape {tuple(logits.shape)} strides {tuple(logits.stride())}')
+    if isinstance(T, bool) or int(T) != T or not 1 <= T <= CONSTRAIN_MAX_T or R % T:
+        raise ValueError(f'constrain_mask: T must be an integer in [1, {CONSTRAIN_MAX_T}] dividing R = {R}, got {T!r}')
+    if state.dtype != torch.int32 or state.dim() != 1 or state.numel() < 1:
+        raise ValueError(f'constrain_mask: state must be (B,) int32, got {tuple(state.shape)} {state.dtype}')
+    B = state.numel()
+    S, nnz = _constraint_table('constrain_mask', offsets, ids, next)
+    if T > 1 and tokens is None:
+        raise ValueError('constrain_mask: T > 1 needs the drafts (tokens)')
+    if rows is None and R // T != B:
+        raise ValueError(f'constrain_mask: {R // T} logits rows of T = {T} for {B} states: pass rows')
+    if tokens is not None and (tokens.dtype != torch.int64 or tuple(tokens.shape) != (B, T)):
+        raise ValueError(f'constrain_mask: tokens must be {(B, T)} int64, got {tuple(tokens.shape)} {tokens.dtype}')
+    if rows is not None and (rows.dtype != torch.int64 or tuple(rows.shape) != (R // T,)):
+        raise ValueError(f'constrain_mask: rows must be {(R // T,)} int64, got {tuple(rows.shape)} {rows.dtype}')
+    if not logits.is_cuda:
+        raise RuntimeError('constrain_mask runs on a CUDA device only (there is no CPU fallback)')
+    _check_cuda('constrain_mask', (state, offsets, ids, next, tokens, rows), logits.device)
+    ld = logits.stride(0) if R > 1 else V
+    p = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().quip_constrain_mask(logits.data_ptr(), ld, R, int(T), V, p(rows), p(tokens),
+                                                   state.data_ptr(), B, offsets.data_ptr(), p(ids), p(next), S, nnz,
+                                                   torch.cuda.current_stream(logits.device).cuda_stream))
+    return logits
+
+
+def constrain_advance(state, tokens, offsets, ids, next, counts=None, rows=None):
+    """quip_constrain_advance: state[b] (state (B,) int32) walked over the first counts[n] (counts (N,) int64; default
+    T) of the committed tokens (N, T) int64 of entry n, b = rows[n] (rows (N,) int64, distinct; default n), through the
+    table offsets (S + 1,), ids and next (nnz,) int32 (include/quip_b200.h).  CUDA, one device; checked before the
+    launch, which runs on the current stream.  Returns state."""
+    if state.dtype != torch.int32 or state.dim() != 1 or state.numel() < 1:
+        raise ValueError(f'constrain_advance: state must be (B,) int32, got {tuple(state.shape)} {state.dtype}')
+    if tokens.dtype != torch.int64 or tokens.dim() != 2 or not 1 <= tokens.shape[1] <= CONSTRAIN_MAX_T:
+        raise ValueError(f'constrain_advance: tokens must be (N, T <= {CONSTRAIN_MAX_T}) int64, got '
+                         f'{tuple(tokens.shape)} {tokens.dtype}')
+    B, (N, T) = state.numel(), tokens.shape
+    S, nnz = _constraint_table('constrain_advance', offsets, ids, next)
+    if rows is None and N != B:
+        raise ValueError(f'constrain_advance: {N} token rows for {B} states: pass rows')
+    for name, t in (('counts', counts), ('rows', rows)):
+        if t is not None and (t.dtype != torch.int64 or tuple(t.shape) != (N,)):
+            raise ValueError(f'constrain_advance: {name} must be ({N},) int64, got {tuple(t.shape)} {t.dtype}')
+    if not state.is_cuda:
+        raise RuntimeError('constrain_advance runs on a CUDA device only (there is no CPU fallback)')
+    _check_cuda('constrain_advance', (tokens, offsets, ids, next, counts, rows), state.device)
+    p = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
+    with torch.cuda.device(state.device):
+        _lib.check(_lib.load().quip_constrain_advance(state.data_ptr(), B, tokens.data_ptr(), T, N, T, p(rows),
+                                                      p(counts), offsets.data_ptr(), p(ids), p(next), S, nnz,
+                                                      torch.cuda.current_stream(state.device).cuda_stream))
+    return state
