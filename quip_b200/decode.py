@@ -23,7 +23,8 @@ its step selects by temperature, top-k and top-p with a per-row seed (quip_sampl
 include/quip_b200.h) instead of argmax, from settings held in device buffers, so one captured graph serves any settings.
 `SpecDecoder` (generate(..., prompt_lookup_num_tokens=k)) verifies k prompt-lookup drafts per row in each captured step:
 T = k + 1 tokens per row through the same layer loops, attention by csrc/attn_decode.cu's extend kernel, drafting and
-acceptance by csrc/spec.cu.  `ContinuousDecoder` (generate(..., max_batch_size=n)) serves requests continuously: each
+acceptance by csrc/spec.cu; `AssistedDecoder` (generate(..., assistant_model=small)) drafts them with a smaller model's
+own steps inside the same graph.  `ContinuousDecoder` (generate(..., max_batch_size=n)) serves requests continuously: each
 holds a decode row and its own pages only while it runs, and queued prompts join through ragged mixed steps
 (csrc/attn_prefill.cu's ragged kernels), scheduled by `ContinuousSchedule`.
 """
@@ -320,9 +321,10 @@ class GraphDecoder:
     def capture(self):
         """Record one step.  The cache and position are restored afterwards, so capture is side-effect free."""
         from .quant import QuantLinear
-        for mod in self.model.modules():                   # sibling groups launch on side streams: not while capturing
-            if isinstance(mod, QuantLinear) and getattr(mod, '_group', None) is not None:
-                raise RuntimeError('dissolve the sibling groups (quant.SiblingGroup.dissolve) before capturing')
+        for model in self._models():                       # sibling groups launch on side streams: not while capturing
+            for mod in model.modules():
+                if isinstance(mod, QuantLinear) and getattr(mod, '_group', None) is not None:
+                    raise RuntimeError('dissolve the sibling groups (quant.SiblingGroup.dissolve) before capturing')
         state = self._capture_state()
         saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=self.dev)
@@ -336,6 +338,10 @@ class GraphDecoder:
         for t, t0 in zip(state, saved):
             t.copy_(t0)
         return self
+
+    def _models(self):
+        """The models whose layers a step runs."""
+        return [self.model]
 
     def _capture_state(self):
         """The buffers a step changes, which capture() puts back after its warm-up steps."""
@@ -783,8 +789,9 @@ class PromptDecoder(GraphDecoder):
     def _attend_multi(self, li, q, k, v, mask, scale):
         """_attend for T > 1 tokens per row (q (B, nh, T, hd), k / v (B, nkv, T, hd)): token i appended at slot
         positions[b] + i and attending over slots 0 .. positions[b] + i.  CUDA: quip_extend_attention(_fp8), token-major
-        operands; CPU: per-row scatter of the T slots, SDPA under the causal mask.  Returns (B, T, nh * hd)."""
-        B, T, nh, nkv, hd = self.batch, self.T, self.nh, self.nkv, self.hd
+        operands; CPU: per-row scatter of the T slots, SDPA under the causal mask.  Returns (B, T, nh * hd).  T is the
+        step's own (q's), so one decoder may run steps of several widths (AssistedDecoder's assistant)."""
+        (B, nh, T, hd), nkv = q.shape, self.nkv
         if self._kernel:
             from . import fused
             o = fused.extend_attention(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous(),
@@ -792,7 +799,7 @@ class PromptDecoder(GraphDecoder):
                                        self.positions, scale, **self._kv_kw(li))
             return o.view(B, T, nh * hd)
         rows = self._rows[:, None].expand(B, T)
-        slots = self.positions[:, None] + self._tarange                                 # (B, T)
+        slots = self.positions[:, None] + self._tar(T)                                  # (B, T)
         self._store(li, rows, slots, k.transpose(1, 2), v.transpose(1, 2))
         kk, vv = self._cached(li, q.dtype)
         if nkv != nh:
@@ -1270,6 +1277,113 @@ class SpecDecoder(PromptDecoder):
         else:
             self.graph.replay()
         return self.logits
+
+
+class AssistedDecoder(SpecDecoder):
+    """SpecDecoder whose drafts come from a smaller model of the same vocabulary (generate(..., assistant_model=...)).
+
+    The assistant is a PromptDecoder over `assistant` (`self.assistant`): its own KV cache (the same kv_dtype, and with
+    n_pages its own pool under the same page table), its own positions.  One captured step (a round) runs, for each row
+    b with c = positions[b] (the slot of its current token hist[b, c]) and g = n_gen[b]:
+      1. tokens[b, 0] = hist[b, c];
+      2. the assistant at T = 2 on hist[b, c - 1], hist[b, c] at its slots c - 1, c (causal extend attention); the
+         logits of the second token give d_1 = select(z, t = g);
+      3. for i = 1 .. k - 1, the assistant at T = 1 on d_i at slot c + i; its logits give d_(i+1) = select(z, t = g + i);
+      4. tokens[b, 1 .. k] = d_1 .. d_k;
+      5. SpecDecoder's verify and accept, unchanged.
+    select is argmax, or with sampling the rule of quip_sample with the row's own temperature, top-k, top-p and seed at
+    step t (quip_sample_at): the uniform the target draws its token g + i with.  So a draft is the target's token
+    whenever the assistant's distribution puts that uniform on the same token (coupled drafts), and the tokens are the
+    ones plain generation selects.  The logits processors and the token constraint act on the target's logits only;
+    drafts are not pruned.
+
+    The cache rule: at the start of every round the assistant's slots 0 .. c - 2 hold the keys and values of
+    hist[b, 0 .. c - 2].  Prefill leaves c at the prompt length, so it holds from the first round.  The T = 2 step
+    rewrites slot c - 1, which covers a round that accepted all k drafts (the assistant never fed the last one); slots
+    past the accepted prefix hold rejected drafts and are each rewritten before anything reads them, the rule the target
+    follows.  A finished row still runs the round and writes at most slot c + k - 1, inside max_len.  On the CPU the same
+    round in torch (_sample_torch_at, per-row scatter and SDPA)."""
+
+    def __init__(self, model, assistant, max_len=256, batch=1, max_new=1, draft_tokens=4, ops=None, kv_dtype=None,
+                 sampling=False, page_table=None, n_pages=None, processing=False, logprobs=None, constraint=False):
+        _check_assistant(model, assistant, max_len)
+        super().__init__(model, max_len=max_len, batch=batch, max_new=max_new, draft_tokens=draft_tokens, ops=ops,
+                         kv_dtype=kv_dtype, sampling=sampling, page_table=page_table, n_pages=n_pages,
+                         processing=processing, logprobs=logprobs, constraint=constraint)
+        self.assistant = PromptDecoder(assistant, max_len=self.max_len, batch=self.batch, kv_dtype=kv_dtype,
+                                       page_table=page_table, n_pages=n_pages)
+        self._draft_tok = torch.zeros(self.batch, 1, dtype=torch.long, device=self.dev)
+        self._draft_t = torch.zeros(self.batch, dtype=torch.long, device=self.dev)
+
+    def _models(self):
+        return [self.model, self.assistant.model]
+
+    def _assist(self, tokens):
+        """The assistant on tokens (B,) or (B, T) at its slots positions[b] + i: the logits (B, vocab) of the last."""
+        a = self.assistant
+        h, pend = a._layers(a._embed(tokens))
+        if h.shape[1] > 1:
+            h, pend = h[:, -1:].contiguous(), None if pend is None else pend[:, -1:].contiguous()
+        return a._head(h, pend)
+
+    def _assist_select(self, z, i):
+        """tokens[:, i + 1] = select(z, t = n_gen + i) for the assistant's logits z (B, vocab)."""
+        out = self._draft_tok
+        if not self.sampling:
+            out.copy_(z.argmax(-1, keepdim=True))
+        elif self._kernel:
+            from . import fused
+            torch.add(self.n_gen, i, out=self._draft_t)
+            fused.sample_at(z[:, None], self.temperature, self.top_k, self.top_p, self.seed, self._draft_t, out)
+        else:
+            out.copy_(_sample_torch_at(z[:, None], self.temperature, self.top_k, self.top_p, self.seed, self.n_gen + i))
+        self.tokens[:, i + 1:i + 2].copy_(out)
+
+    def _draft(self):
+        a, c = self.assistant, self.positions
+        prev = (c - 1).clamp(min=0)           # c >= 1 after prefill; 0 only in a warm-up step before it
+        pair = self.hist.gather(1, torch.stack((prev, c), 1))                           # (B, 2)
+        self.tokens[:, :1].copy_(pair[:, 1:])
+        a.positions.copy_(prev)
+        self._assist_select(self._assist(pair), 0)
+        a.positions.add_(2)
+        for i in range(1, self.k):
+            self._assist_select(self._assist(self.tokens[:, i]), i)
+            a.positions.add_(1)
+
+    def _capture_state(self):
+        # the assistant's positions are set from the target's in every round, so the target's clamp keeps its slots
+        # (c - 1 .. c + k - 1) inside the cache as well
+        a = self.assistant
+        return (super()._capture_state() + [a.positions, a.k_cache, a.v_cache] +
+                ([a.k_scale, a.v_scale] if a._fp8 else []))
+
+    def reset(self):
+        super().reset()
+        self.assistant.reset()
+
+    def prefill(self, prompts, chunk=None, starts=None):
+        """SpecDecoder.prefill, then the assistant's prefill of the same prompts (chunk and starts as given)."""
+        logits = super().prefill(prompts, chunk=chunk, starts=starts)
+        self.assistant.prefill(prompts, chunk=chunk, starts=starts)
+        return logits
+
+
+def _check_assistant(model, assistant, max_len):
+    """Raise ValueError unless `assistant` can draft for `model` with a cache of max_len slots: a Llama or OPT model on
+    the same device, with the same number of logits, and (OPT) learned positions for every slot."""
+    cfg = getattr(assistant, 'config', None)
+    if getattr(cfg, 'model_type', None) not in ('llama', 'opt'):
+        raise ValueError('assistant_model must be a Llama or OPT model')
+    dev, a_dev = next(iter(model.parameters())).device, next(iter(assistant.parameters())).device
+    if a_dev != dev:
+        raise ValueError(f'the assistant is on {a_dev}, the model on {dev}')
+    if assistant.lm_head.out_features != model.lm_head.out_features:
+        raise ValueError(f'the assistant has {assistant.lm_head.out_features} logits per token, the model '
+                         f'{model.lm_head.out_features}: they must share the vocabulary')
+    if cfg.model_type == 'opt' and int(max_len) > cfg.max_position_embeddings:
+        raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the '
+                         'assistant')
 
 
 class _Ragged:
@@ -2266,7 +2380,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
              max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
              beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
-             logprobs=None, top_logprobs=0, token_constraint=None):
+             logprobs=None, top_logprobs=0, token_constraint=None, assistant_model=None, num_assistant_tokens=None):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -2286,6 +2400,17 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     the ones plain generation selects from the same logits (greedy or sampled, with the same seeds); only the step's
     arithmetic differs (other token counts take other kernel routes).  The default max_len grows by k.  spec_stats: a
     dict that receives 'accepted' (drafts taken per row) and 'steps'.
+
+    assistant_model=small (default None: off) generates with assisted drafts (AssistedDecoder): a Llama or OPT model on
+    the same device with the same lm_head.out_features (packed or not; an OPT one needs learned positions for max_len)
+    proposes num_assistant_tokens=k drafts per row (an integer in [1, 7]; default 4) with k cheap steps of its own, and
+    the model verifies them in the same captured step, as for prompt lookup.  The assistant selects each draft by the
+    row's own rule: argmax, or with do_sample the same seed and step the model draws that token with, so the returned
+    tokens are the ones plain generation returns with the same arguments (on the GPU up to the rounding of other token
+    counts); the assistant only changes how many tokens a step yields.  Processors and token_constraint act on the
+    model's logits only, and logprobs are the model's.  The default max_len grows by k; spec_stats receives 'accepted'
+    and 'steps'.  num_assistant_tokens without assistant_model, or assistant_model with prompt_lookup_num_tokens,
+    num_beams > 1 or max_batch_size, raises ValueError before any work.
 
     prefill_chunk_size=C (an int >= 1; default None: one many-token forward of the padded prompts) prefills in chunks
     of C tokens straight into the KV cache (PromptDecoder.prefill(chunk=C)): the prefill's peak memory is bounded by C
@@ -2384,6 +2509,17 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     if isinstance(num_beams, bool) or int(num_beams) != num_beams or not 1 <= num_beams <= 16:
         raise ValueError(f'num_beams must be an integer in [1, 16], got {num_beams!r}')
     nb = int(num_beams)
+    assisted = assistant_model is not None
+    if num_assistant_tokens is not None and not assisted:
+        raise ValueError('num_assistant_tokens sets the drafts of assisted generation: it needs assistant_model')
+    if assisted:
+        for name, on in (('prompt_lookup_num_tokens', prompt_lookup_num_tokens is not None), ('num_beams > 1', nb > 1),
+                         ('max_batch_size', max_batch_size is not None)):
+            if on:
+                raise ValueError(f'{name} does not combine with assistant_model (assisted generation)')
+        k_a = 4 if num_assistant_tokens is None else num_assistant_tokens
+        if isinstance(k_a, bool) or not isinstance(k_a, int) or not 1 <= k_a <= 7:
+            raise ValueError(f'num_assistant_tokens must be an integer in [1, 7], got {num_assistant_tokens!r}')
     if nb > 1 and logprobs is not None:
         raise ValueError('logprobs does not combine with num_beams > 1 (beam_stats has the beams\' scores)')
     if nb > 1:
@@ -2432,6 +2568,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError(f'prompt_lookup_num_tokens must be an integer in [1, 7], got {prompt_lookup_num_tokens}')
         if n_max != max_matching_ngram_size or n_max < 1:
             raise ValueError(f'max_matching_ngram_size must be an integer >= 1, got {max_matching_ngram_size}')
+    if assisted:
+        k = k_a
     # a fixed batch steps every row max(budgets) times; continuous batching steps each row to its own budget
     n, m = (max(zip(lens, budgets), key=sum) if max_batch_size is not None else (max(lens), max_new_tokens))
     max_len = n + m + k if max_len is None else int(max_len)
@@ -2441,7 +2579,9 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     cfg = model.config
     if cfg.model_type == 'opt' and max_len > cfg.max_position_embeddings:
         raise ValueError(f'max_len {max_len} exceeds the {cfg.max_position_embeddings} learned positions of the model')
-    eos = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
+    if assisted:
+        _check_assistant(model, assistant_model, max_len)
+    eos =[] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
                                            [int(e) for e in eos_token_id])
     if not do_sample:
         for name, v, d in (('temperature', temperature, 1.0), ('top_k', top_k, 0), ('top_p', top_p, 1.0), ('seed', seed, 0)):
@@ -2492,7 +2632,10 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         pages['logprobs'] = n_lp
     if constraint is not None:
         pages['constraint'] = True
-    if spec:
+    if assisted:
+        dec = AssistedDecoder(model, assistant_model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens,
+                              draft_tokens=k, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
+    elif spec:
         dec = SpecDecoder(model, max_len=max_len, batch=len(prompts), max_new=max_new_tokens, draft_tokens=k,
                           max_ngram=n_max, kv_dtype=kv_dtype, sampling=bool(do_sample), **pages)
     else:
@@ -2508,7 +2651,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         dec.capture()                                                # before prefill maps a paged table
     dec.prefill(prompts, chunk=prefill_chunk_size, starts=starts)
     eos_t = torch.tensor(eos, dtype=torch.long, device=dec.dev)
-    if spec:
+    if spec or assisted:
         return _generate_spec(dec, budgets, eos_t, spec_stats, logprobs)
     n = 1
     while n < max_new_tokens:

@@ -6,7 +6,8 @@ HBM bandwidth of the H100 SXM data sheet (3.35 TB/s).  Needs a CUDA device.
     python tools/generate_bench.py --out DIR [--models llama7b,llama70b] [--layers70b 80] [--steps 16]
                                    [--sections kernel,prefill,decode,fp8]      (fp8kernel: the fp8 kernel rows only;
                                                                                 sample: the sampling rows;
-                                                                                spec: speculative generation)
+                                                                                spec: speculative generation;
+                                                                                assisted: assisted generation)
 
 Section fp8 measures the e4m3 KV cache (PromptDecoder(kv_dtype=torch.float8_e4m3fn)): the fp8 kernel alone next to the
 fp16 one (bytes: hd per cached K / V vector plus its 4-byte scale), PromptDecoder steps fp16 against fp8 at B = 32 and
@@ -64,6 +65,15 @@ csrc/topk_logprobs.cu): the kernel alone on R in {1, 8, 32, 256} rows of V = 320
 (time, and one pass over the logits per second), and the captured PromptDecoder step at B in {1, 8, 32} (256-token
 prompts, 64 new tokens, greedy) with logprobs off, n = 0 and n = 20, with the logits processors off and on, the three
 decoders alternating over three trials.
+
+Section assisted measures assisted generation (AssistedDecoder, generate(..., assistant_model=...)) at B in {1, 8},
+k in {2, 4, 7}, every row at position 512 of random caches: the assistant's captured T = 1 and T = 2 steps alone, the
+captured round, the target's captured PromptDecoder step, and the break-even yield round / plain step (the tokens a
+round must yield to win).  The 7B-shape target runs with 2-bit synthetic assistants of the 7B shape cut to 2, 4 and 8
+layers, the 70B shape (--layers70b) with the whole 32-layer 7B shape.  On the 7B shape the target is also its own
+assistant, which accepts every draft away from ties: the round's cost at full acceptance, as a captured round and as
+generate() end to end (128 tokens, k = 4, wall time with prefill and capture) against plain generate().  Acceptance on synthetic weights says nothing about real text.  The rows and their cache sizes are printed
+from shapes before any device work.
 
 Prints one line per measurement and writes DIR/generate_bench.json.  The decode steps of both decoders run at the same
 positions on one shared cache, alternating in the same process, and their logits are compared.  A decode configuration
@@ -405,6 +415,128 @@ def spec_generate(model, B, n_new, k, seg=64, reps=2):
         else:
             plain = toks
     out['same_tokens'] = all(torch.equal(a, b) for a, b in zip(plain, toks))
+    return out
+
+
+ASSIST_B, ASSIST_K, ASSIST_CTX = (1, 8), (2, 4, 7), 512
+
+
+def assisted_plan(layers70b):
+    """The rows of the assisted section from shapes alone: (target, its config, {assistant layers: config})."""
+    from quip_b200.synth import model_config
+    t7, t70 = model_config('llama7b'), model_config('llama70b', num_hidden_layers=layers70b)
+    return [('llama7b', t7, {L: model_config('llama7b', num_hidden_layers=L) for L in (2, 4, 8)}),
+            ('llama70b', t70, {32: model_config('llama7b')})]
+
+
+def _graph_ms(fn, reps):
+    """ms per replay of fn captured alone in a CUDA graph (two eager warm-up calls first)."""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.no_grad(), torch.cuda.stream(side):
+        for _ in range(2):
+            fn()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=side, capture_error_mode='thread_local'):
+            fn()
+    torch.cuda.current_stream().wait_stream(side)
+    return events_ms(g.replay, reps)
+
+
+def _timed_steps(dec, ctx, steps, assisted):
+    """ms per captured step of dec, every row starting at position ctx (assisted: a round, n_gen = 1)."""
+    B = dec.batch
+    dec.positions.fill_(ctx)
+    dec._pos_host = [ctx] * B
+    dec._t.fill_(1)
+    dec._t_host = 1
+    if assisted:
+        dec.n_gen.fill_(1)
+        dec._steps_host = 0
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    with torch.no_grad():
+        for _ in range(steps):
+            dec.step()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps
+
+
+def assisted_rows(model, assistant, B, ks, ctx, steps, reps, trials=3):
+    """The assistant's captured T = 1 and T = 2 steps alone, the captured AssistedDecoder round for each k and the
+    captured PromptDecoder step of the target, every row at position ctx of caches filled with random values; the
+    round and the plain step alternate trial by trial.  break_even_yield[k] = round / plain: the tokens a round must
+    yield to beat plain decoding."""
+    from quip_b200.decode import AssistedDecoder, PromptDecoder
+    max_new = steps * (max(ks) + 1) + 2
+    max_len = ctx + max_new + max(ks) + 1
+
+    def filled(dec):
+        for d in (dec, getattr(dec, 'assistant', None)):
+            if d is not None:
+                d.k_cache.normal_(0.0, 0.5)
+                d.v_cache.normal_(0.0, 0.5)
+        return dec
+    plain = filled(PromptDecoder(model, max_len=max_len, batch=B, max_new=max_new)).capture()
+    decs = {}
+    for k in ks:
+        d = filled(AssistedDecoder(model, assistant, max_len=max_len, batch=B, max_new=max_new, draft_tokens=k))
+        d.hist.random_(0, model.config.vocab_size)
+        decs[k] = d.capture()
+    d, a = decs[ks[0]], decs[ks[0]].assistant
+    pair, one = d.hist[:, ctx - 1:ctx + 1].clone(), d.hist[:, ctx].clone()
+    a.positions.fill_(ctx - 1)
+    t2 = _graph_ms(lambda: d._assist(pair), reps)
+    a.positions.fill_(ctx)
+    t1 = _graph_ms(lambda: d._assist(one), reps)
+    res = {'plain': []} | {k: [] for k in ks}
+    for t in range(trials + 1):
+        for key in res:
+            ms = _timed_steps(plain if key == 'plain' else decs[key], ctx, steps, key != 'plain')
+            if t:
+                res[key].append(ms)
+    med = {key: sorted(v)[len(v) // 2] for key, v in res.items()}
+    del plain, decs, d, a
+    torch.cuda.empty_cache()
+    return dict(B=B, context=ctx, assistant_layers=assistant.config.num_hidden_layers, assistant_t1_ms=t1,
+                assistant_t2_ms=t2, plain_step_ms=med['plain'], round_ms={str(k): med[k] for k in ks},
+                break_even_yield={str(k): med[k] / med['plain'] for k in ks},
+                trials_ms={str(k): v for k, v in res.items()})
+
+
+def assisted_generate_self(model, B, n_new, k, P=128, reps=2):
+    """generate() wall time (prefill, capture and the host loop included), plain and with the target as its own
+    assistant: away from ties every draft is accepted, so this is the round's cost at full acceptance."""
+    import time
+
+    from quip_b200.decode import generate
+    g = torch.Generator().manual_seed(4)
+    prompts = [torch.randint(0, model.config.vocab_size, (P,), generator=g) for _ in range(B)]
+    out = dict(B=B, prompt=P, new_tokens=n_new, k=k)
+    toks = {}
+    for name, kw in (('plain', {}), ('assisted', dict(assistant_model=model, num_assistant_tokens=k))):
+        times = []
+        for _ in range(reps + 1):
+            stats = {}
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            toks[name] = generate(model, prompts, n_new, spec_stats=stats, **kw) if kw else generate(model, prompts, n_new)
+            torch.cuda.synchronize()
+            times.append(time.perf_counter() - t0)
+        s = sorted(times[1:])[len(times[1:]) // 2]
+        out[f'{name}_s'] = s
+        out[f'{name}_tok_s'] = sum(int(t.numel()) for t in toks[name]) / s
+        if kw:
+            out['accepted'] = stats['accepted']
+            out['replays'] = stats['steps']
+            # a row's n_new - 1 tokens after the prefill's took n_new - 1 - accepted rounds (the replays past the
+            # last row's last round, until the every-16-steps check, yield nothing)
+            out['tokens_per_round'] = [(n_new - 1) / (n_new - 1 - acc) for acc in stats['accepted']]
+    out['same_tokens'] = all(torch.equal(a, b) for a, b in zip(toks['plain'], toks['assisted']))
+    out['agreeing_prefix'] = [int((a != b).nonzero()[0]) if not torch.equal(a, b) else a.numel()
+                              for a, b in zip(toks['plain'], toks['assisted'])]
     return out
 
 
@@ -1100,10 +1232,25 @@ def main():
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
     #                                                                         score, continuous, beam, logits,
-    #                                                                         logprobs
+    #                                                                         logprobs, assisted
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
     sections = set(a.sections.split(','))
+    if 'assisted' in sections:                         # the rows from shapes alone, before any device work
+        from quip_b200.synth import MODELS
+        unknown = set(a.models.split(',')) - set(MODELS)
+        if unknown:
+            raise SystemExit(f'unknown models {sorted(unknown)}')
+        for name, tcfg, acfgs in assisted_plan(a.layers70b):
+            if name not in a.models.split(','):
+                continue
+            for L, acfg in acfgs.items():
+                for B in ASSIST_B:
+                    max_len = ASSIST_CTX + a.steps * (max(ASSIST_K) + 1) + 2 + max(ASSIST_K) + 1
+                    print(f'assisted plan {name} ({tcfg.num_hidden_layers} layers) + {L}-layer 7B-shape assistant '
+                          f'B={B} k={ASSIST_K} ctx={ASSIST_CTX} max_len={max_len}: target cache '
+                          f'{cache_bytes(tcfg, tcfg.num_hidden_layers, B, max_len) / 2**30:.2f} GiB, assistant cache '
+                          f'{cache_bytes(acfg, L, B, max_len) / 2**30:.2f} GiB per decoder', flush=True)
     if not torch.cuda.is_available():
         raise SystemExit('generate_bench needs a CUDA device')
     from quip_b200.synth import build_synthetic_model, model_config
@@ -1205,7 +1352,7 @@ def main():
                     rec['logprobs_kernel'].append(r)
                     print(f'logprobs kernel R={R} V=32000 n={n}: {1e3 * r["kernel_ms"]:.1f} us '
                           f'({r["bytes_per_s"] / 1e12:.2f} TB/s of logits)', flush=True)
-        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec'} and not (
+        if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec', 'assisted'} and not (
                 sections & {'chunked', 'paged', 'score', 'continuous', 'beam', 'logits', 'logprobs'} and
                 name == 'llama7b'):
             continue
@@ -1352,6 +1499,34 @@ def main():
                 rec['spec_generate'].append(r)
                 print(f'{name} generate B={B} 128 tokens: plain {r["plain_tok_s"]:.0f} tok/s, k=4 {r["spec_tok_s"]:.0f} '
                       f'tok/s, {r["tokens_per_step"]:.2f} tokens per step, same tokens {r["same_tokens"]}', flush=True)
+        if 'assisted' in sections:
+            rec['assisted'] = []
+            plan = {n: acfgs for n, _, acfgs in assisted_plan(a.layers70b)}
+            for L, acfg in plan[name].items():
+                assistant = build_synthetic_model(acfg, torch.device('cuda:0'), bits=2, seed=1, seqlen=4096)
+                for B in ASSIST_B:
+                    r = assisted_rows(model, assistant, B, ASSIST_K, ASSIST_CTX, a.steps, a.kernel_reps)
+                    rec['assisted'].append(r)
+                    print(f'{name} assisted B={B} ctx={ASSIST_CTX} assistant {L} layers: T=1 {r["assistant_t1_ms"]:.3f} '
+                          f'ms, T=2 {r["assistant_t2_ms"]:.3f} ms, plain step {r["plain_step_ms"]:.3f} ms, rounds ' +
+                          ', '.join(f'k={k} {ms:.3f} ms (break-even {r["break_even_yield"][k]:.2f} tokens)'
+                                    for k, ms in r['round_ms'].items()), flush=True)
+                del assistant
+                torch.cuda.empty_cache()
+            if name == 'llama7b':
+                rec['assisted_self'], rec['assisted_self_generate'] = [], []
+                for B in ASSIST_B:
+                    r = assisted_rows(model, model, B, ASSIST_K, ASSIST_CTX, a.steps, a.kernel_reps)
+                    rec['assisted_self'].append(r)
+                    print(f'{name} assisted B={B} ctx={ASSIST_CTX} assistant = target: T=1 {r["assistant_t1_ms"]:.3f} '
+                          f'ms, T=2 {r["assistant_t2_ms"]:.3f} ms, plain step {r["plain_step_ms"]:.3f} ms, rounds ' +
+                          ', '.join(f'k={k} {ms:.3f} ms (break-even {r["break_even_yield"][k]:.2f} tokens)'
+                                    for k, ms in r['round_ms'].items()), flush=True)
+                    r = assisted_generate_self(model, B, 128, 4)
+                    rec['assisted_self_generate'].append(r)
+                    print(f'{name} generate B={B} 128 tokens, assistant = target, k=4: plain {r["plain_tok_s"]:.0f} '
+                          f'tok/s, assisted {r["assisted_tok_s"]:.0f} tok/s, tokens per round {r["tokens_per_round"]}, '
+                          f'same tokens {r["same_tokens"]}, agreeing prefix {r["agreeing_prefix"]}', flush=True)
         # fp16 against fp8 at B = 32, then the configurations only an e4m3 cache fits (7B 48 x 4096, 70B 64 x 4096)
         runs = [(32, 2048, ('fp16', 'fp8')), (32, 4096, ('fp16', 'fp8'))] if 'fp8' in sections else []
         if 'fp8' in sections:
