@@ -143,6 +143,10 @@ def load():
         rows = os.environ.get('QUIP_TC_ROWS')
         if rows:
             check(lib.quip_config(b'tc_rows', int(rows)))
+        # tokens per tile of the wgmma dense pass (blocks wider than 64): 128 or 256 forces one kernel, 0 picks by shape
+        tile = os.environ.get('QUIP_DENSE_TILE')
+        if tile:
+            check(lib.quip_config(b'dense_tile', int(tile)))
     return _lib
 
 

@@ -36,6 +36,7 @@ int qgemm_tc(const QuipLinearDesc* d, const __half* x, const float* xsum, const 
 extern int g_gather_rows, g_pass_min_tiles, g_fewtok;   // rot.cu
 extern int g_fewtok_max_m;                               // rot_fewtok.cu: token count up to which the few-token kernels run (32)
 extern int g_tc_rows;                                    // qgemm_tc.cu: weight rows per 2-bit GEMM tile above 64 tokens (0: by shape)
+extern int g_dense_tile;                                 // qgemm_tc.cu: tokens per dense-pass tile (0: by shape)
 bool side_fused_ok(const QuipSide* sd, int n);               // rot_side.cu
 int side_fused(const QuipSide* sd, const __half* in, __half* out, int64_t M, const int32_t* in_idx, const float* in_scale,
                const int32_t* out_idx, const __half* out_bias, float* xsum, cudaStream_t s);
@@ -204,6 +205,11 @@ extern "C" int quip_config(const char* key, int value) {
   if (!strcmp(key, "tc_rows")) {
     QUIP_CHECK_ARG(value == 0 || value == 128 || value == 256, "quip_config: tc_rows must be 0, 128 or 256");
     g_tc_rows = value;
+    return QUIP_OK;
+  }
+  if (!strcmp(key, "dense_tile")) {
+    QUIP_CHECK_ARG(value == 0 || value == 128 || value == 256, "quip_config: dense_tile must be 0, 128 or 256");
+    g_dense_tile = value;
     return QUIP_OK;
   }
   if (!strcmp(key, "gemv")) { g_use_gemv = value; return QUIP_OK; }

@@ -31,11 +31,11 @@ constexpr int TC_SMEM_MAX = 227 * 1024;                      // opt-in dynamic s
 
 template <int BITS, int BN, bool DENSE, int RB = 1>
 struct TcCfg {
-  static constexpr int BM = TC_BM * RB;                        // packed GEMM: weight rows per tile
+  static constexpr int BM = TC_BM * RB;                        // weight rows (packed GEMM) or tokens (dense) per tile
   // A region of a stage: the fp16 A tile (dense), or the packed words of the tile's BM / 16 row blocks for one k
   // super-block (packed; written on even stages only, the odd stage of the same super-block reads its words from
   // registers (RB = 1) or from the even stage's slot (RB = 2))
-  static constexpr int A_BYTES = DENSE ? TC_BM * TC_BK * 2 : (BM / SB_ROWS) * sb_words(BITS) * 4;   // 16 / 4, 6, 8 KB (x RB)
+  static constexpr int A_BYTES = DENSE ? BM * TC_BK * 2 : (BM / SB_ROWS) * sb_words(BITS) * 4;   // 16 / 4, 6, 8 KB (x RB)
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;        // multiple of 1024: B stays aligned for its swizzle
   // epilogue transpose buffer of one consumer warpgroup: BN token rows x 64 n (packed) or 64 token rows x BN
@@ -46,18 +46,21 @@ struct TcCfg {
   static constexpr int STAGES = STAGES_FIT < 16 ? STAGES_FIT : 16;       // 2 x 16 barriers fill the 256-byte area
   static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + EPI_BYTES;
   static_assert(STAGE_BYTES % 1024 == 0 && 2 * STAGES * 8 <= 256, "stage layout");
-  static_assert(RB == 1 || (!DENSE && BN == 128), "256-row tiles: packed GEMM at BN = 128 only");
+  static_assert(RB == 1 || DENSE || BN == 128, "256-row packed tiles: BN = 128 only");
+  static_assert(RB == 1 || STAGES >= 3, "256-row tiles: at least 3 stages in flight");
 };
 
 // DENSE = false: A is the packed matrix (N rows, K columns); its words are staged by TMA and expanded in registers.
 // DENSE = true : block-diagonal pass with big blocks -- `nblk` independent GEMMs out_b = in_b . F_b^T, A = the
-//                block's p contiguous activation columns (128 tokens per tile), B = fp16 factor F_b (N = K = p)
-//                fetched by TMA (3-D map, rows/cols beyond p zero-filled), output written to the same columns.
+//                block's p contiguous activation columns (128 * RB tokens per tile), B = BN rows of the fp16 factor F_b
+//                (N = K = p) fetched by TMA (3-D map, rows/cols beyond p zero-filled), output written to the same
+//                columns.  RB = 2: each consumer warpgroup owns 128 tokens in two 64-token halves, so a factor tile
+//                fetched from L2 feeds twice the tokens; BN is then sized to the block (dense_cols), not fixed at 128.
 // tmap_a: packed words (DENSE = false; 2-D, one row of KSB * sb_words words per 16-row block) or the factors.
 // RB: 64-row blocks per consumer warpgroup (packed GEMM).  RB = 2 makes 256-row tiles: warpgroup w owns rows
 // 128w..128w+127 in two halves of 64 (one accumulator set each), and every activation tile fetched from L2 feeds
 // twice the weight rows.  Each output element sees the same wgmma k16 steps in the same order and the same epilogue
-// arithmetic as at RB = 1, so the two produce identical bits.
+// arithmetic as at RB = 1, so the two produce identical bits (dense pass: at any BN, too).
 template <int BITS, int BN, bool DENSE, int RB = 1>
 __global__ void __launch_bounds__(RB == 1 ? TC_THREADS : TC_THREADS_TALL, 1)
 qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_a,
@@ -74,10 +77,10 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   __half* epi = reinterpret_cast<__half*>(smem_gen + (size_t)C::STAGES * C::STAGE_BYTES + 256);   // 2 x EPI_HALVES
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // packed GEMM: 128 * RB output rows (wgmma M) x BN tokens (wgmma N).  DENSE pass: 128 TOKENS (wgmma M) x BN factor
-  // rows (wgmma N).
+  // packed GEMM: 128 * RB output rows (wgmma M) x BN tokens (wgmma N).  DENSE pass: 128 * RB TOKENS (wgmma M) x BN
+  // factor rows (wgmma N).
   const int tiles_n = DENSE ? (N + BN - 1) / BN : (N + C::BM - 1) / C::BM;
-  const int tiles_m = DENSE ? (M + TC_BM - 1) / TC_BM : (M + BN - 1) / BN;
+  const int tiles_m = DENSE ? (M + C::BM - 1) / C::BM : (M + BN - 1) / BN;
   const int per_blk = tiles_n * tiles_m;
   const int num_tiles = per_blk * nblk;
   const int KB = (K + TC_BK - 1) / TC_BK;
@@ -104,13 +107,13 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int blk = tile / per_blk, rr = tile % per_blk;
-        const int m0 = (rr / tiles_n) * (DENSE ? TC_BM : BN), n0 = (rr % tiles_n) * (DENSE ? BN : C::BM);
+        const int m0 = (rr / tiles_n) * (DENSE ? C::BM : BN), n0 = (rr % tiles_n) * (DENSE ? BN : C::BM);
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&empty[s], ph ^ 1u);
           unsigned char* stage = smem_gen + (size_t)s * C::STAGE_BYTES;
           if (DENSE) {
             mbar_arrive_expect_tx(&full[s], C::STAGE_BYTES);
-            tma_load_2d(stage, &tmap_x, &full[s], blk * K + kb * TC_BK, m0);                     // A: 128 tokens
+            tma_load_2d(stage, &tmap_x, &full[s], blk * K + kb * TC_BK, m0);                     // A: 128 * RB tokens
             tma_load_3d(stage + C::A_BYTES, &tmap_a, &full[s], kb * TC_BK, n0, shared_factor ? 0 : blk);   // B: BN factor rows
           } else {
             // row blocks beyond N are zero-filled; their output rows are never stored
@@ -124,7 +127,7 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       }
     }
   } else {
-    // ================= consumers: wgmma over the ring, then the epilogue of 64 * RB rows =================
+    // ================= consumers: wgmma over the ring, then the epilogue of 64 * RB rows (dense: tokens) =========
     if constexpr (RB == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TC_TALL_CONSUMER_REGS));
     const int wg = warp >> 2, wtid = threadIdx.x & 127;
     const int frow = (warp & 3) * 16 + (lane >> 2);        // accumulator row of d[j] for (j & 2) == 0; +8 otherwise
@@ -168,12 +171,15 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&full[s], ph);
           const uint32_t a_addr = smem_base + (uint32_t)(s * C::STAGE_BYTES);
-          const uint64_t adesc = make_sw128_desc(a_addr + (uint32_t)(wg * 64 * 128));
           const uint64_t bdesc = make_sw128_desc(a_addr + C::A_BYTES);
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)     // +32 bytes along K inside the swizzle atom = +2 encoded
-            wgmma_f16_ss<BN>(acc[0], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          for (int hf = 0; hf < RB; ++hf) {        // token rows 64 (RB wg + hf).. of the tile
+            const uint64_t adesc = make_sw128_desc(a_addr + (uint32_t)((wg * RB + hf) * 64 * 128));
+#pragma unroll
+            for (int k = 0; k < TC_BK / 16; ++k)   // +32 bytes along K inside the swizzle atom = +2 encoded
+              wgmma_f16_ss<BN>(acc[hf], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          }
           wgmma_commit();
           wgmma_wait<1>();                         // the previous stage's wgmma have read their operands
           if (kb > 0) release(prev);
@@ -298,21 +304,26 @@ qgemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       release(prev);
 
       if constexpr (DENSE) {
-        // eb[token row r][column c], pitch BN + 8
+        // eb[token row r][column c], pitch BN + 8; one 64-token half at a time
         constexpr int EP = BN + 8;
+        const int i0 = (rr % tiles_n) * BN;
 #pragma unroll
-        for (int j = 0; j < BN / 2; j += 2) {
-          const int r = frow + ((j & 2) ? 8 : 0), c = 8 * (j >> 2) + fcol;
-          *reinterpret_cast<__half2*>(&eb[r * EP + c]) = __floats2half2_rn(acc[0][j], acc[0][j + 1]);
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-        const int m_base = (rr / tiles_n) * TC_BM + wg * 64, i0 = (rr % tiles_n) * BN;
-        for (int idx = wtid; idx < 64 * (BN / 8); idx += 128) {
-          const int r = idx / (BN / 8), v = idx % (BN / 8);
-          const int m = m_base + r, i = i0 + 8 * v;
-          if (m < M && i < N)
-            *reinterpret_cast<uint4*>(z + (int64_t)m * ldz + (int64_t)blk * N + i) =
-                *reinterpret_cast<const uint4*>(&eb[r * EP + 8 * v]);
+        for (int hf = 0; hf < RB; ++hf) {
+#pragma unroll
+          for (int j = 0; j < BN / 2; j += 2) {
+            const int r = frow + ((j & 2) ? 8 : 0), c = 8 * (j >> 2) + fcol;
+            *reinterpret_cast<__half2*>(&eb[r * EP + c]) = __floats2half2_rn(acc[hf][j], acc[hf][j + 1]);
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+          const int m_base = (rr / tiles_n) * C::BM + (wg * RB + hf) * 64;
+          for (int idx = wtid; idx < 64 * (BN / 8); idx += 128) {
+            const int r = idx / (BN / 8), v = idx % (BN / 8);
+            const int m = m_base + r, i = i0 + 8 * v;
+            if (m < M && i < N)
+              *reinterpret_cast<uint4*>(z + (int64_t)m * ldz + (int64_t)blk * N + i) =
+                  *reinterpret_cast<const uint4*>(&eb[r * EP + 8 * v]);
+          }
+          if (hf + 1 < RB) asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // eb is free for the next half
         }
       } else {
         // eb[token c][row r], pitch 72; one 64-row half at a time
@@ -434,12 +445,12 @@ static int launch_tc(const QuipLinearDesc* d, const __half* x, const float* xsum
 }
 
 // block-diagonal pass with big contiguous blocks on the tensor cores (see DENSE in the kernel)
-template <int BN>
+template <int BN, int RB = 1>
 static int launch_tc_dense(const QuipPass* ps, const __half* in, __half* out, int M, int n, cudaStream_t s) {
-  using C = TcCfg<2, BN, true>;
+  using C = TcCfg<2, BN, true, RB>;
   PFN_encodeTiled enc = get_encode();
   CUtensorMap tmx, tma;
-  if (int e = make_act_map(&tmx, in, M, n, TC_BM)) return e;       // 128 tokens per tile (MMA M)
+  if (int e = make_act_map(&tmx, in, M, n, C::BM)) return e;       // 128 * RB tokens per tile (MMA M)
   const int p = ps->p;
   cuuint64_t dims[3] = {(cuuint64_t)p, (cuuint64_t)p, (cuuint64_t)(ps->shared ? 1 : ps->nblk)};
   cuuint64_t strides[2] = {(cuuint64_t)p * sizeof(__half), (cuuint64_t)p * p * sizeof(__half)};
@@ -452,20 +463,46 @@ static int launch_tc_dense(const QuipPass* ps, const __half* in, __half* out, in
     set_error("cuTensorMapEncodeTiled (factors) failed with CUresult %d (p=%d nblk=%d)", (int)r, p, ps->nblk);
     return QUIP_ERR_CUDA;
   }
-  auto kern = qgemm_tc_kernel<2, BN, true>;
+  auto kern = qgemm_tc_kernel<2, BN, true, RB>;
   QUIP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-  int tiles = ceil_div(p, BN) * ceil_div(M, TC_BM) * ps->nblk;
+  int tiles = ceil_div(p, BN) * ceil_div(M, C::BM) * ps->nblk;
   int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, TC_THREADS, C::SMEM, s>>>(tmx, tma, nullptr, nullptr, nullptr, nullptr, out, M, p, p, 1,
-                                         ps->nblk, ps->shared ? 1 : 0);
+  kern<<<grid, RB == 1 ? TC_THREADS : TC_THREADS_TALL, C::SMEM, s>>>(tmx, tma, nullptr, nullptr, nullptr, nullptr, out, M,
+                                                                     p, p, 1, ps->nblk, ps->shared ? 1 : 0);
   QUIP_LAUNCHED("qgemm_tc_kernel<dense>");
   return QUIP_OK;
 }
 
+// Tokens per tile of the dense pass (quip_config "dense_tile"): 0 = by shape (256 when the 256-token tiles alone fill
+// every SM and their column width is instantiated, else 128), 128 or 256 = forced.
+int g_dense_tile = 0;
+
+// Factor columns per 256-token tile: the block split into ceil(p / 184) equal tiles, rounded up to 8 columns (688 ->
+// 4 x 176).  At most 184 columns keeps the two 64-token halves' accumulators (2 x 92 per thread) within the consumers'
+// 232 registers.
+static int dense_cols(int p) { return 8 * ceil_div(p, 8 * ceil_div(p, 184)); }
+
 int pass_big_tc(const QuipPass* ps, const __half* in, __half* out, int64_t M, int n, cudaStream_t s) {
   QUIP_CHECK_ARG(!ps->strided && ps->p % 8 == 0 && n % 8 == 0, "tensor-core pass needs contiguous blocks, p %% 8 == 0");
   QUIP_CHECK_ARG((((uintptr_t)in | (uintptr_t)out | (uintptr_t)ps->factors) & 15) == 0, "tensor-core pass: unaligned pointer");
-  return launch_tc_dense<128>(ps, in, out, (int)M, n, s);
+  const int w = dense_cols(ps->p);
+  // the widths of the supported models' blocks: 96, 128, 144, 160 (one tile), 224 -> 2 x 112, 448 -> 3 x 152, 688 -> 4 x 176
+  const bool have = w == 96 || w == 112 || w == 128 || w == 144 || w == 152 || w == 160 || w == 176;
+  bool tall = g_dense_tile == 256;
+  if (g_dense_tile == 0)     // 256-token tiles halve the factor traffic from L2 per flop, but must fill every SM
+    tall = have && (int64_t)ceil_div(ps->p, w) * ceil_div(M, (int64_t)2 * TC_BM) * ps->nblk >= num_sms();
+  if (!tall) return launch_tc_dense<128>(ps, in, out, (int)M, n, s);
+  switch (w) {
+    case 96: return launch_tc_dense<96, 2>(ps, in, out, (int)M, n, s);
+    case 112: return launch_tc_dense<112, 2>(ps, in, out, (int)M, n, s);
+    case 128: return launch_tc_dense<128, 2>(ps, in, out, (int)M, n, s);
+    case 144: return launch_tc_dense<144, 2>(ps, in, out, (int)M, n, s);
+    case 152: return launch_tc_dense<152, 2>(ps, in, out, (int)M, n, s);
+    case 160: return launch_tc_dense<160, 2>(ps, in, out, (int)M, n, s);
+    case 176: return launch_tc_dense<176, 2>(ps, in, out, (int)M, n, s);
+  }
+  set_error("dense pass: no 256-token kernel for %d-column tiles (p=%d)", w, ps->p);
+  return QUIP_ERR_UNSUPPORTED;
 }
 
 // Weight rows per tile of the 2-bit kernel above 64 tokens (quip_config "tc_rows"): 0 = by shape (256 when the
