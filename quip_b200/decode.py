@@ -1435,11 +1435,13 @@ class ContinuousDecoder(PromptDecoder):
 
     # ---- per-row requests
 
-    def admit(self, row, pages, budget, settings=None, prompt=None, proc=None, cstart=-1):
+    def admit(self, row, pages, budget, settings=None, prompt=None, proc=None, cstart=-1, start=0):
         """Give row `row` a new request: its pages (host ids, mapped from slot 0 on), its budget of new tokens, when
         sampling its (temperature, top_k, top_p, seed), with processing its prompt (the start of its history) and
         (repetition_penalty, no_repeat_ngram_size, min_new_tokens), and with constraint=True its start state in the
-        table of set_constraint (-1: unconstrained).  Its prompt is then fed by mixed steps."""
+        table of set_constraint (-1: unconstrained).  Its prompt is then fed by mixed steps from position `start` on:
+        64 S when its first S pages are shared pages that another request writes (prefix cache), so that its position
+        never points into one of them."""
         tbl = torch.full((self.max_pages,), -1, dtype=torch.int32)
         tbl[:len(pages)] = torch.tensor(pages, dtype=torch.int32)
         self.page_table[row].copy_(tbl)
@@ -1447,7 +1449,7 @@ class ContinuousDecoder(PromptDecoder):
         self.done[row] = False
         self.n_gen[row] = 0
         self.budget[row] = int(budget)
-        self.positions[row] = 0
+        self.positions[row] = int(start)
         if self.sampling:
             t, k, p, s = settings
             self.temperature[row] = float(t)
@@ -1901,9 +1903,28 @@ class ContinuousSchedule:
         tokens of the rows still prefilling, taken in admission order -- a long prompt spans several steps and several
         short ones can share a step;
       * retirement (retire): the row and its pages go back to the free lists.
-    A request whose budget exceeds the pool raises ValueError here, before any work."""
+    A request whose budget exceeds the pool raises ValueError here, before any work.
 
-    def __init__(self, lens, max_new, rows, n_pages, chunk):
+    With `prompts` (the requests' token ids) the pool is a prefix cache of refcounted pages (generate(...,
+    prefix_cache=True)).  Shareable pages (shareable_pages) are keyed as plan_prefix_pages keys them (prefix_page_key)
+    in an index that lives as long as the schedule:
+      * admission: the head request matches the leading run of S indexed pages of its prompt and maps them as the first
+        S entries of its table row; it takes need - S pages of its own, registers its own shareable ones in the index at
+        once (in flight: a request admitted later can match them), and its prefill starts at position 64 S.  It is
+        admitted when a row is free and free + evictable pages cover need - S;
+      * counts: a page's count is the number of held rows that map it.  retire() decrements them; a page that reaches
+        0 stays in the index as cached if it is indexed, and goes back to the free list otherwise;
+      * readiness: an indexed page is ready once plan() has handed out its owner's prompt through the page's last slot,
+        in this step or an earlier one.  A filling row whose shared pages are not all ready gets no piece and spends none
+        of the step's chunk.  Pieces run in admission order, and each layer appends a step's keys and values before any
+        of its attention reads, so a sharer's piece may follow its owner's in the same step; the first filling row never
+        waits, so a step with filling rows always has a piece;
+      * eviction: a cached page (count 0) the head request does not match is evictable; when the free list is empty,
+        the least recently released evictable page with no indexed child (lower id on ties) leaves the index and is
+        reused.
+    `prefilled` counts the prompt tokens plan() handed out, `shared[i]` the S of request i."""
+
+    def __init__(self, lens, max_new, rows, n_pages, chunk, prompts=None):
         self.lens, self.max_new = [int(n) for n in lens], [int(m) for m in max_new]
         self.need = [-(-(n + m) // KV_PAGE) for n, m in zip(self.lens, self.max_new)]
         self.chunk = int(chunk)
@@ -1914,21 +1935,102 @@ class ContinuousSchedule:
         self.free_rows = list(range(int(rows)))
         self.free_pages = list(range(int(n_pages)))
         self.req = [None] * int(rows)                # the request each row holds
-        self.pages = [[] for _ in range(int(rows))]
+        self.pages = [[] for _ in range(int(rows))]  # its table row: shared pages first
         self.fed = [0] * int(rows)                   # prompt tokens fed
         self.filling = []                            # rows still prefilling, in admission order
+        self.prefilled = 0
+        self.shared = [0] * len(self.lens)
+        self.tokens = None
+        if prompts is None:
+            return
+        self.tokens = [torch.as_tensor(p).reshape(-1).tolist() for p in prompts]
+        if [len(t) for t in self.tokens] != self.lens:
+            raise ValueError('prompts must have the lengths in lens')
+        n_pages = int(n_pages)
+        self.ref = [0] * n_pages                     # rows mapping each page
+        self.index = {}                              # prefix_page_key -> page
+        self.entry = {}                              # indexed page -> (its key, its node, parent page or -1)
+        self.kids = [0] * n_pages                    # indexed pages keyed under each page's node
+        self.cached = set()                          # indexed pages of count 0
+        self.released = [0] * n_pages                # retire() call that cached each page
+        self.ready = set()                           # indexed pages whose owner's prompt has been handed out over them
+        self.wait = [[] for _ in range(int(rows))]   # each row's shared pages not yet seen ready
+        self.pending = [[] for _ in range(int(rows))]  # each row's own indexed pages: (end slot, page), not yet ready
+        self._nodes = self._retired = 0
+
+    def _match(self, i):
+        """The indexed pages that lead request i's prompt."""
+        t, node, out = self.tokens[i], 0, []
+        for p in range(shareable_pages(len(t))):
+            page = self.index.get(prefix_page_key(node, t, p))
+            if page is None:
+                break
+            out.append(page)
+            node = self.entry[page][1]
+        return out
+
+    def _take(self):
+        """A page for an admitted row: the lowest free one, else the evicted one."""
+        if self.free_pages:
+            return heapq.heappop(self.free_pages)
+        p = min((self.released[q], q) for q in self.cached if not self.kids[q])[1]
+        self.cached.discard(p)
+        self.ready.discard(p)
+        key, _, parent = self.entry.pop(p)
+        del self.index[key]
+        if parent >= 0:
+            self.kids[parent] -= 1
+        return p
 
     def admit(self):
-        """Admit what the policy allows now: [(row, request, pages)]."""
+        """Admit what the policy allows now: [(row, request, pages)], pages the row's table from slot 0 on."""
         out = []
-        while self.queue and self.free_rows and len(self.free_pages) >= self.need[self.queue[0]]:
-            i = self.queue.popleft()
-            r = heapq.heappop(self.free_rows)
-            pages = [heapq.heappop(self.free_pages) for _ in range(self.need[i])]
-            self.req[r], self.pages[r], self.fed[r] = i, pages, 0
+        while self.queue and self.free_rows:
+            i = self.queue[0]
+            if self.tokens is None:
+                if len(self.free_pages) < self.need[i]:
+                    break
+                pages = [heapq.heappop(self.free_pages) for _ in range(self.need[i])]
+                r = heapq.heappop(self.free_rows)
+            else:
+                shared = self._match(i)
+                evictable = len(self.cached) - sum(p in self.cached for p in shared)
+                if len(self.free_pages) + evictable < self.need[i] - len(shared):
+                    break
+                r = heapq.heappop(self.free_rows)
+                pages = self._map(r, i, shared)
+            self.queue.popleft()
+            self.req[r], self.pages[r], self.fed[r] = i, pages, KV_PAGE * self.shared[i]
             self.filling.append(r)
             out.append((r, i, pages))
         return out
+
+    def _map(self, r, i, shared):
+        """Row r's table for request i: the matched pages, then its own, whose shareable ones it registers."""
+        for p in shared:
+            self.ref[p] += 1
+            self.cached.discard(p)
+        S = len(shared)
+        pages = shared + [self._take() for _ in range(self.need[i] - S)]
+        for p in pages[S:]:
+            self.ref[p] = 1
+        parent = shared[-1] if shared else -1
+        node = self.entry[parent][1] if shared else 0
+        pend = []
+        for p in range(S, shareable_pages(self.lens[i])):
+            key = prefix_page_key(node, self.tokens[i], p)
+            self._nodes += 1
+            node = self._nodes
+            self.index[key] = pages[p]
+            self.entry[pages[p]] = (key, node, parent)
+            if parent >= 0:
+                self.kids[parent] += 1
+            parent = pages[p]
+            pend.append((KV_PAGE * (p + 1), pages[p]))
+        self.shared[i] = S
+        self.wait[r] = [p for p in shared if p not in self.ready]
+        self.pending[r] = pend
+        return pages
 
     def plan(self):
         """The next step: (decoding rows, pieces), a piece (row, first prompt position, count); the pieces count as fed.
@@ -1938,18 +2040,40 @@ class ContinuousSchedule:
         for r in self.filling:
             if not left:
                 break
+            if self.tokens is not None:
+                self.wait[r] = [p for p in self.wait[r] if p not in self.ready]
+                if self.wait[r]:
+                    continue
             n = min(self.lens[self.req[r]] - self.fed[r], left)
             pieces.append((r, self.fed[r], n))
             self.fed[r] += n
+            self.prefilled += n
             left -= n
+            if self.tokens is not None:
+                pend = self.pending[r]
+                while pend and pend[0][0] <= self.fed[r]:
+                    self.ready.add(pend.pop(0)[1])
         self.filling = [r for r in self.filling if self.fed[r] < self.lens[self.req[r]]]
         return decoding, pieces
 
     def retire(self, r):
         """Free row r and its pages; returns the request it held."""
         i = self.req[r]
-        for p in self.pages[r]:
-            heapq.heappush(self.free_pages, p)
+        if self.tokens is None:
+            for p in self.pages[r]:
+                heapq.heappush(self.free_pages, p)
+        else:
+            self._retired += 1
+            for p in self.pages[r]:
+                self.ref[p] -= 1
+                if self.ref[p]:
+                    continue
+                if p in self.entry:
+                    self.cached.add(p)
+                    self.released[p] = self._retired
+                else:
+                    heapq.heappush(self.free_pages, p)
+            self.wait[r], self.pending[r] = [], []
         heapq.heappush(self.free_rows, r)
         self.req[r], self.pages[r] = None, []
         return i
@@ -1960,14 +2084,15 @@ class ContinuousSchedule:
 
 
 def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows, kv_pages, chunk, max_len,
-                         proc=None, logprobs=None, top_logprobs=0, constraint=None):
+                         proc=None, logprobs=None, top_logprobs=0, constraint=None, prefix_cache=False):
     """generate()'s continuous path: ContinuousSchedule over a ContinuousDecoder of `rows` rows and `kv_pages` pages;
     proc: the per-prompt (penalties, ngram sizes, min_new_tokens) and the bad words of the logits processors, or None;
     constraint: the packed token automata and each prompt's start state (constrain.pack_automata), or None;
-    logprobs: generate()'s dict, or None.  A request's logprob entries are read with its tokens, before its row takes
-    the next prompt (admission resets n_gen, and the next request writes the same columns)."""
+    logprobs: generate()'s dict, or None; prefix_cache: the schedule shares prompt pages (ContinuousSchedule(prompts=)).
+    A request's logprob entries are read with its tokens, before its row takes the next prompt (admission resets n_gen,
+    and the next request writes the same columns)."""
     lens = [p.numel() for p in prompts]
-    sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk)
+    sched = ContinuousSchedule(lens, max_new, rows, kv_pages, chunk, prompts=prompts if prefix_cache else None)
     dec = ContinuousDecoder(model, max_len, rows, kv_pages, max(max_new), kv_dtype=kv_dtype,
                             sampling=settings is not None, eos=eos, processing=proc is not None,
                             logprobs=None if logprobs is None else top_logprobs, constraint=constraint is not None)
@@ -2003,7 +2128,7 @@ def _generate_continuous(model, prompts, max_new, eos, kv_dtype, settings, rows,
             for r, i, pages in sched.admit():
                 dec.admit(r, pages, max_new[i], None if settings is None else [s[i] for s in settings],
                           prompts[i], None if proc is None else [s[i] for s in proc[:3]],
-                          -1 if constraint is None else constraint[3][i])
+                          -1 if constraint is None else constraint[3][i], start=KV_PAGE * sched.shared[i])
         if sched.finished:
             break
         decoding, pieces = sched.plan()
@@ -2292,6 +2417,19 @@ def _sample_torch(logits, temperature, top_k, top_p, seed, t):
 EOS_CHECK_EVERY = 16
 
 
+def shareable_pages(n):
+    """How many leading pages of an n-token prompt other prompts may share: page p (slots 64p .. 64p + 63) when
+    64 (p + 1) <= n - 1 -- it is full, and the last prompt token, whose logits start generation, is never on it, nor
+    is any slot decode writes."""
+    return max(int(n) - 1, 0) // KV_PAGE
+
+
+def prefix_page_key(node, tokens, p):
+    """The key of page p of a prompt (a list of ids) whose pages 0 .. p - 1 lead to prefix node `node` (0: the empty
+    prefix): prompts share page p exactly when their tokens 0 .. 64 (p + 1) - 1 agree."""
+    return node, tuple(tokens[KV_PAGE * p:KV_PAGE * (p + 1)])
+
+
 def plan_prefix_pages(prompts, budgets, max_pages=None):
     """Page table of a paged KV cache whose rows share their common prompt prefixes.
 
@@ -2319,8 +2457,8 @@ def plan_prefix_pages(prompts, budgets, max_pages=None):
     for r, t in enumerate(toks):
         node, shared = 0, 0
         for p in range(need[r]):
-            if KV_PAGE * (p + 1) <= len(t) - 1:      # shareable; once a page is the row's own, no later one is shared
-                key = (node, tuple(t[KV_PAGE * p:KV_PAGE * (p + 1)]))
+            if p < shareable_pages(len(t)):          # once a page is the row's own, no later one is shared
+                key = prefix_page_key(node, t, p)
                 if key in owner:
                     node, page = owner[key]
                     table[r, p] = page
@@ -2380,7 +2518,8 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
              spec_stats=None, prefill_chunk_size=None, share_prompt_prefixes=False, num_return_sequences=1,
              max_batch_size=None, kv_pages=None, num_beams=1, length_penalty=1.0, early_stopping=False,
              beam_stats=None, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, bad_words_ids=None,
-             logprobs=None, top_logprobs=0, token_constraint=None, assistant_model=None, num_assistant_tokens=None):
+             logprobs=None, top_logprobs=0, token_constraint=None, assistant_model=None, num_assistant_tokens=None,
+             prefix_cache=False):
     """Continuations of a batch of prompts (1-D id tensors, any lengths) of a Llama or OPT model: one tensor of new token
     ids per prompt, cut after its first `eos_token_id` (an id or a list of ids).  The prompts are prefilled in one
     many-token forward; each new token is one replay of a captured PromptDecoder step on CUDA (eager on the CPU).
@@ -2444,8 +2583,17 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
         none waits; a done row's pages go back to the pool and its row to the next prompt.
     Each prompt's tokens are those of generate([p], prefill_chunk_size=C) run alone with its own settings (an int seed
     gives prompt i the seed seed + i), up to the arithmetic of other GEMM token counts.  prompt_lookup_num_tokens,
-    share_prompt_prefixes and num_return_sequences > 1 do not combine with max_batch_size (sharing pages between live
-    requests would need refcounted pages).
+    share_prompt_prefixes and num_return_sequences > 1 do not combine with max_batch_size.
+
+    prefix_cache=True (with max_batch_size; default False: every request prefills its whole prompt into pages of its
+    own) makes the page pool a prefix cache of refcounted pages for the length of the call (ContinuousSchedule with
+    prompts): a request maps the full prompt pages before its last prompt token that an earlier request -- running or
+    finished -- already holds for the same leading tokens (plan_prefix_pages' rule), prefills only the rest, and waits
+    to be fed until those pages are written.  A finished request's indexed pages stay cached until the pool needs them
+    (least recently released first).  For several samples of one prompt, repeat it in the list: its full prompt pages
+    are prefilled once.  It combines with everything max_batch_size takes (sampling, the processors, token_constraint,
+    logprobs, kv_dtype, kv_pages), and each request's tokens stay those of the prompt run alone, up to the arithmetic
+    of other GEMM token counts.  A value that is not a bool, or True without max_batch_size, raises ValueError.
 
     num_beams=K (2 .. 16; default 1: the paths above, unchanged) runs beam search (BeamDecoder): for each prompt p the
     result is what HF's model.generate(p[None], num_beams=K, do_sample=False, max_new_tokens=n_p, length_penalty,
@@ -2501,6 +2649,11 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
     if top_logprobs and logprobs is None:
         raise ValueError('top_logprobs needs a logprobs dict to receive the results')
     n_lp = None if logprobs is None else int(top_logprobs)
+    if not isinstance(prefix_cache, bool):
+        raise ValueError(f'prefix_cache must be True or False, got {prefix_cache!r}')
+    if prefix_cache and max_batch_size is None:
+        raise ValueError('prefix_cache shares pages between the requests of continuous batching: it needs '
+                         'max_batch_size')
     prefill_chunk_size = _chunk_size(prefill_chunk_size)
     n_ret = num_return_sequences
     if isinstance(n_ret, bool) or int(n_ret) != n_ret or n_ret < 1:
@@ -2620,7 +2773,7 @@ def generate(model, prompts, max_new_tokens, max_len=None, eos_token_id=None, kv
             raise ValueError(f'kv_pages must be an integer >= 1, got {kv_pages!r}')
         return _generate_continuous(model, prompts, budgets, eos, kv_dtype, settings if do_sample else None, rows,
                                     int(kv_pages), 512 if prefill_chunk_size is None else prefill_chunk_size, max_len,
-                                    proc, logprobs, int(top_logprobs), constraint)
+                                    proc, logprobs, int(top_logprobs), constraint, prefix_cache)
     pages, starts = {}, None
     if share:
         table, n_pages, starts = plan_prefix_pages(prompts, [n + m + k for n, m in zip(lens, budgets)],

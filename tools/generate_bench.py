@@ -55,6 +55,14 @@ counted from shapes), mean and p99 time between a request's tokens, the time in 
 time per mixed step, and how many requests' tokens agree exactly.  Also ragged against padded chunked prefill alone on
 8 prompts of 64 .. 2048 tokens.
 
+Section prefix (llama7b) measures the prefix cache of continuous batching (generate(..., max_batch_size=32,
+prefix_cache=True)): 256 requests, each one of 8 shared 1024-token preambles plus a unique tail of 32 .. 512 tokens,
+budgets 16 .. 256 (fixed seed), fp16 cache, greedy, no EOS, and a variant of 32 such prompts each repeated 8 times.  The
+cache-off and cache-on arms run the instrumented continuous loop of section continuous (32 rows, chunks of 512) one after
+the other in the same process.  Reported per arm: output tokens/s and wall time, the prompt tokens the schedule fed,
+the time in mixed and in graph steps, mean and p99 time between a request's tokens; and how many requests' tokens agree
+exactly between the arms.
+
 Section logits (llama7b) measures the logits processors (quip_logits_process, csrc/logits_process.cu): the kernel alone
 at B in {1, 32, 128}, V in {32000, 128256} and histories of 512 and 4096 tokens with every processor on (n-gram size 3,
 16 bad words), and the captured PromptDecoder step with and without processors at B in {1, 32}, 512-token prompts and
@@ -844,16 +852,18 @@ def continuous_static(model, prompts, budgets, rows, chunk):
     return time.perf_counter() - t0, outs, gemm
 
 
-def continuous_serve(model, prompts, budgets, rows, chunk):
+def continuous_serve(model, prompts, budgets, rows, chunk, prefix_cache=False, stats=None):
     """generate()'s continuous loop (decode._generate_continuous), with a CUDA event after every step: seconds, outputs,
-    per-step (kind, device ms, host ms, prompt tokens, decode tokens) and each request's token times."""
+    per-step (kind, device ms, host ms, prompt tokens, decode tokens) and each request's token times.  prefix_cache:
+    the schedule shares prompt pages (generate(..., prefix_cache=True)); stats: a dict that receives the schedule's
+    prefilled prompt tokens and shared pages per request."""
     import time
     from quip_b200.decode import EOS_CHECK_EVERY, KV_PAGE, ContinuousDecoder, ContinuousSchedule
     lens = [p.numel() for p in prompts]
     need = max(-(-(n + m) // KV_PAGE) for n, m in zip(lens, budgets))
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    sched = ContinuousSchedule(lens, budgets, rows, rows * need, chunk)
+    sched = ContinuousSchedule(lens, budgets, rows, rows * need, chunk, prompts=prompts if prefix_cache else None)
     dec = ContinuousDecoder(model, max(n + m for n, m in zip(lens, budgets)), rows, rows * need, max(budgets))
     dec.capture()
     out = [None] * len(prompts)
@@ -869,7 +879,7 @@ def continuous_serve(model, prompts, budgets, rows, chunk):
                         out[sched.retire(r)] = dec.generated[r, :int(dec.n_gen[r])].cpu()
                         dec.retire(r)
                 for r, i, pages in sched.admit():
-                    dec.admit(r, pages, budgets[i])
+                    dec.admit(r, pages, budgets[i], start=KV_PAGE * sched.shared[i])
             if sched.finished:
                 break
             decoding, pieces = sched.plan()
@@ -899,9 +909,45 @@ def continuous_serve(model, prompts, budgets, rows, chunk):
         for i in made:
             if len(times[i]) < out[i].numel():               # a request's first n tokens come from its first n steps
                 times[i].append(t)
+    if stats is not None:
+        stats.update(prefilled=sched.prefilled, shared=list(sched.shared))
     del dec
     torch.cuda.empty_cache()
     return secs, out, log, times, split
+
+
+def prefix_workload(V, copies=1, n=256, heads=8, head_len=1024, seed=0):
+    """n requests: `heads` shared preambles of head_len tokens, each prompt one of them plus a unique tail of 32 .. 512
+    tokens, budgets 16 .. 256; with copies > 1, n / copies such prompts each repeated `copies` times in a row."""
+    g = torch.Generator().manual_seed(seed)
+    pre = [torch.randint(0, V, (head_len,), generator=g) for _ in range(heads)]
+    m = n // copies
+    which = torch.randint(0, heads, (m,), generator=g).tolist()
+    tails = torch.randint(32, 513, (m,), generator=g).tolist()
+    prompts = [torch.cat((pre[h], torch.randint(0, V, (t,), generator=g))) for h, t in zip(which, tails)]
+    budgets = torch.randint(16, 257, (m,), generator=g).tolist()
+    return [p for p in prompts for _ in range(copies)], [b for b in budgets for _ in range(copies)]
+
+
+def prefix_arms(model, prompts, budgets, rows=32, chunk=512):
+    """continuous_serve with the prefix cache off, then on: per arm seconds, output tokens/s, prefilled prompt tokens,
+    graph and mixed time, token gaps; and how many requests' tokens agree between the arms."""
+    import numpy as np
+    res, outs = {}, {}
+    for arm, on in (('off', False), ('on', True)):
+        st = {}
+        secs, out, log, times, split = continuous_serve(model, prompts, budgets, rows, chunk, prefix_cache=on, stats=st)
+        gaps = np.concatenate([np.diff(t) for t in times.values() if len(t) > 1])
+        n_out = sum(o.numel() for o in out)
+        res[arm] = dict(seconds=secs, tokens_per_s=n_out / secs, output_tokens=n_out, prefilled=st['prefilled'],
+                        prompt_tokens=sum(p.numel() for p in prompts), shared_pages=sum(st['shared']),
+                        graph_ms=split['graph'][0], graph_steps=split['graph'][1], mixed_ms=split['mixed'][0],
+                        mixed_steps=split['mixed'][1], token_gap_ms_mean=float(gaps.mean()),
+                        token_gap_ms_p99=float(np.percentile(gaps, 99)))
+        outs[arm] = out
+    res['same_requests'] = sum(torch.equal(a, b) for a, b in zip(outs['off'], outs['on']))
+    res['requests'] = len(prompts)
+    return res
 
 
 def ragged_vs_padded_prefill(model, V, chunk=512, reps=3, seed=1):
@@ -1231,7 +1277,7 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--kernel-reps', type=int, default=100)
     ap.add_argument('--sections', default='kernel,prefill,decode,fp8')    # also: fp8kernel, sample, spec, chunked, paged,
-    #                                                                         score, continuous, beam, logits,
+    #                                                                         score, continuous, prefix, beam, logits,
     #                                                                         logprobs, assisted
     ap.add_argument('--score-docs', type=int, default=512, help='documents of 4 choices in the score section')
     a = ap.parse_args()
@@ -1353,7 +1399,7 @@ def main():
                     print(f'logprobs kernel R={R} V=32000 n={n}: {1e3 * r["kernel_ms"]:.1f} us '
                           f'({r["bytes_per_s"] / 1e12:.2f} TB/s of logits)', flush=True)
         if not sections & {'prefill', 'decode', 'fp8', 'sample', 'spec', 'assisted'} and not (
-                sections & {'chunked', 'paged', 'score', 'continuous', 'beam', 'logits', 'logprobs'} and
+                sections & {'chunked', 'paged', 'score', 'continuous', 'prefix', 'beam', 'logits', 'logprobs'} and
                 name == 'llama7b'):
             continue
         model = build_synthetic_model(cfg, torch.device('cuda:0'), bits=2, seed=0, seqlen=4096)
@@ -1433,6 +1479,20 @@ def main():
                   f'({c["graph_steps"]} steps), mixed {c["mixed_ms"] / 1e3:.1f} s ({c["mixed_steps"]} steps, host '
                   f'{c["mixed_host_ms_mean"]:.1f} ms each); identical requests {same} / {len(prompts)}, mean agreeing '
                   f'prefix {np.mean(agree):.1f} tokens', flush=True)
+        if 'prefix' in sections and name == 'llama7b':
+            rec['prefix'] = {}
+            for case, copies in (('preambles', 1), ('preambles_x8', 8)):
+                prompts, budgets = prefix_workload(cfg.vocab_size, copies)
+                r = prefix_arms(model, prompts, budgets)
+                rec['prefix'][case] = r
+                for arm in ('off', 'on'):
+                    x = r[arm]
+                    print(f'{name} prefix {case} cache {arm}: {x["tokens_per_s"]:.0f} tok/s ({x["seconds"]:.1f} s), '
+                          f'prefilled {x["prefilled"]} of {x["prompt_tokens"]} prompt tokens, graph '
+                          f'{x["graph_ms"] / 1e3:.1f} s ({x["graph_steps"]} steps), mixed {x["mixed_ms"] / 1e3:.1f} s '
+                          f'({x["mixed_steps"]} steps), token gap mean {x["token_gap_ms_mean"]:.1f} ms p99 '
+                          f'{x["token_gap_ms_p99"]:.1f} ms', flush=True)
+                print(f'{name} prefix {case}: identical requests {r["same_requests"]} / {r["requests"]}', flush=True)
         if 'beam' in sections and name == 'llama7b':
             rec['beam'] = []
             for fp8 in (False, True):
